@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — EM iterations/s of the GMM-EM hot path on B200 (BASELINE.json metric).
+"""bench.py — EM iterations/s of the GMM-EM hot path on H100 (BASELINE.json metric).
 
   python bench.py --gpus N --steps K --warmup W            (N=1)
   python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...   (N>1)
@@ -12,20 +12,26 @@ DxD inversions + constants + E-step operand (one device kernel; option "finalize
 (N=10M, D=24, K=64; config 4 shards the same 10M events over N GPUs = strong
 scaling).  `value` is measured with the events resident in HBM: a block of exactly
 K steps is timed (barrier + synchronize on both sides, device clock, max over
-ranks); the block is repeated `--repeats` times and the MEDIAN block is reported
-(`blocks_ms_per_step` lists all of them).  `e2e` is measured through the C ABI from
+ranks); with `--repeats R` (default 1) R such blocks are timed and the MEDIAN block
+is reported (`blocks_ms_per_step` lists all of them).  `e2e` is measured through the C ABI from
 HOST buffers (pinned events H2D, parameters H2D, initial E-step, the K steps,
 parameters + log-likelihood D2H all inside the timed region: one upload per K steps).
 
 Also on the line: `roofline` (E-step, HBM), `roofline_mstep` (tensor, against the measured
-dense BF16/FP16 peak — the pipe the kernel's kind::f16 MMAs run on), `cpu_baseline` (the
+dense BF16/FP16 peak — the pipe the kernel's f16 wgmma run on), `cpu_baseline` (the
 sequential-EM CPU port on the host cores, median of 3), `reference_gpu` (the UNMODIFIED
-reference program compiled for sm_100a, oracle/_ref/gaussianMPI_ref_perf, run on this GPU at
+reference program compiled for sm_90a, oracle/_ref/gaussianMPI_ref_perf, run on this GPU at
 config 2 and config 3) and `config5` (the model-order-reduction loop K=128 -> 16, gmm_fit).
 
 `--impl reference` times the reference's algorithm on the host cores (the
 sequential-EM CPU port in oracle/, FP32, OpenMP over the physical cores) on a bounded
 slice of the same workload.
+
+`--dump-outputs DIR` writes, after the timed blocks, what the last timed step computed as
+DIR/<name>.npy (rank 0's shard): the parameters of every cluster (N, pi, constant, means,
+R, Rinv; float32), the log-likelihood (float64) and the responsibilities of a fixed, seeded
+sample of 100,000 events (memberships_sample [K][100000], float32, with the event indices
+in memberships_index).  The inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -58,7 +64,8 @@ def measured_peaks():
         d = json.load(open(p))
         return dict(hbm_gbs=float(d["hbm_gbs"]), bf16_tflops=float(d["bf16_tflops"]),
                     bf16_tflops_sustained=float(d.get("bf16_tflops_sustained", d["bf16_tflops"])), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16/FP16 — not reached, and less on a power-limited card
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="datasheet")
 
 
 class ClockSampler:
@@ -211,7 +218,7 @@ def run_cpu_baseline(workload, sample_events, steps, warmup, repeats):
 def run_reference_gpu(pkg, workload, device, iters=3):
     exe = os.path.join(ROOT, "oracle", "_ref", "gaussianMPI_ref_perf")
     if not os.path.exists(exe):
-        return dict(unavailable="oracle/_ref/gaussianMPI_ref_perf not built (needs /root/reference at build time)")
+        return dict(unavailable="oracle/_ref/gaussianMPI_ref_perf not built (needs the reference sources at build time)")
     wl = WORKLOADS[workload]
     N, D, K = wl["N"], wl["D"], wl["K"]
     with tempfile.TemporaryDirectory(prefix="gmmref_") as td:
@@ -241,8 +248,24 @@ def run_reference_gpu(pkg, workload, device, iters=3):
     return dict(value=1.0 / allin, unit="it/s", kernels_only_its=1.0 / kern, iterations=iters,
                 seconds_per_iteration=dict(estep=prof["E-step Kernel"][2], mstep=prof["M-step Kernel"][2], constants=prof["Consts Kernel"][2],
                                            memcpy_cpu_mpi=sum(extra.values()) / max(1, iters)),
-                how=f"unmodified gaussian.cu/gaussian_kernel.cu compiled -arch=sm_100a with cutil.h/mpi.h shims (oracle/Makefile ref), shipped "
+                how=f"unmodified gaussian.cu/gaussian_kernel.cu compiled -arch=sm_90a with cutil.h/mpi.h shims (oracle/Makefile ref), shipped "
                     f"ENABLE_OUTPUT 0, MIN=MAX_ITERS={iters}, 1 GPU, {workload}: N={N} D={D} K={K}; its own profile_t timers (gaussian.cu:967)")
+
+
+DUMP_SAMPLE = 100_000      # events whose responsibilities --dump-outputs keeps (K x 100k floats: 25.6 MB at K = 64)
+
+
+def dump_outputs(out_dir, eng, K, n_local, ll):
+    """What the timed path returned after its last step: the parameters of the K clusters, the log-likelihood and the
+    responsibilities of a fixed, seeded sample of the events (the full K x N array is 2.56 GB at c3)."""
+    os.makedirs(out_dir, exist_ok=True)
+    res = eng.get_clusters(K, with_memberships=True)
+    for name in ("N", "pi", "constant", "means", "R", "Rinv"):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(getattr(res, name)[:K], dtype=np.float32))
+    np.save(os.path.join(out_dir, "loglik.npy"), np.array([ll], dtype=np.float64))
+    idx = np.sort(np.random.default_rng(12345).choice(n_local, size=min(DUMP_SAMPLE, n_local), replace=False))
+    np.save(os.path.join(out_dir, "memberships_index.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "memberships_sample.npy"), np.ascontiguousarray(res.memberships[:K][:, idx], dtype=np.float32))
 
 
 def main():
@@ -250,14 +273,16 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--repeats", type=int, default=5, help="timed blocks of --steps iterations; the median block is reported")
+    ap.add_argument("--repeats", type=int, default=1, help="timed blocks of --steps iterations; the median block is reported")
     ap.add_argument("--impl", default="b200", choices=["b200", "reference", "cpu-worker"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (parameters, log-likelihood, sampled responsibilities)")
     ap.add_argument("--workload", default=os.environ.get("GMM_BENCH_WORKLOAD", "c3"), choices=list(WORKLOADS))
     ap.add_argument("--path", default=os.environ.get("GMM_BENCH_PATH", "auto"), choices=["auto", "simt", "tensor"])
     ap.add_argument("--scaling", default="strong", choices=["strong", "weak"])
     ap.add_argument("--cpu-sample", type=int, default=1_000_000, help="events in the cpu_baseline slice (0 = skip)")
     ap.add_argument("--no-e2e", action="store_true")
-    ap.add_argument("--no-ref-gpu", action="store_true", help="skip the reference-on-B200 runs (config 2 and 3)")
+    ap.add_argument("--no-ref-gpu", action="store_true", help="skip the runs of the reference program on this GPU (config 2 and 3)")
     ap.add_argument("--c5-iters", type=int, default=int(os.environ.get("GMM_BENCH_C5_ITERS", "2")),
                     help="EM iterations per model order of the config-5 measurement (0 = skip)")
     args = ap.parse_args()
@@ -289,7 +314,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ---------------- B200 arm --------------------------------------------------
+    # ---------------- GPU arm ---------------------------------------------------
     import torch
     import torch.distributed as dist
     if world > 1:
@@ -373,6 +398,8 @@ def main():
     dt_wall = float(np.median(walls))
     prof = eng.profile()
     value = args.steps / dt
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng, K, count, ll)
 
     # ---- end to end from host buffers: e2e ----
     e2e = None
@@ -420,9 +447,9 @@ def main():
     n_tensor, n_simt = int(prof.get("mstep_tensor_launches", 0)), int(prof.get("mstep_simt_launches", 0))
     F = 1 + D + D * (D + 1) // 2
     mt_rows = (F + 127) // 128 * 128
-    # executed MMA flops per launch of mstep_tc_kernel: per 16 events and feature tile one M=128,N=128 (ph x [gh;gl]) and one
-    # M=128,N=64 (pl x gh) MMA = 3 products of the padded (mt_rows x 64-cluster) tile
-    exec_flops = 2.0 * count * mt_rows * ((K + 63) // 64 * 64) * 3 if n_tensor else 0.0
+    # executed MMA flops per launch of mstep_tc_kernel: per 16 events and feature tile one N=64 (ph x [gh;gl]) and one
+    # N=32 (pl x gs) wgmma per 32 clusters = 3 products of the padded (mt_rows x 32-cluster) tile
+    exec_flops = 2.0 * count * mt_rows * ((K + 31) // 32 * 32) * 3 if n_tensor else 0.0
     traffic = traffic_m = None
     tpath = os.path.join(ROOT, "profiles", "ncu_traffic.json")
     if os.path.exists(tpath) and world == 1:
@@ -435,11 +462,11 @@ def main():
                     ms_per_launch=estep_ms, algorithmic_bytes_per_launch=e_bytes)
     roofline_mstep = dict(kernel="mstep_covariance", bound="tensor", achieved=m_tfs, peak=peaks["bf16_tflops_sustained"], unit="TFLOP/s",
                           frac=m_tfs / peaks["bf16_tflops_sustained"], traffic=traffic_m,
-                          peak_source=peaks["source"] + " dense bf16/fp16 sustained (the kernel issues kind::f16 MMAs)",
+                          peak_source=peaks["source"] + " dense bf16/fp16 (the kernel issues f16 wgmma)",
                           ms_per_launch=mstep_ms, algorithmic_flops_per_launch=m_flops,
                           executed_mma_flops_per_launch=exec_flops, executed_tflops=exec_flops / (mstep_ms * 1e-3) / 1e12 if mstep_ms > 0 else 0.0,
                           kernels=dict(mstep_tc_kernel_launches=n_tensor, mstep_simt_kernel_launches=n_simt,
-                                      note="launch counts in the timed region; mstep_tc_kernel = fixed-point leading parts (exact TMEM "
+                                      note="launch counts in the timed region; mstep_tc_kernel = fixed-point leading parts (exact tensor-core "
                                            "accumulation) + FP16 remainders, three products per element"))
 
     # ---- config 5: model-order reduction K0=128 -> 16 (gmm_fit) on the same GPUs ----
@@ -485,10 +512,10 @@ def main():
                 ms_per_step=dt * 1e3 / args.steps, higher_is_better=True, scaling=args.scaling, vs_baseline=None,
                 dtype="f32", data="synthetic",
                 config=dict(workload=f"{args.workload}: N={N} D={D} K={K} Gaussian blobs (seed {pkg.synth.SEED}), "
-                                     f"{count} events on rank 0", path=args.path, l2="inputs (X 0.96 GB + memberships 2.56 GB at c3) exceed the 126 MB L2",
+                                     f"{count} events on rank 0", path=args.path, l2="inputs (X 0.96 GB + memberships 2.56 GB at c3) exceed the 50 MB L2",
                             parallelism=f"dp{world} (events sharded, one all-reduce of {8 * (K * (1 + D + D * (D + 1) // 2) + 1)} B per step)",
                             finalisation=("device (finalize_params_kernel, timed under 'upload')" if dev_fin else "host"),
-                            arithmetic=("fp32 data and results; tensor path: fp16 hi/lo split operands, fp32 TMEM accumulation, fp64 "
+                            arithmetic=("fp32 data and results; tensor path: fp16 hi/lo split operands, fp32 register accumulation, fp64 "
                                         "statistics reduction and finalisation" if args.path != "simt" else
                                         "fp32 E-step, fp64 M-step statistics and host finalisation"),
                             timing=f"median of {len(blocks)} timed blocks of {args.steps} steps each"),

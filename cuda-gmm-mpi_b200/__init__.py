@@ -1,4 +1,4 @@
-"""cuda-gmm-mpi_b200 — B200-native GMM-EM engine (drop-in for the EM hot path of
+"""cuda-gmm-mpi_b200 — H100-native GMM-EM engine (drop-in for the EM hot path of
 Corv/CUDA-GMM-MPI).  The product is the C-ABI shared library
 ``libgmm_b200.so`` (include/gmm.h) built from ``csrc/``; this package is the
 thin ctypes mirror used by the tests, bench.py and __graft_entry__.py.

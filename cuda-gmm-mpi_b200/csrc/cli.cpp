@@ -10,7 +10,7 @@
 //   GMM_GPUS    number of GPUs to use (default: all visible)
 //   GMM_OUTPUT  1 = write .summary/.results content (ENABLE_OUTPUT), default 1
 //   GMM_PRINT   1 = ENABLE_PRINT messages, default 0
-//   GMM_PATH    0 auto, 1 SIMT kernels, 2 tcgen05 kernels
+//   GMM_PATH    0 auto, 1 SIMT kernels, 2 wgmma kernels
 #include <cuda_runtime.h>
 #include <fcntl.h>
 #include <sys/mman.h>
@@ -144,7 +144,7 @@ extern "C" int gmm_main(int argc, char** argv) {
     std::vector<std::vector<double>> prof(G, std::vector<double>(8, 0.0));
 
     // Every context is created (and checked) BEFORE any thread enters the communicator bootstrap: ncclCommInitRank
-    // needs all G ranks, so a rank that failed earlier (no sm_100 device, out of memory, bad GMM_PATH) would leave
+    // needs all G ranks, so a rank that failed earlier (no sm_90 device, out of memory, bad GMM_PATH) would leave
     // the others blocked for ever; the reference exits the whole process on a CUDA failure (CUDA_SAFE_CALL).
     OneShotBarrier created(G);
     std::atomic<int> setup_failed{0};

@@ -276,7 +276,7 @@ struct gmm_ctx {
     int device = 0, n = 0, D = 0, Kmax = 0, F = 0;
     long long n_global = 0, offset = 0;
     cudaStream_t stream = nullptr;
-    int num_sms = 148;
+    int num_sms = 132;
     // events
     float* d_x_aos = nullptr;    // [n][D]  as supplied (TMA source of the tensor path)
     float* d_x_soa = nullptr;    // [D][n]  transpose for the SIMT kernels
@@ -401,7 +401,7 @@ static bool use_tensor_mstep(const gmm_ctx* c, int K) {
 // GMM_PATH_TENSOR never degrades silently: the M-step (the covariance contraction) must be covered.
 static int check_path(const gmm_ctx* c, int K) {
     if (mstep_path_of(c) == GMM_PATH_TENSOR && !tc_mstep_supported(c->D, K))
-        return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the tcgen05 kernels do not cover this (D, K)");
+        return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the wgmma kernels do not cover this (D, K)");
     if (mstep_path_of(c) == GMM_PATH_TENSOR && c->n > 0 && c->have_shift && !tc_mstep_ready(c->tc))
         return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the data range (outliers beyond 64 standard deviations) exceeds the "
                                  "tensor M-step's fixed-point operand budget");
@@ -665,7 +665,7 @@ extern "C" {
 static int peer_exchange_setup(gmm_ctx* c);
 static void peer_exchange_destroy(gmm_ctx* c);
 
-const char* gmm_version(void) { return "cuda-gmm-mpi_b200 0.1 (sm_100a)"; }
+const char* gmm_version(void) { return "cuda-gmm-mpi_b200 0.1 (sm_90a)"; }
 
 int gmm_create(gmm_ctx** out, int device, int n_local, int D, int Kmax, const float* events_aos,
                long long n_global, long long offset) {
@@ -683,8 +683,8 @@ int gmm_create(gmm_ctx** out, int device, int n_local, int D, int Kmax, const fl
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10)
-        return fail(GMM_ERR_CUDA, std::string("device '") + prop.name + "' is not sm_100 (B200); kernels are built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0)
+        return fail(GMM_ERR_CUDA, std::string("device '") + prop.name + "' is not sm_90 (H100); kernels are built for sm_90a only");
 
     gmm_ctx* c = new gmm_ctx();
     c->device = device; c->n = n_local; c->D = D; c->Kmax = Kmax; c->F = num_features(D);
@@ -1188,7 +1188,10 @@ static int run_dev_iterations(gmm_ctx* c, int K, int iters, float* ll_prev) {
         scatter_param_set(c, K);
     }
     c->iterations -= iters - first_bad;
-    if (int rc = upload_params(c, K)) return rc;
+    // A set left by the device finalisation is rebuilt as the host path builds it after its own finalisation: inverse,
+    // constant, pi and the E-step operand from ONE factorisation of R (the device set is bit-identical to it); refactorising
+    // the stored float Rinv would hand the E-step a slightly different operand.
+    if (int rc = upload_params(c, K, /*with_constants=*/first_bad > 0)) return rc;
     if (int rc = zero_stats(c, K)) return rc;
     if (int rc = run_estep(c, K)) return rc;
     float prev = 0.f;

@@ -82,6 +82,11 @@ void constants_cluster(int k, int D, clusters_t* c) {
 // LU inverse plus the separate factorisation of Rinv the tensor E-step's operand needs (W is handed to it directly).
 // Returns false (nothing written) when R is not positive definite: the caller then takes the no-pivot LU path, whose
 // semantics on such matrices are the reference's (invert_matrix.cpp:25-101).
+// Every product is rounded before it is added (no fused multiply-add, whatever the compiler vectorises): the device-side
+// finalisation (finalize_params_kernel) evaluates the same operations in the same order with __dmul_rn / __dsub_rn, so the
+// two finalisations produce bit-identical factors and E-step operands.
+#pragma GCC push_options
+#pragma GCC optimize("fp-contract=off")
 bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out */) {
     double U[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS];
     const float* R = c->R + (size_t)k * D * D;
@@ -120,6 +125,7 @@ bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out 
     c->constant[k] = (float)(-D * 0.5 * std::log(2.0 * kPi) - 0.5 * (2.0 * ld));   // gaussian_kernel.cu:241
     return true;
 }
+#pragma GCC pop_options
 
 void mixing_weights(int K, clusters_t* c) {
     double sum = 0;                                                            // :176-181

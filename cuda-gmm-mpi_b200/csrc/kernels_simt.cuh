@@ -1,9 +1,9 @@
-// kernels_simt.cuh — CUDA-core (SIMT) kernels of the EM hot path for sm_100a.
+// kernels_simt.cuh — CUDA-core (SIMT) kernels of the EM hot path for sm_90a.
 //
 // These are the reference-arithmetic GPU kernels: FP32 quadratic form exactly
 // as estep1 forms it ((x - mu) first, then the D x D form), FP64 accumulation
 // of the M-step statistics.  They are the accuracy anchor on the device and the
-// path for shapes the tcgen05 kernels do not cover.  Layouts:
+// path for shapes the wgmma kernels do not cover.  Layouts:
 //   xs    : events SoA  [D][xpitch] (device transpose of the AoS shard, rows pitched to 32 events; the
 //           reference keeps the same copy: gaussian.cu:209-218, 373-377)
 //   memb  : responsibilities, cluster-major [K][n] (gaussian.h:75)
@@ -110,7 +110,7 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
 // phi = [1, x, x_i x_j (i>=j)].  This is a (K x n) . (n x F) product; here it
 // runs on the FP64 CUDA cores (products of two floats are exact in double, so
 // the statistics are exact up to the final double rounding) — it is the
-// accuracy anchor for the tcgen05 path, not the fast path.
+// accuracy anchor for the wgmma path, not the fast path.
 // Thread layout: 256 threads = 16 (cluster groups of CPT) x 16 (feature lanes,
 // JMAX features each); TE events per shared-memory tile.
 // ---------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// kernels_tc.cu — tcgen05 (UTCHMMA) kernels of the EM hot path for sm_100a.
+// kernels_tc.cu — warpgroup-MMA (wgmma) kernels of the EM hot path for sm_90a.
 //
 // M-step (mstep_N + mstep_means + mstep_covariance1 of the reference,
 // gaussian_kernel.cu:522-677) as ONE tensor-core contraction over the events:
@@ -7,43 +7,36 @@
 //
 // with the per-event feature vector phi = [1, z_d, z_i z_j (i>=j)] (F = 1+D+D(D+1)/2
 // rows, shared by all clusters) as the A operand and the responsibilities as the
-// B operand; FP32 accumulation in TMEM.
+// B operand; FP32 accumulation in registers.
 //
-// Operand arithmetic (round 2).  The FP32 accumulation in TMEM truncates toward zero (tc_probe T2/T7) — but it
-// is EXACT as long as every partial sum is a multiple of one quantum and fits 24 bits (tc_probe T8).  The
-// operands are therefore split into a FIXED-POINT leading part and a small remainder:
+// Operand arithmetic.  The tensor cores' FP32 accumulation does not round to nearest — but it is EXACT as long as
+// every partial sum is a multiple of one quantum and fits 24 bits.  The operands are therefore split into a
+// FIXED-POINT leading part and a small remainder:
 //     phi_f = ph + pl,   ph = q_f * round(phi_f / q_f),   |ph| <= 2^11 q_f     (q_f: power of two per feature row,
 //                                                                              from the data's largest |z_d|)
 //     g     = gh + gl,   gh = 2^-6 * round(2^6 g)   (0 .. 64 quanta)
-// (both by a magic-number add: no conversion round trip), and the products go to two accumulators per
-// 128-row feature tile:
-//     columns [0, 64):    sum ph * gh                 — every product a multiple of q_f 2^-6, at most 2^17 quanta;
+// (both by a magic-number add: no conversion round trip), and the products go to two accumulator column groups
+// per feature tile:
+//     columns [0, 32):    sum ph * gh                 — every product a multiple of q_f 2^-6, at most 2^17 quanta;
 //                                                       128 events per chain: <= 2^24 quanta: NO rounding at all
-//     columns [64, 128):  sum ph * gl + pl * gs       — gs = g rounded once to FP16 (11 bits RELATIVE): with gh alone
+//     columns [32, 64):   sum ph * gl + pl * gs       — gs = g rounded once to FP16 (11 bits RELATIVE): with gh alone
 //                                                       the dropped pl * gl would be O(pl / phi) of every event whose
-//                                                       g is below the quantum (measured: 1.6e-4 on covariances);
-//                                                       ~1 % of the magnitude, its truncation bias (~1e-6 relative to
-//                                                       itself) is 1e-8 of the statistic
-// The raw-moment cancellation |mu - shift|^2 / sigma^2 ~ 100 that amplified the old split's systematic error
-// (1.5e-3 on responsibilities after 100 EM iterations) now multiplies unbiased rounding noise only.
-// With B = [gh ; gl] stacked as ONE N = 128 operand, ph x [gh ; gl] is a single MMA at the tensor pipe's math
-// rate (64 cycles; N = 64 runs at 49.8, operand-fetch bound) that fills both column groups; pl x gs (N = 64)
-// adds into the second group: 114 instead of 149 cycles per (tile, k-step) and 14 instead of 18 KB of operand
-// fetch.
+//                                                       g is below the quantum; ~1 % of the magnitude, its truncation
+//                                                       bias is 1e-8 of the statistic
+// The raw-moment cancellation |mu - shift|^2 / sigma^2 ~ 100 multiplies unbiased rounding noise only.
+// With B = [gh ; gl] stacked as ONE N = 64 operand, ph x [gh ; gl] is a single MMA that fills both column groups;
+// pl x gs (N = 32) adds into the second group.
 //
-// Dataflow per CTA (persistent over a contiguous range of events, 512 threads):
+// Dataflow per CTA (persistent over a contiguous range of events, 32 clusters per CTA row of the grid):
 //   warp 0      TMA producer: tile [D][32 events] of the pre-standardised SoA copy z and raw
-//               responsibility tile [64 clusters][32 events] (2-D tensor maps, SWIZZLE_128B for
+//               responsibility tile [32 clusters][32 events] (2-D tensor maps, SWIZZLE_128B for
 //               the latter, zero fill out of bounds)
 //   warps 4-11  operand builders (two warpgroups on alternate tiles): form the products, split
-//               them, write the UMMA operand images (SWIZZLE_NONE core-matrix layout)
-//   warp 1      MMA issuer: per 32 events and feature tile 2 x (M=128, N=128, K=16) + 2 x (M=128, N=64, K=16)
-//   warps 12-15 flush: accumulators are SINGLE-buffered (3 tiles x 128 columns at D = 24); each feature tile
-//               is drained every 128 events, the three tiles staggered by one sub-tile so that a drain
-//               (TMEM -> registers, FP32 round-to-nearest adds into 192 register-resident partial sums per
-//               thread) overlaps the MMAs of the other tiles.  The partial sums stay in registers for the whole
-//               CTA range and are written ONCE (no scratch zeroing, no atomics: round 1 moved 1.7 GB of
-//               RED.ADD.F64 traffic per launch).
+//               them, write the wgmma operand images (no-swizzle core-matrix layout)
+//   warpgroups 3 .. 2+MT  consumers, one per 128-row feature tile: per 32 events 2 x 2 x (m64n64k16 + m64n32k16)
+//               wgmma with the accumulators in registers.  The exact group is drained every 128 events and the
+//               remainder group every 512 into FP32 round-to-nearest partial sums held in shared memory (one private
+//               slot per thread), written ONCE per CTA (no scratch zeroing, no atomics).
 // A second tiny kernel reduces the per-CTA partials in double and un-scales.
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -79,12 +72,11 @@ using namespace ptx;
 // M-step kernel configuration
 // ---------------------------------------------------------------------------
 constexpr int kTE = 32;          // events per sub-tile (MMA K extent per operand part)
-constexpr int kNCL = 64;         // clusters per CTA pass
-constexpr int kNST = 3;          // operand stages
+constexpr int kNCL = 32;         // clusters per CTA pass (N of the exact / remainder groups: register budget of the consumers)
+constexpr int kNST = 2;          // operand stages
 constexpr int kNRAW = 4;         // raw (TMA) stages
 constexpr int kChunkSub = 4;     // sub-tiles per chain of the exact column group: 128 events (the bit budget below)
 constexpr int kChunkSub2 = 16;   // sub-tiles per chain of the remainder column group (no exactness to protect: drained 4x less often)
-constexpr int kMThreads = 512;
 // Bit budget of the exact accumulator: 11 (ph, every integer up to 2048 is an FP16 value) + 6 (gh) + 7 (128 events) = 24.
 // The split favours phi: the remainder pl is rounded to FP16 RELATIVE to itself, so its (unbiased) rounding noise scales
 // with the quantum of ph — on covariance entries 6e-6 per call with 9 + 8 bits, 1.2e-6 with 11 + 6 (scripts/emu_mstep.py).
@@ -122,12 +114,28 @@ template <int D> struct MCfg {
     static constexpr int OFF_G = OFF_PHI + kNST * PHI_STAGE;
     static constexpr int OFF_RAWX = OFF_G + kNST * G_STAGE;
     static constexpr int OFF_RAWG = OFF_RAWX + kNRAW * RAWX;
-    static constexpr int OFF_BAR = OFF_RAWG + kNRAW * RAWG;
+    static constexpr int NCT = MT * 128;                  // consumer threads (one warpgroup per 128-row feature tile)
+    static constexpr int OFF_RACC = OFF_RAWG + kNRAW * RAWG;   // [32][NCT] FP32 partial sums, one private column per thread
+    static constexpr int OFF_BAR = OFF_RACC + 32 * NCT * 4;
     static constexpr int SMEM_BYTES = OFF_BAR + 512;
-    static constexpr int TMEM_COLS = MT * 128;            // per feature tile: [ph gh | ph gl + pl gh]
+    static constexpr int THREADS = 384 + NCT;             // producer warpgroup, two builder warpgroups, consumers
+    // register pools: producer / builders / consumers.  The kernel is launched with REG_LAUNCH registers per thread
+    // (the __launch_bounds__ maximum, which ptxas uses when setmaxnreg is present); setmaxnreg only redistributes that
+    // allocation, so a warpgroup's increase waits until the others' decreases have freed enough — the sum must fit.
+    static constexpr int REG_LAUNCH = (65536 / THREADS) / 8 * 8 > 255 ? 255 : (65536 / THREADS) / 8 * 8;
+    static constexpr int REG_P = MT == 1 ? 40 : 24;
+    static constexpr int REG_B = MT == 3 ? 80 : 112;
+    static constexpr int REG_C = MT == 3 ? 96 : (MT == 2 ? 112 : 240);
+    static_assert(128 * REG_P + 256 * REG_B + NCT * REG_C <= THREADS * REG_LAUNCH, "register pools");
     static_assert(OFF_RAWG % 1024 == 0 && RAWG % 1024 == 0, "SWIZZLE_128B TMA destinations need 1024-byte alignment");
-    static_assert(MT <= 3, "accumulator tiles");
+    static_assert(MT <= 3, "feature tiles");
 };
+
+template <int R, int L>
+__device__ __forceinline__ void set_regs() {
+    if constexpr (R < L) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+    else if constexpr (R > L) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 
 // Rounding constants: (v + magic) - magic = q * round(v / q) with magic = 1.5 * 2^23 * q.  One quantum for the
 // coordinate rows and one for the product rows (bound = the largest |z_d| of the data over ALL dimensions, rounded up
@@ -206,7 +214,7 @@ static RowInfo tc_row_info(int D, int row) {
 }
 
 // Feature tile `mt` is drained after sub-tile i when its 128-event chain ends there: the chains of the tiles are
-// staggered by one sub-tile each, so that only one tile is being drained at a time (single-buffered accumulators).
+// staggered by one sub-tile each, so that the consumer warpgroups do not all drain after the same sub-tile.
 // The remainder column group rides along and is drained (and restarted) only at every fourth of those points.
 __device__ __forceinline__ bool chain_ends(int i, int mt, int nsub) { return ((i + mt) % kChunkSub) == kChunkSub - 1 || i == nsub - 1; }
 __device__ __forceinline__ bool chain_starts(int i, int mt) { return i == 0 || ((i + mt) % kChunkSub) == 0; }
@@ -214,7 +222,7 @@ __device__ __forceinline__ bool chain2_ends(int i, int mt, int nsub) { return ((
 __device__ __forceinline__ bool chain2_starts(int i, int mt) { return i == 0 || ((i + mt) % kChunkSub2) == 0; }
 
 template <int D>
-__global__ void __launch_bounds__(kMThreads, 1)
+__global__ void __launch_bounds__(MCfg<D>::THREADS, 1)
 mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_g, int n,
                 float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic) {
     using C = MCfg<D>;
@@ -224,9 +232,6 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     uint64_t* raw_empty = bars + kNRAW;        // [kNRAW]
     uint64_t* op_full = bars + 2 * kNRAW;      // [kNST]
     uint64_t* op_empty = op_full + kNST;       // [kNST]
-    uint64_t* acc_full = op_empty + kNST;      // [MT]  chain of feature tile mt complete (tcgen05.commit)
-    uint64_t* acc_empty = acc_full + 3;        // [MT]  tile mt drained (4 flush warps)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 3);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int e_begin = blockIdx.x * events_per_cta;
@@ -235,81 +240,32 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     const int k0 = blockIdx.y * kNCL;
 
     // ---- one-time setup ----
-    for (int i = threadIdx.x * 16; i < C::OFF_RAWX; i += kMThreads * 16) *reinterpret_cast<uint4*>(smem + i) = make_uint4(0, 0, 0, 0);
+    for (int i = threadIdx.x * 16; i < C::OFF_RAWX; i += C::THREADS * 16) *reinterpret_cast<uint4*>(smem + i) = make_uint4(0, 0, 0, 0);
     if (threadIdx.x == 0) {
         for (int s = 0; s < kNRAW; s++) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 4); }
-        for (int s = 0; s < kNST; s++) { mbar_init(&op_full[s], 4); mbar_init(&op_empty[s], 1); }
-        for (int s = 0; s < 3; s++) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4); }
+        for (int s = 0; s < kNST; s++) { mbar_init(&op_full[s], 4); mbar_init(&op_empty[s], 4 * C::MT); }
         fence_mbar_init();
     }
-    if (warp == 2) tmem_alloc<512>(tmem_slot);
     fence_proxy_async_smem();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    // register re-partition between the warpgroups (64K registers per SM):
-    //   WG0 (TMA / MMA / alloc) 40, WG1-2 (builders) 112, WG3 (flush accumulators) 240
     if (warp < 4) {
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-      if (warp == 0) {
-        // ===================== TMA producer =====================
-        if (elect_one()) {
-            for (int i = 0; i < nsub; i++) {
-                const int st = i % kNRAW, ph = (i / kNRAW) & 1;
-                mbar_wait_parked(&raw_empty[st], ph ^ 1, 500);
-                mbar_arrive_expect_tx(&raw_full[st], kTE * D * 4 + C::RAWG);
-                const int e0 = e_begin + i * kTE;
-                tma_load_2d(smem + C::OFF_RAWX + st * C::RAWX, &tm_x, e0, 0, &raw_full[st]);
-                tma_load_2d(smem + C::OFF_RAWG + st * C::RAWG, &tm_g, e0, k0, &raw_full[st]);
-            }
-        }
-      } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc128 = make_idesc_f16(128, 2 * kNCL, /*A MN-major*/ true, /*B MN-major*/ false);
-            constexpr uint32_t idesc64 = make_idesc_f16(128, kNCL, true, false);
-            uint32_t drained = 0;                              // bit mt: wait parity of acc_empty[mt]
-            uint32_t used = 0;                                 // bit mt: tile mt has completed at least one chain
-            for (int i = 0; i < nsub; i++) {
-                const int os = i % kNST, oph = (i / kNST) & 1;
-                mbar_wait_parked(&op_full[os], oph, 100);
-                tc_fence_after();
-                const uint32_t phi = smem_u32(smem + C::OFF_PHI + os * C::PHI_STAGE);
-                const uint32_t gam = smem_u32(smem + C::OFF_G + os * C::G_STAGE);
-#pragma unroll
-                for (int mt = 0; mt < C::MT; mt++) {
-                    const bool first = chain_starts(i, mt), first2 = chain2_starts(i, mt);
-                    if (first && ((used >> mt) & 1u)) {        // the previous chain of this tile must have been drained
-                        mbar_wait_parked(&acc_empty[mt], (drained >> mt) & 1u, 100);
-                        drained ^= 1u << mt;
-                        tc_fence_after();
-                    }
-                    const uint32_t dcol = tmem + mt * 128;
-#pragma unroll
-                    for (int ks = 0; ks < kTE / 16; ks++) {
-                        const uint64_t bdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // rows 0-63 gh, 64-127 gl
-                        const uint64_t sdesc = make_smem_desc(gam + 2 * C::G_PART + ks * 256, 128, 512);     // gs
-                        const uint64_t ah = make_smem_desc(phi + mt * 8192 + ks * 256, /*LBO*/ 128, /*SBO*/ 512);
-                        const uint64_t al = make_smem_desc(phi + C::PHI_PART + mt * 8192 + ks * 256, 128, 512);
-                        if (first && !first2 && ks == 0) {     // restart the exact group only: the two halves as separate N = 64 steps
-                            const uint64_t ldesc = make_smem_desc(gam + C::G_PART + ks * 256, 128, 512);
-                            mma_f16_ss(dcol, ah, bdesc, idesc64, false);                //  ph gh
-                            mma_f16_ss(dcol + kNCL, ah, ldesc, idesc64, true);          //          += ph gl
-                        } else {
-                            mma_f16_ss(dcol, ah, bdesc, idesc128, !(first && ks == 0)); // [ph gh | ph gl]
-                        }
-                        mma_f16_ss(dcol + kNCL, al, sdesc, idesc64, true);             //          += pl gs
-                    }
-                    if (chain_ends(i, mt, nsub)) { mma_commit(&acc_full[mt]); used |= 1u << mt; }
+        set_regs<C::REG_P, C::REG_LAUNCH>();
+        if (warp == 0) {
+            // ===================== TMA producer =====================
+            if (elect_one()) {
+                for (int i = 0; i < nsub; i++) {
+                    const int st = i % kNRAW, ph = (i / kNRAW) & 1;
+                    mbar_wait_parked(&raw_empty[st], ph ^ 1, 500);
+                    mbar_arrive_expect_tx(&raw_full[st], kTE * D * 4 + C::RAWG);
+                    const int e0 = e_begin + i * kTE;
+                    tma_load_2d(smem + C::OFF_RAWX + st * C::RAWX, &tm_x, e0, 0, &raw_full[st]);
+                    tma_load_2d(smem + C::OFF_RAWG + st * C::RAWG, &tm_g, e0, k0, &raw_full[st]);
                 }
-                mma_commit(&op_empty[os]);                    // operand stage reusable once these MMAs retire
             }
         }
-      }
     } else if (warp < 12) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 112;");
+        set_regs<C::REG_B, C::REG_LAUNCH>();
         // ===================== operand builders =====================
         // two builder warpgroups work on alternate sub-tiles (two sub-tiles in flight), the four warps
         // of a group split the 16-byte feature chunks (c = part mod 4)
@@ -328,40 +284,37 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
 #pragma unroll
                 for (int d = 0; d < D; d++) { z[d] = xr[dd * kTE]; dd = dd + 1 == D ? 0 : dd + 1; }
             }
-            // --- responsibilities: thread -> (cluster row k, 8-event chunk ce), two items per thread.
+            // --- responsibilities: thread -> (cluster row k, 8-event chunk ce), one item per thread.
             // The raw tile is written by TMA with SWIZZLE_128B (16-byte chunk c of row r sits at chunk
             // c ^ (r & 7)), so 8 lanes reading the same chunk of 8 consecutive rows hit 8 different
             // bank groups; the operand image puts the 4 K-chunks of an 8-row group next to each other
             // (LBO = 128, SBO = 512), so a warp stores 512 contiguous bytes: no bank conflicts either way.
-            uint4 gh[2], gl[2], gs[2];
-            float gdep = 0.0f;
-#pragma unroll
-            for (int it2 = 0; it2 < 2; it2++) {
-                const int item = bt + it2 * 128;
-                const int kg = item >> 5, l = item & 31;
+            uint4 gh, gl, gs;
+            float gdep;
+            {
+                const int kg = bt >> 5, l = bt & 31;
                 const int k = kg * 8 + (l & 7), ce = l >> 3;
                 const uint8_t* grow = smem + C::OFF_RAWG + rs * C::RAWG + k * (kTE * 4);
                 const float4 a = *reinterpret_cast<const float4*>(grow + (((2 * ce) ^ (k & 7)) << 4));
                 const float4 b = *reinterpret_cast<const float4*>(grow + (((2 * ce + 1) ^ (k & 7)) << 4));
                 const float g[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                gdep += a.x + b.x;
+                gdep = a.x + b.x;
                 float hi[8], lo[8];
 #pragma unroll
                 for (int u = 0; u < 8; u++) {                  // gh = 16 * round(64 g) (0 .. 1024), gl = 1024 g - gh, both from the exact product
                     hi[u] = __fsub_rn(__fmaf_rn(g[u], kGammaScale, kGammaMagic), kGammaMagic);
                     lo[u] = __fmaf_rn(g[u], kGammaScale, -hi[u]);
                 }
-                gh[it2] = make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
-                gl[it2] = make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
-                gs[it2] = make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
-                                     pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
+                gh = make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
+                gl = make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
+                gs = make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
+                                pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
             }
             // The raw tiles must BE in registers before the stage goes back to the TMA producer: an mbarrier arrive does
-            // not wait for the warp's outstanding LDS (measured in round 1: with nothing consuming the z loads before the
-            // arrive, the refill of the stage overtook the loads of the last dimensions).  The arrive is therefore made
-            // data-dependent on every load of this thread: a sum over z and one component of each responsibility vector,
-            // folded into the arrive's own operand list below (the asm statement consumes the value, so neither the
-            // compiler nor the hardware can retire it before the loads have landed).
+            // not wait for the warp's outstanding shared-memory loads.  The arrive is therefore made data-dependent on
+            // every load of this thread: a sum over z and one component of the responsibility vector, folded into the
+            // arrive's own operand list below (the asm statement consumes the value, so neither the compiler nor the
+            // hardware can retire it before the loads have landed).
             float dep = gdep;
 #pragma unroll
             for (int d = 0; d < D; d++) dep += z[d];
@@ -373,68 +326,80 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
             uint8_t* phi_lo = phi_hi + C::PHI_PART;
             build_phi_chunks<D>(z, magic, phi_hi, phi_lo, lane, part);
             {
-                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512); gl = rows 64..127
+                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512); gl = rows 32..63
                 uint8_t* g_hi = smem + C::OFF_G + os * C::G_STAGE;
-#pragma unroll
-                for (int it2 = 0; it2 < 2; it2++) {
-                    const int item = bt + it2 * 128;
-                    const int kg = item >> 5, l = item & 31;
-                    *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) = gh[it2];
-                    *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) = gl[it2];
-                    *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) = gs[it2];
-                }
+                const int kg = bt >> 5, l = bt & 31;
+                *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) = gh;
+                *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) = gl;
+                *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) = gs;
             }
             fence_proxy_async_smem();
             __syncwarp();
             if (lane == 0) mbar_arrive(&op_full[os]);
         }
     } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
-        // ===================== flush: TMEM -> register-resident FP32 partial sums =====================
-        const int q = warp - 12;                                   // TMEM lane quadrant (= warp % 4)
-        float racc[C::MT * kNCL];
+        set_regs<C::REG_C, C::REG_LAUNCH>();
+        // ===================== consumers: wgmma, accumulators in registers =====================
+        const int mt = (warp - 12) >> 2;                           // feature tile of this warpgroup (rows 128 mt ..)
+        const int ct = threadIdx.x - 384;                          // consumer thread 0 .. NCT-1
+        const int wq = warp & 3, gid = lane >> 2, qd = lane & 3;
+        float* racc = reinterpret_cast<float*>(smem + C::OFF_RACC) + ct;     // [32][NCT]: racc[j * NCT]
 #pragma unroll
-        for (int j = 0; j < C::MT * kNCL; j++) racc[j] = 0.0f;
-        uint32_t full = 0;                                         // bit mt: wait parity of acc_full[mt]
+        for (int j = 0; j < 32; j++) racc[j * C::NCT] = 0.0f;
+        float acc[2][32];                                          // per 64-row half: regs 0-15 exact group, 16-31 remainder group
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int j = 0; j < 32; j++) acc[h][j] = 0.0f;
         for (int i = 0; i < nsub; i++) {
+            const int os = i % kNST, oph = (i / kNST) & 1;
+            mbar_wait_parked(&op_full[os], oph, 100);
+            const uint32_t phi = smem_u32(smem + C::OFF_PHI + os * C::PHI_STAGE);
+            const uint32_t gam = smem_u32(smem + C::OFF_G + os * C::G_STAGE);
+            wgmma_fence();
 #pragma unroll
-            for (int mt = 0; mt < C::MT; mt++) {
-                if (!chain_ends(i, mt, nsub)) continue;
-                mbar_wait_parked(&acc_full[mt], (full >> mt) & 1u, 300);
-                full ^= 1u << mt;
-                tc_fence_after();
-                const uint32_t tbase = tmem + ((uint32_t)(q * 32) << 16) + mt * 128;
-                // group 0: exact leading products; group 1 (only when its longer chain ends here): remainder products.
-                // One copy of the code for both (not unrolled: the kernel's SASS has to stay inside the 32 KB L1.5 I-cache).
-                const int ngroups = chain2_ends(i, mt, nsub) ? 2 : 1;
-#pragma unroll 1
-                for (int grp = 0; grp < ngroups; grp++) {
+            for (int h = 0; h < 2; h++) {
 #pragma unroll
-                    for (int b = 0; b < kNCL / 32; b++) {
-                        uint32_t a[32];
-                        tmem_ld_32x32(tbase + grp * kNCL + b * 32, a);
-                        tmem_ld_wait();
-#pragma unroll
-                        for (int j = 0; j < 32; j++) racc[mt * kNCL + b * 32 + j] += __uint_as_float(a[j]);
-                    }
+                for (int ks = 0; ks < kTE / 16; ks++) {
+                    const uint64_t bdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // rows 0-31 gh, 32-63 gl
+                    const uint64_t sdesc = make_smem_desc(gam + 2 * C::G_PART + ks * 256, 128, 512);     // gs
+                    const uint32_t arow = mt * 8192 + h * 4096 + ks * 256;
+                    const uint64_t ah = make_smem_desc(phi + arow, /*LBO*/ 128, /*SBO*/ 512);
+                    const uint64_t al = make_smem_desc(phi + C::PHI_PART + arow, 128, 512);
+                    wgmma_m64n64k16_ss_tn(acc[h], ah, bdesc);                                          // [ph gh | ph gl]
+                    wgmma_m64n32k16_ss_tn(*reinterpret_cast<float(*)[16]>(&acc[h][16]), al, sdesc);     //        += pl gs
                 }
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&acc_empty[mt]);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&op_empty[os]);         // operand stage reusable: these MMAs have read it
+            // drain: exact group at the end of its 128-event chain, remainder group at the end of its longer chain
+            if (chain_ends(i, mt, nsub)) {
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+#pragma unroll
+                    for (int j = 0; j < 16; j++) { racc[(h * 16 + j) * C::NCT] += acc[h][j]; acc[h][j] = 0.0f; }
+            }
+            if (chain2_ends(i, mt, nsub)) {
+#pragma unroll
+                for (int h = 0; h < 2; h++)
+#pragma unroll
+                    for (int j = 0; j < 16; j++) { racc[(h * 16 + j) * C::NCT] += acc[h][16 + j]; acc[h][16 + j] = 0.0f; }
             }
         }
-        // one plain store of this thread's partial sums: [cta][tile][row][64 clusters]
-        float* my = scratch + ((size_t)(blockIdx.y * gridDim.x + blockIdx.x) * C::MT * 128 + q * 32 + lane) * kNCL;
+        // one plain store of this thread's partial sums: [cta][tile][row][32 clusters]
+        float* my = scratch + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * C::MT * 128 * kNCL + (size_t)mt * 128 * kNCL;
 #pragma unroll
-        for (int mt = 0; mt < C::MT; mt++)
+        for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int j = 0; j < kNCL; j += 4)
-                *reinterpret_cast<float4*>(my + (size_t)mt * 128 * kNCL + j) =
-                    make_float4(racc[mt * kNCL + j], racc[mt * kNCL + j + 1], racc[mt * kNCL + j + 2], racc[mt * kNCL + j + 3]);
+            for (int j = 0; j < 16; j += 2) {
+                const int row = h * 64 + wq * 16 + gid + 8 * ((j >> 1) & 1);
+                const int col = (j >> 2) * 8 + 2 * qd;
+                *reinterpret_cast<float2*>(my + (size_t)row * kNCL + col) =
+                    make_float2(racc[(h * 16 + j) * C::NCT], racc[(h * 16 + j + 1) * C::NCT]);
+            }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc<512>(tmem);
 }
 
 // z = (x - shift) * inv_scale over the SoA event copy, once per data set: the centred/scaled copy the M-step
@@ -455,8 +420,9 @@ __global__ void standardise_soa_kernel(const float* __restrict__ xs, float* __re
 __global__ void __launch_bounds__(256)
 mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, int K, int F, const int3* __restrict__ rowmap,
                          const double* __restrict__ scale, double* __restrict__ stats) {
-    // one block per operand row; thread -> (cluster column, quarter of the CTAs): 256-byte coalesced reads
-    __shared__ double part[4][kNCL];
+    // one block per operand row; thread -> (cluster column, eighth of the CTAs): 128-byte coalesced reads
+    constexpr int NQ = 256 / kNCL;
+    __shared__ double part[NQ][kNCL];
     const int3 rm = rowmap[blockIdx.x];
     if (rm.x < 0) return;
     const int mt = blockIdx.x / 128, row = blockIdx.x % 128;
@@ -466,12 +432,17 @@ mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, 
     if (rm.z >= 0) fac *= scale[rm.z];
     for (int ty = 0; ty * kNCL < K; ty++) {
         double s = 0;
-        for (int cx = q; cx < ncta_x; cx += 4)
+        for (int cx = q; cx < ncta_x; cx += NQ)
             s += (double)scratch[(((size_t)(ty * ncta_x + cx) * MT + mt) * 128 + row) * kNCL + col];
         part[q][col] = s;
         __syncthreads();
         const int k = ty * kNCL + col;
-        if (q == 0 && k < K) stats[(size_t)k * F + rm.x] += (part[0][col] + part[1][col] + part[2][col] + part[3][col]) * fac;
+        if (q == 0 && k < K) {
+            double t = 0;
+#pragma unroll
+            for (int u = 0; u < NQ; u++) t += part[u][col];
+            stats[(size_t)k * F + rm.x] += t * fac;
+        }
         __syncthreads();
     }
 }
@@ -479,401 +450,260 @@ mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, 
 // ===========================================================================
 // E-step (estep1 + estep2 of the reference, gaussian_kernel.cu:383-512) on
 // tensor cores.  With Rinv = W^T W (W upper triangular, from the Cholesky
-// factor of Rinv computed on the host) the quadratic form is
+// factor of Rinv) the quadratic form is
 //     q_k(x) = || W_k (x - mu_k) ||^2 = || W'_k z + v_k ||^2 ,   z = (x - shift) * inv_scale,
 // i.e. ONE GEMM  Y[n][(k,d)] = Z~[n][:] . B[(k,d)][:]  with the constant folded in
 // through a ones column, followed by a square-and-sum epilogue, the log-sum-exp
 // over the clusters and the log-likelihood reduction.  Operands are FP16 hi/lo
-// split (z = zh + zl, W' = Wh + Wl); the K dimension concatenates
-//     [ zh_c zl_c ]_c | [ zh | 1 1 0.. ]     x     [ Wh_c Wh_c ]_c | [ Wl | vh vl 0.. ]
-// (the lo*lo product is dropped), FP32 accumulation in TMEM.  The duplicated Wh
-// chunk is not stored twice: the B descriptor of those MMA steps uses a leading
-// byte offset of 0, so both 8-element K chunks alias the same shared-memory chunk
-// (verified by csrc/probe/tc_probe.cu, test T5).  That makes the whole B operand
-// (all clusters: 172 KB at K=64, D=24) RESIDENT in the shared memory of one CTA;
-// only the event tiles stream.
+// split (z = zh + zl, W' = Wh + Wl); the products kept are zh Wh, zl Wh, zh Wl and
+// 1 v (the lo*lo product is dropped), FP32 accumulation in registers.  The whole
+// B operand (all clusters of a pass: 168 KB at K=64, D=24) is RESIDENT in the
+// shared memory of one CTA; only the events stream, and they never touch shared
+// memory: each thread converts its own rows straight into wgmma A fragments
+// (register operand), so one k-step may pair ANY two B chunks (start + LBO).
 //
-// One persistent CTA per SM, 768 threads in six warpgroups (round 2: the epilogue is split in two stages — round 1's
-// eight epilogue warps did squares, log-sum-exp and stores back to back, 6370 cycles per 128-event tile of which the MMA
-// issuer was stalled 3500 behind full accumulators while they were busy with log-sum-exp and stores; the per-phase
-// counters of that kernel are in profiles/):
-//   warp 1       MMA issuer: per 128-event tile, per supergroup of 16 clusters and per block c of 8
-//                output dimensions, the k-steps that block needs (tcgen05.mma M=128, N=128, K=16)
-//   warp 2       TMEM allocation: 3 accumulator buffers x 128 columns + 2 x 64 columns for the hand-over of q
-//   warps 4-7    converters: coalesced loads of the event rows, centre/scale, FP16 hi/lo
-//                split, K-major SWIZZLE_NONE operand image (2 stages)
-//   warps 8-15   squares (two warpgroups, each takes 8 of the 16 clusters of every supergroup): tcgen05.ld of the
-//                accumulators (buffer released as soon as the values are in registers) -> packed fma.f32x2 sums of
-//                squares carried over the blocks -> q[event][cluster] written back to TMEM (tcgen05.st)
-//   warps 16-23  log-sum-exp + stores (two warpgroups, 32 clusters each): tcgen05.ld of q -> base-2 logits ->
-//                max / sum-exp2 (+ exchange between the warpgroups) -> responsibilities (coalesced 128-byte row
-//                segments) + log-likelihood (double) — for tile t while the MMAs and the squares of tile t+1 run
+// One persistent CTA per SM, NWG independent warpgroups; each takes 64-event tiles in turn and per supergroup of 16
+// clusters and block c of 8 output dimensions issues the k-steps that block needs (m64n128k16, A from registers),
+// then squares and sums the 8 columns of each cluster (a quad of lanes holds them), the log-sum-exp over the
+// clusters (again within the quad) and writes the responsibilities and the log-likelihood.  The warpgroups
+// interleave, so one's MMAs overlap another's epilogue.
 // ===========================================================================
 
 // Block structure.  W is upper triangular, so the 8 output columns d in [8c, 8c+8) of a cluster
 // ("block" c) only need the K chunks z_j with j >= c.  Columns are therefore grouped by block:
 // one MMA N tile = block c of 16 clusters (N = 128), and block c issues only the k-steps it needs —
-// 5 + 4 + 2 = 11 instead of 15 at D = 24 (-27 % tensor work and TMEM accumulator traffic).
+// 5 + 4 + 2 = 11 instead of 15 at D = 24.
 template <int D> struct ECfg {
     static_assert(D % 8 == 0, "tensor E-step: D must be a multiple of 8");
     static constexpr int CP = D / 8;                          // 8-wide chunks of z / blocks of output columns
-    static constexpr int NLO = (CP + 1 + 1) / 2 * 2;          // chunks of the [zh | ones (| pad)] x [Wl | v] part
-    static constexpr int NCHKA = 2 * CP + 2;                  // A image chunks: (zh_c, zl_c) pairs, then the constant chunks ones, zero
+    static constexpr int NLO = (CP + 1 + 1) / 2 * 2;          // chunks of the [Wl | v (| pad)] part of the B image
     static constexpr int NCHKB = CP + NLO;                    // B image chunks: Wh_c, then Wl.., v, pad
     static constexpr int GB = 16;                             // clusters per supergroup
     static constexpr int N = GB * 8;                          // MMA N = one block of a supergroup (128 columns)
     static constexpr int MAXSG = 64 / GB;                     // up to 64 clusters resident
-    static constexpr int NBUF = 3;                            // TMEM accumulator buffers (3 x 128 columns)
-    static constexpr int QCOL = NBUF * N;                     // first column of the q hand-over: 2 tiles x 64 clusters
-    static constexpr int NWG = 2;                             // warpgroups per epilogue stage
-    static constexpr int CW = GB / NWG;                       // clusters per warpgroup per supergroup
-    static constexpr int LPT = MAXSG * CW;                    // logits held per log-sum-exp thread (32)
-    static constexpr int A_STAGE = NCHKA * 128 * 16;
     static constexpr int B_BLOCK = NCHKB * N * 16;            // one block of one supergroup
     static constexpr int B_SG = CP * B_BLOCK;
     static constexpr int OFF_B = 0;
-    static constexpr int OFF_A = OFF_B + MAXSG * B_SG;
-    static constexpr int OFF_CK = OFF_A + 2 * A_STAGE;        // float[64] (constant + ln(pi)) * log2(e), then float[64] -0.5 * log2(e) / scale_k^2
-    static constexpr int OFF_EX = OFF_CK + 512;               // exchange: [2 parity][NWG][128] x (max, sum)
-    static constexpr int OFF_BAR = OFF_EX + 2 * NWG * 128 * 8;
-    static constexpr int SMEM_BYTES = OFF_BAR + 512;
-    static constexpr int THREADS = 256 + 2 * 128 * NWG;       // warpgroup 0, converters, 2 square + 2 log-sum-exp warpgroups
-    static_assert(QCOL + 2 * 64 <= 512, "TMEM columns");
+    static constexpr int OFF_CK = OFF_B + MAXSG * B_SG;       // float[64] (constant + ln(pi)) * log2(e), then float[64] -0.5 * log2(e) / scale_k^2
+    static constexpr int OFF_SH = OFF_CK + 512;               // float[32] shift, float[32] inverse scale
+    static constexpr int OFF_BAR = OFF_SH + 256;
+    static constexpr int SMEM_BYTES = OFF_BAR + 64;
+    static constexpr int NWG = 2;                             // warpgroups per CTA (255 registers each: no spills at D = 24)
+    static constexpr int THREADS = 128 * NWG;
 };
 
 template <int D>
-__global__ void __launch_bounds__(768, 1)
+__global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
 estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
                 const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float* __restrict__ memb,
                 size_t pitch, int n, int K, int NSG, double* __restrict__ ll_out, int mode, const float* den_in,
                 float* den_out) {
     // K / NSG / b_img / ck / memb describe ONE pass of at most 64 clusters.  More than 64 clusters take 2P - 1 launches
-    // for P passes, and every responsibility is written exactly once (round 1 normalised each pass within itself and
-    // rescaled all of them in a read-modify-write pass over the memberships):
+    // for P passes, and every responsibility is written exactly once:
     //   mode 1 (passes 0 .. P-2)  log-denominator only: den_out[e] = ln(sum_k exp(logit)) (+ den_in[e] in log space), no stores
     //   mode 2 (pass P-1)         its own log-sum-exp joined with den_in[e] (all other passes): final responsibilities of this
     //                             pass, den_out[e] = the event's total log-denominator, log-likelihood
-    //   mode 3 (passes 0 .. P-2)  responsibilities against the known total den_in[e]: no log-sum-exp, no exchange
+    //   mode 3 (passes 0 .. P-2)  responsibilities against the known total den_in[e]: no log-sum-exp
     //   mode 0                    single pass (K <= 64)
     using C = ECfg<D>;
-    constexpr int NWG = C::NWG;
+    constexpr int CP = C::CP;
     extern __shared__ __align__(1024) uint8_t smem[];
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
-    uint64_t* a_full = bars;            // [2]  4 converter warps
-    uint64_t* a_empty = bars + 2;       // [2]  tcgen05.commit
-    uint64_t* b_full = bars + 4;        // [1]
-    uint64_t* acc_full = bars + 5;      // [NBUF]  tcgen05.commit
-    uint64_t* acc_empty = bars + 8;     // [NBUF]  8 square warps
-    uint64_t* q_full = bars + 11;       // [2]  8 square warps: q of a tile is in TMEM
-    uint64_t* q_empty = bars + 13;      // [2]  8 log-sum-exp warps: q of a tile is in their registers
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
     float* ck_s = reinterpret_cast<float*>(smem + C::OFF_CK);          // [64] additive logit constants, [64] multipliers
-    float2* ex = reinterpret_cast<float2*>(smem + C::OFF_EX);
-    float* sh_s = reinterpret_cast<float*>(smem + C::OFF_BAR + 128);   // [32] shift, [32] inverse scale
+    float* sh_s = reinterpret_cast<float*>(smem + C::OFF_SH);          // [32] shift, [32] inverse scale
     float* isc_s = sh_s + 32;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int ntiles = (n + 127) / 128;
-    const int my_tiles = (int)blockIdx.x < ntiles ? (ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int gid = lane >> 2, qd = lane & 3;
+    const int ntiles = (n + 63) / 64;
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < 2; s++) { mbar_init(&a_full[s], 4); mbar_init(&a_empty[s], 1); }
-        for (int s = 0; s < C::NBUF; s++) { mbar_init(&acc_full[s], 1); mbar_init(&acc_empty[s], 4 * NWG); }
-        for (int s = 0; s < 2; s++) { mbar_init(&q_full[s], 4 * NWG); mbar_init(&q_empty[s], 4 * NWG); }
-        mbar_init(b_full, 1);
-        fence_mbar_init();
-    }
+    if (threadIdx.x == 0) { mbar_init(b_full, 1); fence_mbar_init(); }
     // base-2 logits in the epilogue: l2 = ck * log2(e) + (-0.5 * log2(e) / scale_k^2) * |scale_k * y|^2   (the per-cluster
     // power-of-two scale_k keeps the FP16 whitening factors in range whatever the cluster's width, see bimg_cluster)
     if (threadIdx.x < 64) { ck_s[threadIdx.x] = ck[threadIdx.x] * 1.4426950408889634f; ck_s[64 + threadIdx.x] = ck[64 + threadIdx.x]; }
     if (threadIdx.x < D) { sh_s[threadIdx.x] = shift_f[threadIdx.x]; isc_s[threadIdx.x] = inv_scale_f[threadIdx.x]; }
-    if (threadIdx.x >= 128 && threadIdx.x < 256) {             // constant chunks of both A stages: {1, 1, 0 ...} and zeros
-        const int row = threadIdx.x - 128;
-#pragma unroll
-        for (int st = 0; st < 2; st++) {
-            uint8_t* a = smem + C::OFF_A + st * C::A_STAGE + row * 16;
-            *reinterpret_cast<uint4*>(a + (2 * C::CP) * 2048) = make_uint4(0x3C003C00u, 0u, 0u, 0u);
-            *reinterpret_cast<uint4*>(a + (2 * C::CP + 1) * 2048) = make_uint4(0u, 0u, 0u, 0u);
-        }
-        fence_proxy_async_smem();
-    }
     __syncthreads();
     if (threadIdx.x == 0) {                    // resident B operand: one TMA bulk copy per block
         mbar_arrive_expect_tx(b_full, (uint32_t)NSG * C::B_SG);
-        for (int g = 0; g < NSG * C::CP; g++) tma_load_1d(smem + C::OFF_B + g * C::B_BLOCK, b_img + (size_t)g * C::B_BLOCK, C::B_BLOCK, b_full);
+        for (int g = 0; g < NSG * CP; g++) tma_load_1d(smem + C::OFF_B + g * C::B_BLOCK, b_img + (size_t)g * C::B_BLOCK, C::B_BLOCK, b_full);
     }
-    if (warp == 2) tmem_alloc<512>(tmem_slot);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
 
-    // register pools (launch: 768 x 80 = 61440): WG0 24, converters 72, squares 2 x 112, log-sum-exp 2 x 80
-    if (warp < 4) {
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
-      if (warp == 1) {
-        // ===================== MMA issuer =====================
-        if (elect_one()) {
-            constexpr uint32_t idesc = make_idesc_f16(128, C::N, false, false);
-            uint32_t pe = (1u << C::NBUF) - 1u;                // wait parity of acc_empty[b], one bit per buffer
-            mbar_wait(b_full, 0);                              // the resident B image has landed (the converters did not wait for it)
-            for (int it = 0; it < my_tiles; it++) {
-                const int as = it & 1, aph = (it >> 1) & 1;
-                mbar_wait_parked(&a_full[as], aph, 200);
-                tc_fence_after();
-                const uint32_t abase = smem_u32(smem + C::OFF_A + as * C::A_STAGE);
-                uint32_t buf = 0;                              // the buffer sequence restarts with every tile (squares: same rule)
-                for (int sg = 0; sg < NSG; sg++) {
+    // rows r0 = 16 warp + gid and r1 = r0 + 8 of each 64-event tile; K positions 2 qd, 2 qd + 1 of every 8-wide chunk
+    const int r0 = warp * 16 + gid;
+    float2 xa[CP], xb[CP];                     // raw coordinates of the two rows (prefetched one tile ahead)
+    auto load_rows = [&](int t) {
+        const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
 #pragma unroll
-                    for (int c = 0; c < C::CP; c++) {
-                        mbar_wait_parked(&acc_empty[buf], (pe >> buf) & 1u, 100);
-                        pe ^= 1u << buf;
-                        tc_fence_after();
-                        const uint32_t bbase = smem_u32(smem + C::OFF_B + (sg * C::CP + c) * C::B_BLOCK);
-                        bool acc = false;
+        for (int j = 0; j < CP; j++) {
+            xa[j] = e0 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e0 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+            xb[j] = e1 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e1 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+        }
+    };
+    const int stride = (int)gridDim.x * C::NWG;
+    int t = (int)blockIdx.x * C::NWG + wg;
+    if (t < ntiles) load_rows(t);
+    const uint32_t ones = qd == 0 ? 0x3C003C00u : 0u;         // chunk {1, 1, 0 ...}: K elements 0 and 1 are held by qd == 0
+    const uint32_t bsm = smem_u32(smem + C::OFF_B);
+    constexpr uint32_t CH = C::N * 16;                        // bytes per B chunk
+    double ll_acc = 0.0;
+    constexpr float kLn2 = 0.6931471805599453f;
+    mbar_wait(b_full, 0);
+
+    for (; t < ntiles; t += stride) {
+        uint32_t zh[CP][2], zl[CP][2];                         // [chunk][row]: FP16 pairs, hi and lo parts
 #pragma unroll
-                        for (int j = c; j < C::CP; j++) {       // (zh_j, zl_j) x (Wh_j, Wh_j): B chunk aliased through LBO = 0
-                            const uint64_t adesc = make_smem_desc(abase + (2 * j) * 2048, /*LBO*/ 2048, /*SBO*/ 128);
-                            const uint64_t bdesc = make_smem_desc(bbase + j * (C::N * 16), /*LBO*/ 0, /*SBO*/ 128);
-                            mma_f16_ss(tmem + buf * C::N, adesc, bdesc, idesc, acc);
-                            acc = true;
-                        }
+        for (int j = 0; j < CP; j++) {
+            const float s0 = sh_s[8 * j + 2 * qd], s1 = sh_s[8 * j + 2 * qd + 1];
+            const float i0 = isc_s[8 * j + 2 * qd], i1 = isc_s[8 * j + 2 * qd + 1];
 #pragma unroll
-                        for (int t = 0; t < C::NLO / 2; t++) {  // (zh.., ones) x (Wl.., v): needed iff it holds a chunk index >= c
-                            if (2 * t + 1 >= c) {
-                                // A side of this step: elements 2t and 2t+1 of [zh_0 .. zh_{CP-1}, ones, zero] — zh_m is the chunk the
-                                // (zh_m, zl_m) steps already use (chunk 2m), so the step's two K chunks are simply further apart
-                                constexpr int CP_ = C::CP;
-                                const int m0 = 2 * t, m1 = 2 * t + 1;
-                                const int ch0 = m0 < CP_ ? 2 * m0 : 2 * CP_ + (m0 - CP_), ch1 = m1 < CP_ ? 2 * m1 : 2 * CP_ + (m1 - CP_);
-                                const uint64_t adesc = make_smem_desc(abase + ch0 * 2048, /*LBO*/ (uint32_t)(ch1 - ch0) * 2048, /*SBO*/ 128);
-                                const uint64_t bdesc = make_smem_desc(bbase + (C::CP + 2 * t) * (C::N * 16), /*LBO*/ C::N * 16, /*SBO*/ 128);
-                                mma_f16_ss(tmem + buf * C::N, adesc, bdesc, idesc, acc);
-                                acc = true;
-                            }
-                        }
-                        mma_commit(&acc_full[buf]);
-                        buf = (buf + 1) % C::NBUF;
-                    }
-                }
-                mma_commit(&a_empty[as]);
+            for (int r = 0; r < 2; r++) {
+                const float2 x = r ? xb[j] : xa[j];
+                const float z0 = __fmul_rn(__fsub_rn(x.x, s0), i0), z1 = __fmul_rn(__fsub_rn(x.y, s1), i1);
+                const __half2 h = __floats2half2_rn(z0, z1);
+                const float2 f = __half22float2(h);
+                zh[j][r] = *reinterpret_cast<const uint32_t*>(&h);
+                zl[j][r] = pack_half2(z0 - f.x, z1 - f.y);
             }
         }
-      }
-    } else if (warp < 8) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 72;");
-        // ===================== converters =====================
-        const int row = threadIdx.x - 128;
-        for (int it = 0; it < my_tiles; it++) {
-            const int st = it & 1, ph = (it >> 1) & 1;
-            const long long e = (long long)((int)blockIdx.x + it * (int)gridDim.x) * 128 + row;
-            float4 xv[D / 4];
-            if (e < n) {
-                const float4* xr = reinterpret_cast<const float4*>(x_aos + (size_t)e * D);
+        const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
+        if (t + stride < ntiles) load_rows(t + stride);
+
+        float lg[C::MAXSG][8];                                 // base-2 logits: [supergroup][4 clusters x 2 rows]
 #pragma unroll
-                for (int v = 0; v < D / 4; v++) xv[v] = __ldg(xr + v);
-            } else {
+        for (int sg = 0; sg < C::MAXSG; sg++) {
+            if (sg >= NSG) {
 #pragma unroll
-                for (int v = 0; v < D / 4; v++) xv[v] = make_float4(0.f, 0.f, 0.f, 0.f);
+                for (int u = 0; u < 8; u++) lg[sg][u] = -INFINITY;
+                continue;
             }
-            uint32_t hi[D / 2], lo[D / 2];
+            float sq[32];                                      // sums of squares: [cluster 0..15][row]
 #pragma unroll
-            for (int v = 0; v < D / 4; v++) {
-                const float4 t = xv[v];
-                const float4 s4 = reinterpret_cast<const float4*>(sh_s)[v], i4 = reinterpret_cast<const float4*>(isc_s)[v];
-                const float z0 = (t.x - s4.x) * i4.x, z1 = (t.y - s4.y) * i4.y;
-                const float z2 = (t.z - s4.z) * i4.z, z3 = (t.w - s4.w) * i4.w;
-                const __half2 h01 = __floats2half2_rn(z0, z1), h23 = __floats2half2_rn(z2, z3);
-                const float2 f01 = __half22float2(h01), f23 = __half22float2(h23);
-                hi[2 * v] = *reinterpret_cast<const uint32_t*>(&h01);
-                hi[2 * v + 1] = *reinterpret_cast<const uint32_t*>(&h23);
-                lo[2 * v] = pack_half2(z0 - f01.x, z1 - f01.y);
-                lo[2 * v + 1] = pack_half2(z2 - f23.x, z3 - f23.y);
-            }
-            mbar_wait_parked(&a_empty[st], ph ^ 1, 1000);
-            uint8_t* a = smem + C::OFF_A + st * C::A_STAGE + row * 16;     // K-major: [chunk][row][16 B]
+            for (int u = 0; u < 32; u++) sq[u] = 0.f;
 #pragma unroll
-            for (int c = 0; c < C::CP; c++) {                  // the constant chunks (ones, zero) were written once at kernel start
-                const uint4 h = make_uint4(hi[4 * c], hi[4 * c + 1], hi[4 * c + 2], hi[4 * c + 3]);
-                const uint4 l = make_uint4(lo[4 * c], lo[4 * c + 1], lo[4 * c + 2], lo[4 * c + 3]);
-                *reinterpret_cast<uint4*>(a + (2 * c) * 2048) = h;
-                *reinterpret_cast<uint4*>(a + (2 * c + 1) * 2048) = l;
+            for (int c = 0; c < CP; c++) {
+                const uint32_t bb = bsm + (uint32_t)(sg * CP + c) * C::B_BLOCK;
+                float acc[64];
+#pragma unroll
+                for (int u = 0; u < 64; u++) acc[u] = 0.f;
+                wgmma_fence();
+                bool accum = false;
+#pragma unroll
+                for (int j = c; j < CP; j++) {                 // (Wh_j, Wl_j) x (zh_j, zh_j)
+                    wgmma_m64n128k16_rs(acc, zh[j][0], zh[j][1], zh[j][0], zh[j][1], make_smem_desc(bb + j * CH, CP * CH, 128), accum);
+                    accum = true;
+                }
+                // (Wh_j) x (zl_j) for j >= c, then v x ones, two at a time; a lone v step pairs with a zero A chunk
+#pragma unroll
+                for (int p = c; p < CP + 1; p += 2) {
+                    const int x = p, y = p + 1;                // list items: j < CP -> Wh_j x zl_j, j == CP -> v x ones
+                    if (y <= CP) {
+                        const uint32_t yc = y < CP ? (uint32_t)y : 2u * CP;
+                        const uint32_t a2 = y < CP ? zl[y < CP ? y : 0][0] : ones, a3 = y < CP ? zl[y < CP ? y : 0][1] : ones;
+                        wgmma_m64n128k16_rs(acc, zl[x][0], zl[x][1], a2, a3, make_smem_desc(bb + x * CH, (yc - x) * CH, 128), true);
+                    } else {                                   // x == CP: v alone, paired with chunk c under a zero A chunk
+                        wgmma_m64n128k16_rs(acc, 0u, 0u, ones, ones, make_smem_desc(bb + c * CH, (2 * CP - c) * CH, 128), true);
+                    }
+                }
+                wgmma_commit();
+                wgmma_wait_all();
+#pragma unroll
+                for (int i = 0; i < 16; i++) {
+                    sq[2 * i] = fmaf(acc[4 * i], acc[4 * i], fmaf(acc[4 * i + 1], acc[4 * i + 1], sq[2 * i]));
+                    sq[2 * i + 1] = fmaf(acc[4 * i + 2], acc[4 * i + 2], fmaf(acc[4 * i + 3], acc[4 * i + 3], sq[2 * i + 1]));
+                }
             }
-            fence_proxy_async_smem();
+            // sum over the quad (the 8 columns of a cluster are spread over its 4 lanes), transposing as it goes:
+            // lane qd ends with clusters cb .. cb+3 of the supergroup, cb = 8 (qd & 1) + 4 (qd >> 1), both rows
+            float w[16];
+            const bool b1 = qd & 1, b2 = (qd >> 1) & 1;
+#pragma unroll
+            for (int u = 0; u < 16; u++) {
+                const float send = b1 ? sq[u] : sq[16 + u], keep = b1 ? sq[16 + u] : sq[u];
+                w[u] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+            }
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const float send = b2 ? w[u] : w[8 + u], keep = b2 ? w[8 + u] : w[u];
+                const float qv = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+                const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
+                lg[sg][u] = fmaf(ck_s[64 + k], qv, ck_s[k]);
+            }
+        }
+        // log-sum-exp over the clusters (estep2, gaussian_kernel.cu:481-503), per row: this lane's 16 logits, then the quad
+        float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+        for (int sg = 0; sg < C::MAXSG; sg++)
+#pragma unroll
+            for (int u = 0; u < 8; u++) mx[u & 1] = fmaxf(mx[u & 1], lg[sg][u]);
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        }
+        float scale[2] = {1.f, 1.f};
+        const long long er[2] = {e0, e1};
+        if (mode == 3) {
+            // the event's total log-denominator is known: gamma = 2^(l2 - denom * log2 e)
+            float d2[2];
+#pragma unroll
+            for (int r = 0; r < 2; r++) d2[r] = er[r] < n ? den_in[er[r]] * 1.4426950408889634f : 0.f;
+#pragma unroll
+            for (int sg = 0; sg < C::MAXSG; sg++)
+#pragma unroll
+                for (int u = 0; u < 8; u++) lg[sg][u] = ex2_approx(lg[sg][u] - d2[u & 1]);
+        } else {
+            float sm[2] = {0.f, 0.f};
+#pragma unroll
+            for (int sg = 0; sg < C::MAXSG; sg++)
+#pragma unroll
+                for (int u = 0; u < 8; u++) { lg[sg][u] = ex2_approx(lg[sg][u] - mx[u & 1]); sm[u & 1] += lg[sg][u]; }
+            float dx[2];
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                sm[r] += __shfl_xor_sync(0xffffffffu, sm[r], 1);
+                sm[r] += __shfl_xor_sync(0xffffffffu, sm[r], 2);
+                // den_in may alias den_out (running log-denominator updated in place): every lane reads before any writes
+                dx[r] = (mode != 0 && den_in != nullptr && er[r] < n) ? den_in[er[r]] : 0.f;
+            }
             __syncwarp();
-            if (lane == 0) mbar_arrive(&a_full[st]);
-        }
-    } else if (warp < 16) {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 112;");
-        // ===================== squares: accumulators -> q[event][cluster] (TMEM) =====================
-        const int sq = (warp - 8) >> 2, qd = warp & 3;
-        const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-        uint32_t pf = 0u;                                      // wait parity of acc_full[b], one bit per buffer
-        for (int it = 0; it < my_tiles; it++) {
-            const int tb = it & 1;
-            mbar_wait_parked(&q_empty[tb], ((it >> 1) & 1) ^ 1, 200);      // the previous tile in this q buffer has been read
-            tc_fence_after();
-            uint32_t buf = 0;                                  // the buffer sequence restarts with every tile (MMA issuer: same rule)
-#pragma unroll 1
-            for (int sg = 0; sg < NSG; sg++) {                 // not unrolled: the kernel's SASS has to stay inside the 32 KB L1.5 I-cache
-                {
-                    uint64_t qa[C::CW], qb[C::CW];             // packed partial sums of squares of this warpgroup's 8 clusters
 #pragma unroll
-                    for (int i = 0; i < C::CW; i++) { qa[i] = 0ull; qb[i] = 0ull; }
-#pragma unroll
-                    for (int c = 0; c < C::CP; c++) {
-                        mbar_wait_parked(&acc_full[buf], (pf >> buf) & 1u, 200);
-                        pf ^= 1u << buf;
-                        tc_fence_after();
-                        const uint32_t tcol = tmem + lane_base + buf * C::N + sq * (C::CW * 8);
-                        uint32_t v[C::CW * 8];                 // CW clusters x 8 columns
-                        tmem_ld_32x32(tcol, *reinterpret_cast<uint32_t(*)[32]>(&v[0]));
-                        tmem_ld_32x32(tcol + 32, *reinterpret_cast<uint32_t(*)[32]>(&v[32]));
-                        tmem_ld_wait();
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&acc_empty[buf]);   // the block is in registers: hand the buffer back
-                        buf = buf + 1 == C::NBUF ? 0 : buf + 1;
-#pragma unroll
-                        for (int i = 0; i < C::CW; i++) {
-                            sq_acc2(qa[i], v[i * 8 + 0], v[i * 8 + 1]);
-                            sq_acc2(qb[i], v[i * 8 + 2], v[i * 8 + 3]);
-                            sq_acc2(qa[i], v[i * 8 + 4], v[i * 8 + 5]);
-                            sq_acc2(qb[i], v[i * 8 + 6], v[i * 8 + 7]);
-                        }
-                    }
-                    uint32_t qv[C::CW];
-#pragma unroll
-                    for (int i = 0; i < C::CW; i++) qv[i] = __float_as_uint(hsum2(qa[i], qb[i]));
-                    // column of cluster (sg, sq, i) in the hand-over: tile buffer tb, warpgroup sq, then sg * 8 + i
-                    tmem_st_32x8(tmem + lane_base + C::QCOL + tb * 64 + sq * (C::MAXSG * C::CW) + sg * C::CW, qv);
-                }
-            }
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&q_full[tb]);
-        }
-    } else {
-        // ===================== log-sum-exp + stores (80 registers: the launch allocation) =====================
-        const int wg = (warp - 16) >> 2, qd = warp & 3;
-        const int row = qd * 32 + lane;
-        const uint32_t lane_base = (uint32_t)(qd * 32) << 16;
-        double ll_acc = 0.0;
-        constexpr float kLn2 = 0.6931471805599453f;
-        for (int it = 0; it < my_tiles; it++) {
-            const int tb = it & 1;
-            const long long e = (long long)((int)blockIdx.x + it * (int)gridDim.x) * 128 + row;
-            // q, then base-2 logits, then 2^(logit - max), as PACKED pairs of neighbouring clusters (fma / add / mul .f32x2:
-            // half the instructions and FMA-pipe cycles of this stage; the pipe is shared with the squares)
-            uint64_t lgp[C::LPT / 2];
-            mbar_wait_parked(&q_full[tb], (it >> 1) & 1, 200);
-            tc_fence_after();
-            {
-                uint32_t qraw[C::LPT];
-                tmem_ld_32x32(tmem + lane_base + C::QCOL + tb * 64 + wg * C::LPT, qraw);
-                tmem_ld_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&q_empty[tb]);
-#pragma unroll
-                for (int sg = 0; sg < C::MAXSG; sg++) {
-                    if (sg < NSG) {
-                        const float4* cp = reinterpret_cast<const float4*>(ck_s + sg * C::GB + wg * C::CW);
-                        const float4* mp = reinterpret_cast<const float4*>(ck_s + 64 + sg * C::GB + wg * C::CW);
-                        const float4 c0 = cp[0], c1 = cp[1], m0 = mp[0], m1 = mp[1];
-                        const int j = sg * C::CW;
-                        lgp[j / 2 + 0] = ffma2(pack2f(m0.x, m0.y), pack2u(qraw[j + 0], qraw[j + 1]), pack2f(c0.x, c0.y));
-                        lgp[j / 2 + 1] = ffma2(pack2f(m0.z, m0.w), pack2u(qraw[j + 2], qraw[j + 3]), pack2f(c0.z, c0.w));
-                        lgp[j / 2 + 2] = ffma2(pack2f(m1.x, m1.y), pack2u(qraw[j + 4], qraw[j + 5]), pack2f(c1.x, c1.y));
-                        lgp[j / 2 + 3] = ffma2(pack2f(m1.z, m1.w), pack2u(qraw[j + 6], qraw[j + 7]), pack2f(c1.z, c1.w));
-                    } else {                                   // columns of unused supergroups are not written
-#pragma unroll
-                        for (int u = 0; u < C::CW / 2; u++) lgp[sg * C::CW / 2 + u] = pack2f(-INFINITY, -INFINITY);
-                    }
-                }
-            }
-            float mx = -INFINITY;
-#pragma unroll
-            for (int u = 0; u < C::LPT / 2; u++) { mx = fmaxf(mx, lo2f(lgp[u])); mx = fmaxf(mx, hi2f(lgp[u])); }
-            float scale;
-            if (mode == 3) {
-                // the event's total log-denominator is known: gamma = 2^(l2 - denom * log2 e)
-                const float d2 = e < n ? den_in[e] * 1.4426950408889634f : 0.f;
-                const uint64_t nd = pack2f(-d2, -d2);
-#pragma unroll
-                for (int u = 0; u < C::LPT / 2; u++) {
-                    const uint64_t t2 = fadd2(lgp[u], nd);
-                    lgp[u] = pack2f(ex2_approx(lo2f(t2)), ex2_approx(hi2f(t2)));
-                }
-                scale = 1.0f;
-            } else {
-                // log-sum-exp over the clusters (estep2, gaussian_kernel.cu:481-503): local part, then the two warpgroups combine
-                const uint64_t nm = pack2f(-mx, -mx);
-                uint64_t s0 = 0ull, s1 = 0ull;                       // two packed running sums (four independent chains)
-#pragma unroll
-                for (int u = 0; u < C::LPT / 2; u++) {
-                    const uint64_t t2 = fadd2(lgp[u], nm);
-                    lgp[u] = pack2f(ex2_approx(lo2f(t2)), ex2_approx(hi2f(t2)));
-                    if (u & 1) s1 = fadd2(s1, lgp[u]); else s0 = fadd2(s0, lgp[u]);
-                }
-                const uint64_t s2 = fadd2(s0, s1);
-                const float sm = lo2f(s2) + hi2f(s2);
-                float2* exb = ex + (it & 1) * (NWG * 128);
-                exb[wg * 128 + row] = make_float2(mx, sm);
-                // den_in may alias den_out (running log-denominator updated in place by warpgroup 0): both warpgroups read
-                // it BEFORE the barrier, the write comes after
-                const float dx = (mode != 0 && den_in != nullptr && e < n) ? den_in[e] : 0.f;
-                named_bar_sync(1, NWG * 128);
-                const float2 o = exb[(wg ^ 1) * 128 + row];
-                const float M = fmaxf(mx, o.x);
-                const float own = ex2_approx(mx - M);
-                const float S = sm * own + o.y * ex2_approx(o.x - M);
-                float denom = fmaf(M, kLn2, logf(S));                // :490-494, back in natural units
-                scale = own / S;                                     // exp(l - denom) = 2^(l2 - mx) * 2^(mx - M) / S
-                if (mode != 0 && e < n) {
-                    if (den_in != nullptr) {                         // join with the other passes' log-denominator
-                        const float g = fmaxf(denom, dx);
-                        const float tot = g + logf(__expf(denom - g) + __expf(dx - g));
-                        scale *= __expf(denom - tot);
+            for (int r = 0; r < 2; r++) {
+                float denom = fmaf(mx[r], kLn2, logf(sm[r]));      // :490-494, back in natural units
+                scale[r] = 1.0f / sm[r];                            // exp(l - denom) = 2^(l2 - M) / S
+                if (mode != 0 && er[r] < n) {
+                    if (den_in != nullptr) {                        // join with the other passes' log-denominator
+                        const float g = fmaxf(denom, dx[r]);
+                        const float tot = g + logf(__expf(denom - g) + __expf(dx[r] - g));
+                        scale[r] *= __expf(denom - tot);
                         denom = tot;
                     }
-                    if (wg == 0) den_out[e] = denom;
+                    if (qd == 0) den_out[er[r]] = denom;
                 }
-                if (wg == 0 && e < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
-            }
-            if (e < n && mode != 1) {
-                // Rows [K, 8*ceil(K/8)) are written too (zeros of the padding clusters): the buffer is allocated in
-                // multiples of 8 rows, which keeps the 8 stores of a group unpredicated.
-                float* gp = memb + (size_t)(wg * C::CW) * pitch + e;      // row of this warpgroup's first cluster
-                const uint64_t sc2 = pack2f(scale, scale);
-#pragma unroll
-                for (int sg = 0; sg < C::MAXSG; sg++) {
-                    if (sg * C::GB + wg * C::CW < K) {
-                        float* gq = gp + (size_t)(sg * C::GB) * pitch;
-#pragma unroll
-                        for (int u = 0; u < C::CW / 2; u++) {
-                            const uint64_t g2 = fmul2(lgp[sg * C::CW / 2 + u], sc2);      // :498-501
-                            gq[0] = lo2f(g2);
-                            gq[pitch] = hi2f(g2);
-                            gq += 2 * pitch;
-                        }
-                    }
-                }
+                if (qd == 0 && er[r] < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
             }
         }
-        if (wg == 0 && (mode == 0 || mode == 2)) {
-            ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 16);
-            ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 8);
-            ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 4);
-            ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 2);
-            ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 1);
-            if (lane == 0) atomicAdd(ll_out, ll_acc);
+        if (mode != 1) {
+            // Rows [K, 8*ceil(K/8)) are written too (zeros of the padding clusters): the buffer is allocated in
+            // multiples of 8 rows.
+#pragma unroll
+            for (int sg = 0; sg < C::MAXSG; sg++) {
+#pragma unroll
+                for (int u = 0; u < 8; u++) {
+                    const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
+                    const long long e = er[u & 1];
+                    if (sg < NSG && (k & ~7) < K && e < n) memb[(size_t)k * pitch + e] = lg[sg][u] * scale[u & 1];   // :498-501
+                }
+            }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc<512>(tmem);
+    if (mode == 0 || mode == 2) {
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 16);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 8);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 4);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 2);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 1);
+        if (lane == 0) atomicAdd(ll_out, ll_acc);
+    }
 }
 
 // ---------------------------------------------------------------------------
@@ -885,7 +715,7 @@ struct TcState {
     float* d_z_soa = nullptr;        // [D][memb_pitch] centred/scaled SoA copy (M-step TMA source)
     float* d_memb = nullptr;
     size_t memb_pitch = 0;
-    int n = 0, D = 0, Kmax = 0, num_sms = 148;
+    int n = 0, D = 0, Kmax = 0, num_sms = 132;
     CUtensorMap tm_x{}, tm_g{};
     bool maps_ok = false;
     float* d_shift_f = nullptr;      // [32]
@@ -1162,7 +992,7 @@ static int bimg_cluster(TcState* t, const clusters_t* host, int k, int K, const 
             double v = 0.0;
             for (int j = 0; j < D; j++) {
                 const double w = (j >= d) ? Gc[j][d] : 0.0;
-                v -= w * ((double)host->means[(size_t)k * D + j] - t->h_shift[j]);
+                v = std::fma(-w, (double)host->means[(size_t)k * D + j] - t->h_shift[j], v);   // finalize_params_kernel: the same fused steps
                 wrow[d][j] = (float)(w * t->h_scale[j]);
                 amax = std::fmax(amax, std::fabs(wrow[d][j]));
             }
@@ -1204,7 +1034,7 @@ static int bimg_cluster(TcState* t, const clusters_t* host, int k, int K, const 
             if (C::NCHKB > 2 * C::CP + 1) std::memset(rowp(d, 2 * C::CP + 1), 0, 16);
         }
         float* ckp = t->h_ck + (size_t)(k / 64) * 128 + (k % 64);
-        ckp[0] = host->constant[k] + logf(host->pi[k]);      // additive term of estep1 (gaussian_kernel.cu:442)
+        ckp[0] = host->constant[k] + (float)std::log((double)host->pi[k]);   // additive term of estep1 (gaussian_kernel.cu:442); ln pi in double, as on the device
         ckp[64] = (float)std::ldexp(-0.5 * 1.4426950408889634, -2 * e2);
     }
     return bad;
@@ -1270,11 +1100,10 @@ int tc_upload_params(TcState* t, const clusters_t* host, int K, cudaStream_t str
 // and the next E-step — N, means, R (gaussian.cu:611-622, 663-679 with the rules of mstep_covariance1,
 // gaussian_kernel.cu:658-675), inverse + constant + pi (constants_kernel, :172-259) and the E-step's resident
 // operand (bimg_cluster above) — so that an EM iteration needs no device -> host -> device round trip
-// (D2H of the statistics, thread-team wake-up, H2D of the operand: 60 us of an iteration that is 3.1 ms on one GPU
-// and 0.6 ms on eight).  Same arithmetic as host_math.cpp (double, results stored as float): reverse Cholesky
-// R = U U^T, W = U^-1, Rinv = W^T W, ln det R = 2 sum ln U_ii, here with a right-looking factorisation (rank-1
-// updates of the trailing block, all threads) — the summation order differs from the host's dot products in the
-// last bit of a double.  A cluster the host would NOT serve this way (R not positive definite, factor outside FP16)
+// (D2H of the statistics, thread-team wake-up, H2D of the operand).  The same operations in the same order as
+// host_math.cpp (double, results stored as float): reverse Cholesky R = U U^T, W = U^-1, Rinv = W^T W,
+// ln det R = 2 sum ln U_ii, so that the device and the host finalisation produce bit-identical parameter sets and
+// E-step operands (EM amplifies any last-bit difference between the two).  A cluster the host would NOT serve this way (R not positive definite, factor outside FP16)
 // is not handled here: the kernel records the iteration in bad[0] (first failure wins), every later launch returns
 // immediately, and the host replays from the last good parameter set through its own path (gmm_api.cu).
 // Parameter set layout (floats, stride Kmax): N | pi | constant | means [Kmax][D] | R [Kmax][D][D] | Rinv [Kmax][D][D].
@@ -1297,11 +1126,9 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
                        const double* __restrict__ scale, float* __restrict__ set, int Kmax, int K, int kp,
                        uint8_t* __restrict__ bimg, float* __restrict__ ck, double* __restrict__ ll_out, int* __restrict__ bad, int iter,
                        int fault_iter) {
-    // Latency-bound by construction (one CTA works through a 24 x 24 factorisation, 64 CTAs on 148 SMs; dependent FP64 operations
-    // cost ~45 cycles each here — build-time phase stamps, GMM_FIN_PROF): one global round trip (the cluster's statistics row is staged
-    // in shared memory), a THREAD PER MATRIX ELEMENT so that the rank-1 update of a column / row step is one pass (three serial passes of
-    // 256 threads cost 880 cycles per column), one barrier per column of the factorisation and per row of the triangular inverse, and a
-    // reciprocal square root of the pivot from the FP32 approximation + one Newton step (relative error ~1e-13: the results are stored as floats).
+    // Latency-bound by construction (one CTA works through a 24 x 24 factorisation, 64 CTAs on 132 SMs): one global round trip
+    // (the cluster's statistics row is staged in shared memory), then the host's factorisation and inverse with a thread per row /
+    // column (see below), and a thread per matrix element for everything else.
 #ifdef GMM_FIN_PROF
     long long fin_t[10];
 #endif
@@ -1323,7 +1150,7 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
         return;
     }
     FIN_STAMP(0);
-    __shared__ double sS[F + 3], sA[D][LD], sU[D][LD], sW[D][LD], srd[D], spiv[D], sdm[D], sscale[D], svd[D], sredd[NW];
+    __shared__ double sS[F + 3], sA[D][LD], sU[D][LD], sW[D][LD], sdm[D], sscale[D], svd[D], sredd[NW];
     __shared__ float swr[D][LD], sredf[NW];
     __shared__ int sbad;
     // ---- stage: the statistics row, the S0 of every cluster (pi), shift / scale ----
@@ -1382,19 +1209,23 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
     }
     __syncthreads();
     FIN_STAMP(2);
-    // ---- R = U U^T from the last column: ONE barrier per column.  sA keeps the unscaled trailing block (upper triangle),
-    //      the scaled column goes to sU, its reciprocal pivot to srd, the pivot's square to spiv (ln det) ----
+    // ---- R = U U^T from the last column (reverse Cholesky), then W = U^-1: the operations and their order of
+    //      constants_cluster_spd (host_math.cpp), every product rounded before it is subtracted (__dmul_rn / __dsub_rn,
+    //      as the host is compiled), correctly rounded sqrt and division — the device and the host finalisation give
+    //      bit-identical factors.  Column j: thread i <= j forms its dot product over the finished columns m > j
+    //      (thread j's is the pivot, which every thread recomputes), ONE barrier per column ----
     bool ok = true;
     for (int j = D - 1; j >= 0; j--) {
-        const double d = sA[j][j];
+        double d = sA[j][j];
+        for (int m = j + 1; m < D; m++) d = __dsub_rn(d, __dmul_rn(sU[j][m], sU[j][m]));
         if (!(d > 0.0) || !isfinite(d)) { ok = false; break; }    // the same value in every thread
-        const double y0 = (d > 1e-30 && d < 1e30) ? (double)rsqrtf((float)d) : rsqrt(d);   // 22 bits (float range), else the full routine
-        const double rp = y0 * fma(-0.5 * d, y0 * y0, 1.5), invd = rp * rp;
-        if (tid < j) sU[tid][j] = sA[tid][j] * rp;
-        else if (tid == j) { srd[j] = rp; spiv[j] = d; }
-        for (int idx = tid; idx < D * D; idx += T) {            // (i, m) with i <= m < j:  A[i][m] -= A[i][j] A[m][j] / d
-            const int i = idx / D, m = idx % D;
-            if (i <= m && m < j) sA[i][m] -= sA[i][j] * sA[m][j] * invd;
+        const double piv = sqrt(d), rp = 1.0 / piv;
+        if (tid < j) {
+            double v = sA[tid][j];
+            for (int m = j + 1; m < D; m++) v = __dsub_rn(v, __dmul_rn(sU[tid][m], sU[j][m]));
+            sU[tid][j] = __dmul_rn(v, rp);
+        } else if (tid == j) {
+            sU[j][j] = piv;
         }
         __syncthreads();
     }
@@ -1403,21 +1234,18 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
         return;
     }
     FIN_STAMP(3);
-    // ---- W = U^-1 (upper triangular), row by row from the bottom, ONE barrier per row: when row m is final, every row i < m
-    //      takes its term U[i][m] W[m][j]; the thread that completes row m - 1 scales it (W[i][j] = -(sum) / U[i][i]) ----
-    if (tid < D) sW[tid][tid] = srd[tid];
-    __syncthreads();
-    for (int m = D - 1; m >= 1; m--) {
-        for (int idx = tid; idx < D * D; idx += T) {
-            const int i = idx / D, j = idx % D;
-            if (i < m && j >= m) {
-                double acc = sW[i][j] + sU[i][m] * sW[m][j];
-                if (i == m - 1) acc = -acc * srd[i];
-                sW[i][j] = acc;
-            }
+    // ---- W = U^-1 (upper triangular), a thread per column j: W[i][j] = -(sum_{m=i+1..j} U[i][m] W[m][j]) / U[i][i] ----
+    if (tid < D) {
+        const int j = tid;
+        for (int i = D - 1; i > j; i--) sW[i][j] = 0.0;
+        sW[j][j] = 1.0 / sU[j][j];
+        for (int i = j - 1; i >= 0; i--) {
+            double v = 0.0;
+            for (int m = i + 1; m <= j; m++) v = __dsub_rn(v, __dmul_rn(sU[i][m], sW[m][j]));
+            sW[i][j] = v / sU[i][i];
         }
-        __syncthreads();
     }
+    __syncthreads();
     FIN_STAMP(4);
     // ---- Rinv = W^T W, ln det, constant (gaussian_kernel.cu:241), N, pi; operand rows: W'[d][j] = W[d][j] * scale_j, v = -W (mu - shift) ----
     {
@@ -1427,7 +1255,7 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
             if (j < i) continue;
             double v = 0.0;
 #pragma unroll 4
-            for (int m = 0; m <= i; m++) v += sW[m][i] * sW[m][j];
+            for (int m = 0; m <= i; m++) v = __dadd_rn(v, __dmul_rn(sW[m][i], sW[m][j]));
             Ri[i * D + j] = (float)v; Ri[j * D + i] = (float)v;
         }
     }
@@ -1443,22 +1271,21 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
         const int d = tid - 64;
         double v = 0.0;
 #pragma unroll 4
-        for (int j = d; j < D; j++) v -= sW[d][j] * sdm[j];
+        for (int j = d; j < D; j++) v = fma(-sW[d][j], sdm[j], v);     // bimg_cluster: the same fused steps
         svd[d] = v;
         amax = fmaxf(amax, (float)fabs(v));
     }
-    double ld2 = (tid >= 32 && tid < 32 + D) ? log(spiv[tid - 32]) : 0.0;   // ln det R = sum ln (pivot^2)
-    if (tid >= 32 && tid < 64) {
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) ld2 += __shfl_xor_sync(0xffffffffu, ld2, o);
-        if (tid == 32) sredd[0] = ld2;
+    if (tid == 32) {                                           // sum ln U_jj in the host's order
+        double ld = 0.0;
+        for (int j = D - 1; j >= 0; j--) ld += log(sU[j][j]);
+        sredd[0] = ld;
     }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
     if ((tid & 31) == 0) sredf[tid >> 5] = amax;
     __syncthreads();
     FIN_STAMP(6);
-    const double ld = 0.5 * sredd[0];                          // sum ln U_jj
+    const double ld = sredd[0];                                // sum ln U_jj
     const float cst = (float)(-D * 0.5 * log(2.0 * 3.1415926535897931) - 0.5 * (2.0 * ld));
     if (tid == 0) { set[k] = Nf; set[Kmax + k] = pik; set[2 * (size_t)Kmax + k] = cst; }
     amax = 0.f;
@@ -1497,7 +1324,7 @@ finalize_params_kernel(const double* __restrict__ stats, const float* __restrict
         if (C::NCHKB > 2 * C::CP + 1) *reinterpret_cast<uint4*>(rowp(d, 2 * C::CP + 1)) = make_uint4(0u, 0u, 0u, 0u);
     }
     if (tid == 0) {
-        ckp[0] = cst + logf(pik);                              // additive term of estep1 (gaussian_kernel.cu:442)
+        ckp[0] = cst + (float)log((double)pik);                // additive term of estep1 (gaussian_kernel.cu:442); ln pi as on the host
         ckp[64] = (float)ldexp(-0.5 * 1.4426950408889634, -2 * e2);
     }
     __syncthreads();
@@ -1590,7 +1417,6 @@ template <int D>
 static int launch_mstep_d(TcState* t, int K, double* d_stats, cudaStream_t stream) {
     using C = MCfg<D>;
     static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
-    static_assert(C::TMEM_COLS <= 512, "TMEM budget");
     if (!t->attr_mstep) {
         TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_mstep = true;
@@ -1602,7 +1428,7 @@ static int launch_mstep_d(TcState* t, int K, double* d_stats, cudaStream_t strea
     const int gy = (K + kNCL - 1) / kNCL;
     if ((size_t)gx * gy * C::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
     dim3 grid(gx, gy);
-    mstep_tc_kernel<D><<<grid, kMThreads, C::SMEM_BYTES, stream>>>(t->tm_x, t->tm_g, t->n, t->d_scratch, per, t->magic);
+    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(t->tm_x, t->tm_g, t->n, t->d_scratch, per, t->magic);
     TC_CUDA_TRY(cudaGetLastError());
     mstep_tc_finalize_kernel<<<C::NCHUNK * 8, 256, 0, stream>>>(t->d_scratch, gx, C::MT, K, C::F, t->d_rowmap, t->d_scale, d_stats);
     TC_CUDA_TRY(cudaGetLastError());

@@ -1,4 +1,4 @@
-// kernels_tc.cuh — tcgen05 (5th-generation tensor core) path of the EM hot
+// kernels_tc.cuh — warpgroup-MMA (wgmma) tensor-core path of the EM hot
 // path.  Interface used by gmm_api.cu; implementation in kernels_tc.cu.
 #pragma once
 #include <cuda_runtime.h>

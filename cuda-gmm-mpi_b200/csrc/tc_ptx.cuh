@@ -1,8 +1,7 @@
-// tc_ptx.cuh — thin inline-PTX wrappers for the Blackwell (sm_100a) features the
-// tensor-core kernels use: mbarrier, TMA bulk copies (cp.async.bulk -> UBLKCP),
-// TMEM allocation, tcgen05.mma / commit / ld, proxy fences.  Descriptor bit
-// layouts follow the PTX ISA "matrix descriptor" / "instruction descriptor"
-// tables (cross-checked against cute/arch/mma_sm100_desc.hpp).
+// tc_ptx.cuh — thin inline-PTX wrappers for the Hopper (sm_90a) features the
+// tensor-core kernels use: mbarrier, TMA bulk copies (cp.async.bulk), warpgroup
+// MMA (wgmma.mma_async / fence / commit / wait), proxy fences.  Descriptor bit
+// layouts follow the PTX ISA "matrix descriptor" table of wgmma.
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -63,47 +62,8 @@ __device__ __forceinline__ void mbar_wait_parked(uint64_t* bar, uint32_t parity,
             : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity), "r"(ns) : "memory");
     }
 }
-// packed FP32 pair: acc.xy += y.xy * y.xy   (SASS: FFMA2)
-__device__ __forceinline__ void sq_acc2(uint64_t& acc, uint32_t y_lo, uint32_t y_hi) {
-    uint64_t y;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(y) : "r"(y_lo), "r"(y_hi));
-    asm("fma.rn.f32x2 %0, %1, %1, %0;" : "+l"(acc) : "l"(y));
-}
-__device__ __forceinline__ float hsum2(uint64_t a, uint64_t b) {   // (a.x + a.y) + (b.x + b.y)
-    uint64_t s;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(s) : "l"(a), "l"(b));
-    float lo, hi;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(s));
-    return lo + hi;
-}
-
-// packed FP32 pairs (fma / add / mul .f32x2: SASS FFMA2 / FADD2 / FMUL2)
-__device__ __forceinline__ uint64_t pack2u(uint32_t lo, uint32_t hi) {
-    uint64_t r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "r"(lo), "r"(hi));
-    return r;
-}
-__device__ __forceinline__ uint64_t pack2f(float lo, float hi) { return pack2u(__float_as_uint(lo), __float_as_uint(hi)); }
-__device__ __forceinline__ float lo2f(uint64_t v) { return __uint_as_float((uint32_t)v); }
-__device__ __forceinline__ float hi2f(uint64_t v) { return __uint_as_float((uint32_t)(v >> 32)); }
-__device__ __forceinline__ uint64_t ffma2(uint64_t a, uint64_t b, uint64_t c) {
-    uint64_t r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ uint64_t fadd2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ uint64_t fmul2(uint64_t a, uint64_t b) {
-    uint64_t r;
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-
 // ---- proxy fences -----------------------------------------------------------
-// Generic-proxy shared-memory writes -> visible to the async proxy (TMA, tcgen05.mma operands).
+// Generic-proxy shared-memory writes -> visible to the async proxy (TMA, wgmma operands).
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -116,26 +76,12 @@ __device__ __forceinline__ void tma_load_1d(void* smem_dst, const void* gmem_src
         ::"r"(smem_u32(smem_dst)), "l"(gmem_src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
 
-// ---- TMEM -------------------------------------------------------------------
-// ncols: power of two in [32, 512].  Executed by one full warp.
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)), "n"(NCOLS) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
 // ---- descriptors ------------------------------------------------------------
-// Shared-memory matrix descriptor, SWIZZLE_NONE ("interleaved" core-matrix layout):
+// Shared-memory matrix descriptor of wgmma, no swizzle ("interleaved" core-matrix layout):
 //   bits [0,14)  start address >> 4
 //   bits [16,30) leading-dimension byte offset >> 4  (distance between core matrices adjacent in K)
 //   bits [32,46) stride-dimension byte offset >> 4   (distance between core matrices adjacent in M/N)
-//   bits [46,48) descriptor version = 1 (Blackwell);  bits [61,64) layout type = 0 (no swizzle)
+//   bits [49,52) base offset = 0;  bits [62,64) layout type = 0 (no swizzle)
 // A core matrix is 8 rows x 16 bytes, stored as 128 contiguous bytes.
 //   K-major  operand: element (r, k)  at (r/8)*SBO + (k_bytes/16)*LBO + (r%8)*16 + k_bytes%16
 //   MN-major operand: element (mn, k) at (mn_bytes/16)*SBO + (k/8)*LBO + (k%8)*16 + mn_bytes%16
@@ -144,75 +90,53 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
     return d;
 }
-// Instruction descriptor for kind::f16 (A, B fp16; D fp32):
-//   [4,6) D format (1 = F32)  [7,10) A format (0 = F16)  [10,13) B format (0 = F16)
-//   [15] A major (1 = MN-major)  [16] B major (1 = MN-major)  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N, bool a_mn_major, bool b_mn_major) {
-    return (1u << 4) | (0u << 7) | (0u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
 
-// D[tmem] (+)= A[smem] * B[smem]; issued by ONE thread.
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, bool accumulate) {
+// ---- warpgroup MMA ------------------------------------------------------------
+// Accumulator fragment of an m64nN f32 result, thread t of the warpgroup (warp w = t/32, lane l):
+//   d[i] -> row 16w + l/4 + 8*((i/2)%2), column 8*(i/4) + 2*(l%4) + i%2
+// A fragment from registers (f16, m64k16): a0 = row l/4 cols {2q, 2q+1}, a1 = row l/4+8 same cols,
+//   a2 / a3 = the same rows at cols {8+2q, 9+2q}   (rows offset by 16w, q = l%4)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// D[64 x 128] (+)= A[64 x 16] (registers, K-major fragments) * B[16 x 128] (shared memory, K-major); one warpgroup.
+__device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc, bool accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]: the A operand (M = 128 rows = TMEM lanes, K-major: two FP16 per 32-bit column, 8 columns per
-// K = 16 step) is read from tensor memory instead of shared memory.
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, bool accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"((uint32_t)accumulate) : "memory");
-}
-// Arrive on an mbarrier when all previously issued MMAs of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"((uint32_t)accumulate));
 }
 
-// TMEM -> registers: 32 lanes x 32 columns (one column per register, lane = thread).
-// taddr: lane base in bits [31:16] (must be the warp's quadrant 32*(warp%4)), column in [15:0].
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
+// D[64 x 64] += A[64 x 16] * B[16 x 64], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
+__device__ __forceinline__ void wgmma_m64n64k16_ss_tn(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-          "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-          "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr) : "memory");
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
+
+// D[64 x 32] += A[64 x 16] * B[16 x 32], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
+__device__ __forceinline__ void wgmma_m64n32k16_ss_tn(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
     asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, 1, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "%16, %17, p, 1, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(a_desc), "l"(b_desc));
 }
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-        : "r"(taddr) : "memory");
-}
-// registers -> TMEM: 32 lanes x 8 columns
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&r)[8]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]) : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
@@ -236,10 +160,6 @@ __device__ __forceinline__ float ex2_approx(float x) {
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
     return r;
-}
-
-__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
 
 }}  // namespace gmm::ptx

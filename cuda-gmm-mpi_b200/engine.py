@@ -37,7 +37,7 @@ def library_path():
 
 
 def build_library(force=False):
-    """Compile csrc/ for sm_100a (nvcc cross-compiles without a GPU)."""
+    """Compile csrc/ for sm_90a (nvcc cross-compiles without a GPU)."""
     args = ["make", "-s", "-C", os.path.join(_HERE, "csrc"), "-j8"]
     if force:
         subprocess.check_call(args[:4] + ["clean"])

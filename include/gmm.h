@@ -1,5 +1,5 @@
 /*
- * gmm.h — C ABI of the B200-native GMM-EM engine (libgmm_b200.so).
+ * gmm.h — C ABI of the H100-native GMM-EM engine (libgmm_b200.so).
  *
  * This is the drop-in boundary for the hot path of Corv/CUDA-GMM-MPI.  The
  * reference has no plugin/FFI layer: its seven kernels are #included into the
@@ -7,7 +7,7 @@
  * boundary a maintainer can bind is therefore (1) the clusters_t / events
  * memory layout, (2) the operator granularity of the kernels, (3) the CLI.
  * Every entry point below names the reference code it replaces (file:line in
- * /root/reference).
+ * the reference repository).
  *
  * Conventions
  *   - extern "C", plain pointers and sizes; no torch / CUDA types.
@@ -19,7 +19,7 @@
  *     not re-entrant; different ctxs may be driven from different threads or
  *     processes.  Multi-GPU = one ctx per GPU joined by gmm_comm_init().
  *   - There is NO CPU fallback: every compute entry point fails with
- *     GMM_ERR_CUDA when no sm_100 device is usable.
+ *     GMM_ERR_CUDA when no sm_90 device is usable.
  */
 #ifndef GMM_B200_H
 #define GMM_B200_H
@@ -63,7 +63,7 @@ enum {
 /* E/M-step implementation selector (gmm_set_option "path").               */
 #define GMM_PATH_AUTO   0   /* tensor-core path when the shape allows it    */
 #define GMM_PATH_SIMT   1   /* FP32/FP64 CUDA-core kernels                  */
-#define GMM_PATH_TENSOR 2   /* tcgen05 kernels (fails if shape unsupported) */
+#define GMM_PATH_TENSOR 2   /* wgmma kernels (fails if shape unsupported) */
 
 const char* gmm_last_error(void);
 const char* gmm_version(void);

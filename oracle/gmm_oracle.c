@@ -10,15 +10,15 @@
  * (SURVEY.md §4) and its EM exists only as CUDA kernels, so it cannot run in
  * the (GPU-less) build container.  The oracle is pinned by
  *   (1) the fixtures in tests/golden/ref_c1_*, produced by the UNMODIFIED
- *       reference sources compiled for sm_100a (oracle/Makefile target `ref`,
- *       oracle/ref_wrapper.cu) and run on a B200 by tests/golden/make_ref_golden.sh;
+ *       reference sources compiled for sm_90a (oracle/Makefile target `ref`,
+ *       oracle/ref_wrapper.cu) and run on an H100 by tests/golden/make_ref_golden.sh;
  *   (2) an independent cross-check against scikit-learn's GaussianMixture
  *       M-step/E-step (tests/test_oracle.py).
  * Until (1) has been generated the header of tests/golden/README.md says
  * "parity unpinned".
  *
  * Every function cites the reference file:line it follows (paths relative to
- * /root/reference).  The arithmetic ORDER of the reference's block/thread
+ * the reference repository).  The arithmetic ORDER of the reference's block/thread
  * decomposition is restated literally where it affects FP32 results
  * (strided per-thread partial sums, butterfly reduction, thread-0 serial sum).
  *

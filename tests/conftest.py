@@ -10,7 +10,7 @@ import __graft_entry__ as entry  # noqa: E402
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a GPU machine)")
 
 
 @pytest.fixture(scope="session")

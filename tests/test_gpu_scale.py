@@ -1,4 +1,4 @@
-"""GPU parity tests beyond one operator on one small input (run with -m gpu on a B200):
+"""GPU parity tests beyond one operator on one small input (run with -m gpu on an H100):
 
 * gmm_em_iterations (the unit bench.py times) against the oracle's EM, from every state it can be entered in;
 * the sharded path through the C ABI — one gmm_ctx per GPU driven from one host thread each, joined by the

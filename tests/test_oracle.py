@@ -1,7 +1,7 @@
 """CPU tests of the oracle itself (oracle/gmm_oracle.c): invariants, agreement of
 the FP32 (reference arithmetic) and FP64 builds, an independent cross-check
 against scikit-learn, and the golden fixtures produced by the unmodified
-reference on a B200 (tests/golden/, when present)."""
+reference on an H100 (tests/golden/, when present)."""
 import os
 
 import numpy as np
@@ -175,7 +175,7 @@ def _parse_summary(path):
                     reason="golden fixtures from the reference binary not generated yet (parity unpinned)")
 def test_oracle_matches_reference_golden(pkg, oracle64, oracle32):
     """tests/golden/ref_c1.* were written by the UNMODIFIED reference program
-    (oracle/_ref/gaussianMPI_ref, built by oracle/Makefile `ref`) on a B200:
+    (oracle/_ref/gaussianMPI_ref, built by oracle/Makefile `ref`) on an H100:
     K=8 on the config-1 data set (N=10k, D=4), GMM_REF_ITERS iterations, target 8."""
     meta = dict(l.strip().split("=") for l in open(os.path.join(GOLDEN, "ref_c1.meta")))
     iters, K = int(meta["iters"]), int(meta["K"])
