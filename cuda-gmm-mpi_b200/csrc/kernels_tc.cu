@@ -24,8 +24,10 @@
 //                                                       g is below the quantum; ~1 % of the magnitude, its truncation
 //                                                       bias is 1e-8 of the statistic
 // The raw-moment cancellation |mu - shift|^2 / sigma^2 ~ 100 multiplies unbiased rounding noise only.
-// With B = [gh ; gl] stacked as ONE N = 64 operand, ph x [gh ; gl] is a single MMA that fills both column groups;
-// pl x gs (N = 32) adds into the second group.
+// Each column group is its own N = 32 accumulator: ph x gh into the exact one, then ph x gl and pl x gs into the
+// remainder one.  All MMAs of a consumer have the same shape and no two accumulators overlap, so ptxas keeps the
+// wgmma of a sub-tile in flight together (an N = 64 MMA filling both groups plus an N = 32 MMA into its upper half
+// made it wait for every MMA before issuing the next, C7511).
 //
 // Dataflow per CTA (persistent over a contiguous range of events, 32 clusters per CTA row of the grid):
 //   warp 0      TMA producer: tile [D][32 events] of the pre-standardised SoA copy z and raw
@@ -33,8 +35,9 @@
 //               the latter, zero fill out of bounds)
 //   warps 4-11  operand builders (two warpgroups on alternate tiles): form the products, split
 //               them, write the wgmma operand images (no-swizzle core-matrix layout)
-//   warpgroups 3 .. 2+MT  consumers, one per 128-row feature tile: per 32 events 2 x 2 x (m64n64k16 + m64n32k16)
-//               wgmma with the accumulators in registers.  The exact group is drained every 128 events and the
+//   warpgroups 3 .. 2+MT  consumers, one per 128-row feature tile: per 32 events 2 x 2 x 3 m64n32k16 wgmma, committed
+//               as one group, with the accumulators in registers; a sub-tile's group is still running while the next
+//               sub-tile's MMAs are issued (three operand stages).  The exact group is drained every 128 events and the
 //               remainder group every 512 into FP32 round-to-nearest partial sums held in shared memory (one private
 //               slot per thread), written ONCE per CTA (no scratch zeroing, no atomics).
 // A second tiny kernel reduces the per-CTA partials in double and un-scales.
@@ -73,7 +76,7 @@ using namespace ptx;
 // ---------------------------------------------------------------------------
 constexpr int kTE = 32;          // events per sub-tile (MMA K extent per operand part)
 constexpr int kNCL = 32;         // clusters per CTA pass (N of the exact / remainder groups: register budget of the consumers)
-constexpr int kNST = 2;          // operand stages
+constexpr int kNST = 3;          // operand stages: one read by the in-flight MMAs, one built by each builder warpgroup
 constexpr int kNRAW = 4;         // raw (TMA) stages
 constexpr int kChunkSub = 4;     // sub-tiles per chain of the exact column group: 128 events (the bit budget below)
 constexpr int kChunkSub2 = 16;   // sub-tiles per chain of the remainder column group (no exactness to protect: drained 4x less often)
@@ -104,10 +107,13 @@ template <int D> struct MCfg {
     static constexpr int CPP = (RPP + 7) / 8;             // 16-byte chunks per warp
     static constexpr int NCHUNK = 4 * CPP;                // chunks written per event
     static constexpr int MT = (NCHUNK * 8 + 127) / 128;   // M tiles of 128 feature rows
-    static constexpr int PHI_PART = MT * 128 * kTE * 2;   // bytes of one part (leading or remainder)
+    // Bytes of one part (leading or remainder): only the NCHUNK * 8 rows the builders write.  The MMAs of the last tile
+    // read up to MT * 128 rows, i.e. past the end of the part into the next part or the gamma stages: FP16 values that
+    // land only in accumulator rows tc_row_info() marks as unused.
+    static constexpr int PHI_PART = NCHUNK * 8 * kTE * 2;
     static constexpr int PHI_STAGE = 2 * PHI_PART;
     static constexpr int G_PART = kNCL * kTE * 2;
-    static constexpr int G_STAGE = 3 * G_PART;            // [gh (64 rows) ; gl (64 rows)] = ONE K-major N = 128 image, then gs
+    static constexpr int G_STAGE = 3 * G_PART;            // gh, gl, gs: three K-major N = 32 images
     static constexpr int RAWX = D * kTE * 4;              // [D][32 events] from the SoA copy
     static constexpr int RAWG = kNCL * kTE * 4;
     static constexpr int OFF_PHI = 0;
@@ -128,6 +134,7 @@ template <int D> struct MCfg {
     static constexpr int REG_C = MT == 3 ? 96 : (MT == 2 ? 112 : 240);
     static_assert(128 * REG_P + 256 * REG_B + NCT * REG_C <= THREADS * REG_LAUNCH, "register pools");
     static_assert(OFF_RAWG % 1024 == 0 && RAWG % 1024 == 0, "SWIZZLE_128B TMA destinations need 1024-byte alignment");
+    static_assert((MT * 128 - NCHUNK * 8) * kTE * 2 <= kNST * G_STAGE, "the last part's over-read stays inside the operand stages");
     static_assert(MT <= 3, "feature tiles");
 };
 
@@ -340,54 +347,75 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     } else {
         set_regs<C::REG_C, C::REG_LAUNCH>();
         // ===================== consumers: wgmma, accumulators in registers =====================
-        const int mt = (warp - 12) >> 2;                           // feature tile of this warpgroup (rows 128 mt ..)
+        // feature tile of this warpgroup (rows 128 mt ..); the shuffle shows ptxas that it is warp-uniform, so the
+        // branches on it do not make ptxas serialise the wgmma
+        const int mt = __shfl_sync(0xffffffffu, (warp - 12) >> 2, 0);
         const int ct = threadIdx.x - 384;                          // consumer thread 0 .. NCT-1
         const int wq = warp & 3, gid = lane >> 2, qd = lane & 3;
         float* racc = reinterpret_cast<float*>(smem + C::OFF_RACC) + ct;     // [32][NCT]: racc[j * NCT]
 #pragma unroll
         for (int j = 0; j < 32; j++) racc[j * C::NCT] = 0.0f;
-        float acc[2][32];                                          // per 64-row half: regs 0-15 exact group, 16-31 remainder group
+        float ex[2][16], rm[2][16];                                // per 64-row half: exact group, remainder group
 #pragma unroll
         for (int h = 0; h < 2; h++)
 #pragma unroll
-            for (int j = 0; j < 32; j++) acc[h][j] = 0.0f;
+            for (int j = 0; j < 16; j++) { ex[h][j] = 0.0f; rm[h][j] = 0.0f; }
+        int held = -1;                                             // stage of the previous sub-tile while its MMAs may run
         for (int i = 0; i < nsub; i++) {
             const int os = i % kNST, oph = (i / kNST) & 1;
             mbar_wait_parked(&op_full[os], oph, 100);
             const uint32_t phi = smem_u32(smem + C::OFF_PHI + os * C::PHI_STAGE);
             const uint32_t gam = smem_u32(smem + C::OFF_G + os * C::G_STAGE);
+            // a chain starts with its first MMA overwriting the accumulators (the drain leaves them as they are)
+            const bool new1 = chain_starts(i, mt), new2 = chain2_starts(i, mt);
             wgmma_fence();
 #pragma unroll
             for (int h = 0; h < 2; h++) {
 #pragma unroll
                 for (int ks = 0; ks < kTE / 16; ks++) {
-                    const uint64_t bdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // rows 0-31 gh, 32-63 gl
+                    const uint64_t hdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // gh
+                    const uint64_t ldesc = make_smem_desc(gam + C::G_PART + ks * 256, 128, 512);         // gl
                     const uint64_t sdesc = make_smem_desc(gam + 2 * C::G_PART + ks * 256, 128, 512);     // gs
                     const uint32_t arow = mt * 8192 + h * 4096 + ks * 256;
                     const uint64_t ah = make_smem_desc(phi + arow, /*LBO*/ 128, /*SBO*/ 512);
                     const uint64_t al = make_smem_desc(phi + C::PHI_PART + arow, 128, 512);
-                    wgmma_m64n64k16_ss_tn(acc[h], ah, bdesc);                                          // [ph gh | ph gl]
-                    wgmma_m64n32k16_ss_tn(*reinterpret_cast<float(*)[16]>(&acc[h][16]), al, sdesc);     //        += pl gs
+                    wgmma_m64n32k16_ss_tn(ex[h], ah, hdesc, ks > 0 || !new1);     // ph gh
+                    wgmma_m64n32k16_ss_tn(rm[h], ah, ldesc, ks > 0 || !new2);     // ph gl
+                    wgmma_m64n32k16_ss_tn(rm[h], al, sdesc);                      // + pl gs
                 }
             }
             wgmma_commit();
-            wgmma_wait_all();
+            // the previous sub-tile's MMAs have read their stage once at most this sub-tile's group is in flight
+            wgmma_wait<1>();
             __syncwarp();
-            if (lane == 0) mbar_arrive(&op_empty[os]);         // operand stage reusable: these MMAs have read it
+            if (lane == 0 && held >= 0) mbar_arrive(&op_empty[held]);
+            held = os;
             // drain: exact group at the end of its 128-event chain, remainder group at the end of its longer chain
+            // (the second ends only where the first does)
             if (chain_ends(i, mt, nsub)) {
+                wgmma_wait<0>();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&op_empty[os]);
+                held = -1;
+                // one half at a time (the empty asm keeps ptxas from hoisting all 32 loads): with every accumulator
+                // live, 32 loads in flight would not fit the consumers' registers at D = 24
 #pragma unroll
-                for (int h = 0; h < 2; h++)
+                for (int h = 0; h < 2; h++) {
 #pragma unroll
-                    for (int j = 0; j < 16; j++) { racc[(h * 16 + j) * C::NCT] += acc[h][j]; acc[h][j] = 0.0f; }
-            }
-            if (chain2_ends(i, mt, nsub)) {
+                    for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += ex[h][j];
+                    asm volatile("" ::: "memory");
+                }
+                if (chain2_ends(i, mt, nsub)) {
 #pragma unroll
-                for (int h = 0; h < 2; h++)
+                    for (int h = 0; h < 2; h++) {
 #pragma unroll
-                    for (int j = 0; j < 16; j++) { racc[(h * 16 + j) * C::NCT] += acc[h][16 + j]; acc[h][16 + j] = 0.0f; }
+                        for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += rm[h][j];
+                        asm volatile("" ::: "memory");
+                    }
+                }
             }
         }
+        wgmma_wait<0>();            // (the last sub-tile drained: nothing in flight; without it ptxas waits in every iteration)
         // one plain store of this thread's partial sums: [cta][tile][row][32 clusters]
         float* my = scratch + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * C::MT * 128 * kNCL + (size_t)mt * 128 * kNCL;
 #pragma unroll

@@ -101,6 +101,9 @@ __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D[64 x 128] (+)= A[64 x 16] (registers, K-major fragments) * B[16 x 128] (shared memory, K-major); one warpgroup.
 __device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc, bool accumulate) {
@@ -114,28 +117,17 @@ __device__ __forceinline__ void wgmma_m64n128k16_rs(float (&d)[64], uint32_t a0,
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"((uint32_t)accumulate));
 }
 
-// D[64 x 64] += A[64 x 16] * B[16 x 64], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
-__device__ __forceinline__ void wgmma_m64n64k16_ss_tn(float (&d)[32], uint64_t a_desc, uint64_t b_desc) {
+// D[64 x 32] (+)= A[64 x 16] * B[16 x 32], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
+// accumulate = false overwrites D (scale-d = 0): a new accumulation chain starts without writing the registers first.
+__device__ __forceinline__ void wgmma_m64n32k16_ss_tn(float (&d)[16], uint64_t a_desc, uint64_t b_desc, bool accumulate = true) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, 1, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-        "%32, %33, p, 1, 1, 1, 0;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-        : "l"(a_desc), "l"(b_desc));
-}
-
-// D[64 x 32] += A[64 x 16] * B[16 x 32], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
-__device__ __forceinline__ void wgmma_m64n32k16_ss_tn(float (&d)[16], uint64_t a_desc, uint64_t b_desc) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, 1, 0;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
         "%16, %17, p, 1, 1, 1, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(a_desc), "l"(b_desc));
+        : "l"(a_desc), "l"(b_desc), "r"((uint32_t)accumulate));
 }
 
 __device__ __forceinline__ bool elect_one() {
