@@ -1,6 +1,7 @@
 """CPU emulation of the tensor M-step's operand arithmetic (exact accumulation): which part of the per-call
 covariance error comes from the FP16 hi/lo operand split (truncating vs round-to-nearest, 3 vs 4 products)?
-Test infrastructure (uses the oracle); not part of the product."""
+Test infrastructure (uses the oracle); not part of the product.  The scheme the kernel runs now, with its CTA ranges,
+chains and drains, is emulated by tests/test_mstep_error_model.py (python tests/test_mstep_error_model.py prints its table)."""
 import sys, os
 import numpy as np
 sys.path.insert(0, os.getcwd())
