@@ -268,6 +268,45 @@ allreduce_peer_kernel(PeerTable t, double* __restrict__ stats, int len, int pari
     }
 }
 
+// gmm_score's own buffers (nothing of the EM state is touched): per slot s of two, a pinned input stage and a device
+// chunk of events, device outputs and their pinned mirror laid out [ll double | flag int | pad][labels][max_resp][logp],
+// plus the running state of the tensor kernel's passes (K > 64).
+struct ScoreBuffers {
+    long long cap = 0;                          // events per chunk
+    float* h_in[2] = {nullptr, nullptr};
+    float* d_in[2] = {nullptr, nullptr};
+    char* d_out[2] = {nullptr, nullptr};
+    char* h_out[2] = {nullptr, nullptr};
+    float* d_run_den = nullptr;
+    float* d_run_bl = nullptr;
+    int* d_run_bk = nullptr;
+    cudaStream_t copy = nullptr;                // H2D of the next chunk / D2H of the last one, beside the kernels
+    cudaEvent_t h2d[2] = {nullptr, nullptr}, kern[2] = {nullptr, nullptr}, d2h[2] = {nullptr, nullptr};
+    cudaEvent_t t0[2] = {nullptr, nullptr}, t1[2] = {nullptr, nullptr};
+    double kernel_ms = 0, wall_ms = 0;          // gmm_get_score_profile
+    long long tensor_chunks = 0, simt_chunks = 0;
+    static constexpr size_t kHeader = 16;
+    static size_t out_bytes(long long cap) { return kHeader + (size_t)cap * 12; }
+    void release() {
+        for (int s = 0; s < 2; s++) {
+            if (h_in[s]) cudaFreeHost(h_in[s]);
+            if (h_out[s]) cudaFreeHost(h_out[s]);
+            cudaFree(d_in[s]); cudaFree(d_out[s]);
+            h_in[s] = d_in[s] = nullptr; h_out[s] = d_out[s] = nullptr;
+        }
+        cudaFree(d_run_den); cudaFree(d_run_bl); cudaFree(d_run_bk);
+        d_run_den = d_run_bl = nullptr; d_run_bk = nullptr;
+        cap = 0;
+    }
+    void destroy() {
+        release();
+        for (int s = 0; s < 2; s++)
+            for (cudaEvent_t* e : {&h2d[s], &kern[s], &d2h[s], &t0[s], &t1[s]})
+                if (*e) { cudaEventDestroy(*e); *e = nullptr; }
+        if (copy) { cudaStreamDestroy(copy); copy = nullptr; }
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -336,6 +375,9 @@ struct gmm_ctx {
     PhaseTimer t_final;
     long long dev_finalize_launches = 0, dev_replays = 0;
     int fin_fault_iter = -1;     // option "finalize_fault_iter" (tests): that iteration of the next batch reports a failure
+    bool params_partial = false; // gmm_mstep has updated N, means, R but not yet Rinv / constants / the operand (upload_params clears)
+    ScoreBuffers score;          // gmm_score: streaming buffers, allocated on first use
+    long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score
 };
 
 namespace gmm {
@@ -471,7 +513,8 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
         CUDA_TRY(cudaMemcpyAsync(c->d_avgvar, stage, sizeof(float) * (size_t)K, cudaMemcpyHostToDevice, c->stream));
     }
     c->cur_K = K;
-    c->memcpy_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    c->params_partial = false;
+    c->memcpy_ms +=std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return GMM_OK;
 }
 
@@ -486,6 +529,26 @@ static int launch_estep_simt(gmm_ctx* c, int K) {
     if (c->n == 0) return GMM_OK;
     switch (c->D) {
 #define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K); break;
+        GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
+        GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
+        GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
+        GMM_CASE(25) GMM_CASE(26) GMM_CASE(27) GMM_CASE(28) GMM_CASE(29) GMM_CASE(30) GMM_CASE(31) GMM_CASE(32)
+#undef GMM_CASE
+        default: return fail(GMM_ERR_ARG, "unsupported dimension count");
+    }
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+
+template <int D>
+static void launch_score_simt_d(gmm_ctx* c, int K, const TcScoreIo& io) {
+    score_simt_kernel<D><<<(io.n + kEstepThreads - 1) / kEstepThreads, kEstepThreads, 0, c->stream>>>(io.x, io.n, K, c->d_epack, io.labels,
+                                                                                                     io.max_resp, io.logp, io.ll);
+}
+static int launch_score_simt(gmm_ctx* c, int K, const TcScoreIo& io) {
+    if (io.n <= 0) return GMM_OK;
+    switch (c->D) {
+#define GMM_CASE(d) case d: launch_score_simt_d<d>(c, K, io); break;
         GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
         GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
         GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
@@ -834,6 +897,7 @@ void gmm_destroy(gmm_ctx* c) {
     peer_exchange_destroy(c);
     if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
     tc_destroy(c->tc);
+    c->score.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -989,6 +1053,10 @@ int gmm_set_option(gmm_ctx* c, const char* key, double value) {
     else if (k == "allreduce") c->allreduce_mode = value != 0 ? 1 : 0;
     else if (k == "finalize") { c->finalize_mode = value != 0 ? 1 : 0; if (value != 0) c->dev_fin_failed = false; }
     else if (k == "finalize_fault_iter") c->fin_fault_iter = (int)value;
+    else if (k == "score_chunk") {
+        if (!(value >= 1 && value <= 268435456.0)) return fail(GMM_ERR_ARG, "gmm_set_option: score_chunk must be in [1, 2^28] events");
+        c->score_chunk = (long long)value;
+    }
     else return fail(GMM_ERR_ARG, "gmm_set_option: unknown key '" + k + "'");
     return GMM_OK;
 }
@@ -1087,6 +1155,7 @@ int gmm_mstep(gmm_ctx* c, int K) {
     c->h_stats[(size_t)K * c->F] = ll_keep;
     // gmm_mstep stops before constants_kernel: N, means, R only (gaussian.cu:538-687)
     finalize_from_stats(c->h_stats, c->shift, K, c->D, &c->host, c->host_threads, /*with_constants=*/false);
+    c->params_partial = true;
     collect_all(c);
     return GMM_OK;
 }
@@ -1276,6 +1345,175 @@ int gmm_em(gmm_ctx* c, int K, int min_iters, int max_iters, float epsilon, float
     collect_all(c);
     if (loglik_out) *loglik_out = likelihood;
     if (iters_out) *iters_out = iters;
+    return GMM_OK;
+}
+
+// ---- scoring of new events ------------------------------------------------------------------------------------------
+// Buffers for chunks of c->score_chunk events: allocated on first use, grown (never shrunk) when the option grows.
+static int score_buffers(gmm_ctx* c) {
+    ScoreBuffers& s = c->score;
+    if (!s.copy) {
+        CUDA_TRY(cudaStreamCreateWithFlags(&s.copy, cudaStreamNonBlocking));
+        for (int b = 0; b < 2; b++) {
+            for (cudaEvent_t* e : {&s.h2d[b], &s.kern[b], &s.d2h[b]}) CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+            CUDA_TRY(cudaEventCreate(&s.t0[b]));
+            CUDA_TRY(cudaEventCreate(&s.t1[b]));
+        }
+    }
+    const long long want = c->score_chunk;
+    if (s.cap >= want) return GMM_OK;
+    s.release();
+    for (int b = 0; b < 2; b++) {
+        CUDA_TRY(cudaMallocHost(&s.h_in[b], sizeof(float) * (size_t)want * c->D));
+        CUDA_TRY(cudaMalloc(&s.d_in[b], sizeof(float) * (size_t)want * c->D));
+        CUDA_TRY(cudaMalloc(&s.d_out[b], ScoreBuffers::out_bytes(want)));
+        CUDA_TRY(cudaMallocHost(&s.h_out[b], ScoreBuffers::out_bytes(want)));
+    }
+    if (c->Kmax > 64) {
+        CUDA_TRY(cudaMalloc(&s.d_run_den, sizeof(float) * (size_t)want));
+        CUDA_TRY(cudaMalloc(&s.d_run_bl, sizeof(float) * (size_t)want));
+        CUDA_TRY(cudaMalloc(&s.d_run_bk, sizeof(int) * (size_t)want));
+    }
+    s.cap = want;
+    return GMM_OK;
+}
+
+// Output pointers of slot b (device or pinned host image of the same layout).
+static TcScoreIo score_io(gmm_ctx* c, char* base, int b, int n) {
+    ScoreBuffers& s = c->score;
+    TcScoreIo io{};
+    io.x = s.d_in[b];
+    io.n = n;
+    io.ll = reinterpret_cast<double*>(base);
+    io.flag = reinterpret_cast<int*>(base + 8);
+    io.labels = reinterpret_cast<int*>(base + ScoreBuffers::kHeader);
+    io.max_resp = reinterpret_cast<float*>(base + ScoreBuffers::kHeader + 4 * (size_t)s.cap);
+    io.logp = reinterpret_cast<float*>(base + ScoreBuffers::kHeader + 8 * (size_t)s.cap);
+    io.run_den = s.d_run_den; io.run_bl = s.d_run_bl; io.run_bk = s.d_run_bk;
+    return io;
+}
+
+// Chunks of the batch go through slot i & 1: host rows -> pinned stage -> (copy stream) device chunk -> (compute stream)
+// score kernel -> (copy stream) outputs -> pinned mirror -> caller's arrays.  Chunk i's H2D and the host staging of
+// chunk i + 1 overlap chunk i - 1's kernel and D2H; a chunk is finished (outputs handed over, re-scored if needed)
+// while the next one is already queued.
+static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, int* labels, float* max_resp, float* logp, double* ll_sum) {
+    ScoreBuffers& s = c->score;
+    const int D = c->D;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;     // (the buffers hold at least this many)
+    const bool tensor = c->estep_tensor_ready;
+    bool epack_ready = !tensor;            // while the tensor operand serves the parameters d_epack is not maintained
+    auto ensure_epack = [&]() -> int {
+        if (epack_ready) return GMM_OK;
+        build_epack(K, D, &c->host, c->h_epack);
+        CUDA_TRY(cudaMemcpyAsync(c->d_epack, c->h_epack, sizeof(float) * (size_t)K * epack_stride(D), cudaMemcpyHostToDevice, c->stream));
+        epack_ready = true;
+        return GMM_OK;
+    };
+    auto launch = [&](int b, int m, bool on_tensor) -> int {
+        const TcScoreIo io = score_io(c, s.d_out[b], b, m);
+        CUDA_TRY(cudaMemsetAsync(s.d_out[b], 0, ScoreBuffers::kHeader, c->stream));
+        if (!on_tensor)
+            if (int rc = ensure_epack()) return rc;
+        CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
+        int rc = on_tensor ? tc_launch_score(c->tc, K, io, c->stream) : launch_score_simt(c, K, io);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
+        (on_tensor ? s.tensor_chunks : s.simt_chunks)++;
+        return GMM_OK;
+    };
+    // D2H of the header and of the requested outputs of slot b
+    auto fetch = [&](int b, int m, cudaStream_t st) -> int {
+        const TcScoreIo dv = score_io(c, s.d_out[b], b, m), hv = score_io(c, s.h_out[b], b, m);
+        CUDA_TRY(cudaMemcpyAsync(s.h_out[b], s.d_out[b], ScoreBuffers::kHeader, cudaMemcpyDeviceToHost, st));
+        if (labels) CUDA_TRY(cudaMemcpyAsync(hv.labels, dv.labels, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, st));
+        if (max_resp) CUDA_TRY(cudaMemcpyAsync(hv.max_resp, dv.max_resp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
+        if (logp) CUDA_TRY(cudaMemcpyAsync(hv.logp, dv.logp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
+        return GMM_OK;
+    };
+    auto kernel_ms = [&](int b) {
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) s.kernel_ms += ms;
+    };
+    auto issue = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
+        std::memcpy(s.h_in[b], ev + (size_t)e0 * D, sizeof(float) * (size_t)m * D);
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the chunk buffer's previous kernel is done with it
+        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyHostToDevice, s.copy));
+        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous outputs have left the device
+        if (int rc = launch(b, m, tensor)) return rc;
+        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
+        if (int rc = fetch(b, m, s.copy)) return rc;
+        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
+        return GMM_OK;
+    };
+    auto finish = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
+        kernel_ms(b);
+        const TcScoreIo hv = score_io(c, s.h_out[b], b, m);
+        if (tensor && *hv.flag) {
+            // an event beyond the FP16 event operand's range (or not finite): the SIMT kernel scores the chunk again
+            // (its rows are still in the slot's device buffer: the next H2D into it is issued after this)
+            if (estep_path_of(c) == GMM_PATH_TENSOR)
+                return fail(GMM_ERR_STATE, "gmm_score: an event lies outside the tensor E-step's FP16 operand range (beyond 2^14 "
+                                           "standard deviations, or not finite) and the path is GMM_PATH_TENSOR");
+            s.tensor_chunks--;                                    // its outputs come from the SIMT kernel
+            if (int rc = launch(b, m, false)) return rc;
+            if (int rc = fetch(b, m, c->stream)) return rc;
+            CUDA_TRY(cudaStreamSynchronize(c->stream));
+            kernel_ms(b);
+        }
+        *ll_sum += *hv.ll;
+        if (labels) std::memcpy(labels + e0, hv.labels, sizeof(int) * (size_t)m);
+        if (max_resp) std::memcpy(max_resp + e0, hv.max_resp, sizeof(float) * (size_t)m);
+        if (logp) std::memcpy(logp + e0, hv.logp, sizeof(float) * (size_t)m);
+        return GMM_OK;
+    };
+    for (long long i = 0; i < nchunks; i++) {
+        if (int rc = issue(i)) return rc;
+        if (i > 0)
+            if (int rc = finish(i - 1)) return rc;
+    }
+    return finish(nchunks - 1);
+}
+
+int gmm_score(gmm_ctx* c, int K, const float* events_aos, long long n, int* labels, float* max_resp, float* logp, double* loglik_out) {
+    if (int rc = check_K(c, K, "gmm_score")) return rc;
+    if (n < 0 || (n > 0 && !events_aos)) return fail(GMM_ERR_ARG, "gmm_score: bad events (n < 0, or no rows)");
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_score: parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, "gmm_score: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    double ll = 0.0;
+    int rc = GMM_OK;
+    if (n > 0) {
+        rc = score_buffers(c);
+        if (rc == GMM_OK) rc = score_batch(c, K, events_aos, n, labels, max_resp, logp, &ll);
+        // nothing of this call may still be in flight when it returns (also after a failure)
+        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
+        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = fail(GMM_ERR_CUDA, std::string("gmm_score: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    c->score.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (rc == GMM_OK && loglik_out) *loglik_out = ll;
+    return rc;
+}
+
+int gmm_get_score_profile(gmm_ctx* c, double out[4], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_score_profile: bad argument");
+    ScoreBuffers& s = c->score;
+    out[0] = s.kernel_ms; out[1] = s.wall_ms; out[2] = (double)s.tensor_chunks; out[3] = (double)s.simt_chunks;
+    if (reset) { s.kernel_ms = s.wall_ms = 0; s.tensor_chunks = s.simt_chunks = 0; }
     return GMM_OK;
 }
 

@@ -104,6 +104,78 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
 }
 
 // ---------------------------------------------------------------------------
+// Scoring of new events (gmm_score) for every D and any K in one launch: the E-step above with the same cluster staging
+// and the same logit arithmetic, reading the caller's AoS chunk [n][D] directly, keeping an online log-sum-exp and a
+// running arg-max (lowest k on ties; NaN logits never win, -1 when every logit is NaN) and storing only the label,
+// max_resp = expf(l_max - denom) (bit-identical to the stored responsibility of estep_simt_kernel) and logp = denom.
+// ---------------------------------------------------------------------------
+template <int D>
+__global__ void __launch_bounds__(kEstepThreads)
+score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __restrict__ epack, int* __restrict__ labels,
+                  float* __restrict__ max_resp, float* __restrict__ logp, double* __restrict__ ll_out) {
+    constexpr int STRIDE = epack_stride_c(D);
+    constexpr int COEF = (D + 3) & ~3;
+    constexpr int NCOEF = D * (D + 1) / 2;
+    __shared__ __align__(16) float sp[kEstepClusterChunk * STRIDE];
+    __shared__ double sred[kEstepThreads / 32];
+
+    const int e = blockIdx.x * kEstepThreads + threadIdx.x;
+    const bool valid = e < n;
+    float x[D];
+#pragma unroll
+    for (int d = 0; d < D; d++) x[d] = valid ? x_aos[(size_t)e * D + d] : 0.0f;
+
+    float run_max = -INFINITY, run_sum = 0.0f, best_l = -INFINITY;
+    int best_k = -1;
+    for (int k0 = 0; k0 < K; k0 += kEstepClusterChunk) {
+        const int kc = min(kEstepClusterChunk, K - k0);
+        __syncthreads();
+        {
+            const float4* src = reinterpret_cast<const float4*>(epack + (size_t)k0 * STRIDE);
+            float4* dst = reinterpret_cast<float4*>(sp);
+            for (int i = threadIdx.x; i < kc * STRIDE / 4; i += kEstepThreads) dst[i] = src[i];
+        }
+        __syncthreads();
+        for (int kk = 0; kk < kc; kk++) {
+            const float* p = sp + kk * STRIDE;
+            float dx[D];
+#pragma unroll
+            for (int d = 0; d < D; d++) dx[d] = x[d] - p[d];
+            float q = 0.0f;
+            int idx = COEF;
+#pragma unroll
+            for (int i = 0; i < D; i++) {
+                float t = 0.0f;
+#pragma unroll
+                for (int j = i; j < D; j++) t = fmaf(p[idx++], dx[j], t);
+                q = fmaf(dx[i], t, q);
+            }
+            const float l = fmaf(-0.5f, q, p[COEF + NCOEF]);
+            if (l > best_l || (best_k < 0 && l == l)) { best_l = l; best_k = k0 + kk; }
+            const float m2 = fmaxf(run_max, l);
+            run_sum = run_sum * expf(run_max - m2) + expf(l - m2);
+            run_max = m2;
+        }
+    }
+    const float denom = run_max + logf(run_sum);
+    if (valid) {
+        labels[e] = best_k;
+        max_resp[e] = best_k >= 0 ? expf(best_l - denom) : __int_as_float(0x7fc00000);
+        logp[e] = denom;
+    }
+    double ll = valid ? (double)denom : 0.0;
+    ll = warp_sum(ll);
+    if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = ll;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0;
+#pragma unroll
+        for (int w = 0; w < kEstepThreads / 32; w++) s += sred[w];
+        atomicAdd(ll_out, s);
+    }
+}
+
+// ---------------------------------------------------------------------------
 // M-step statistics: mstep_N + mstep_means + mstep_covariance1 of the
 // reference (gaussian_kernel.cu:522-677) as ONE pass over the events and the
 // responsibilities:  stats[k][f] += sum_n g[k][n] * phi_f(x_n - shift), with

@@ -520,6 +520,120 @@ template <int D> struct ECfg {
     static constexpr int THREADS = 128 * NWG;
 };
 
+// ---- pieces shared by estep_tc_kernel and score_tc_kernel (same operand path, different epilogues) ----------------
+// Shared-memory staging of one pass: constants, shift / inverse scale, and the resident B image (one TMA bulk copy per
+// block, completion on b_full).  Followed by a __syncthreads inside; the caller waits on b_full before the first MMA.
+template <int D>
+__device__ __forceinline__ void tc_stage_operand(uint8_t* smem, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
+                                                 const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, int NSG) {
+    using C = ECfg<D>;
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
+    float* ck_s = reinterpret_cast<float*>(smem + C::OFF_CK);
+    float* sh_s = reinterpret_cast<float*>(smem + C::OFF_SH);
+    if (threadIdx.x == 0) { mbar_init(b_full, 1); fence_mbar_init(); }
+    // base-2 logits in the epilogue: l2 = ck * log2(e) + (-0.5 * log2(e) / scale_k^2) * |scale_k * y|^2   (the per-cluster
+    // power-of-two scale_k keeps the FP16 whitening factors in range whatever the cluster's width, see bimg_cluster)
+    if (threadIdx.x < 64) { ck_s[threadIdx.x] = ck[threadIdx.x] * 1.4426950408889634f; ck_s[64 + threadIdx.x] = ck[64 + threadIdx.x]; }
+    if (threadIdx.x < D) { sh_s[threadIdx.x] = shift_f[threadIdx.x]; sh_s[32 + threadIdx.x] = inv_scale_f[threadIdx.x]; }
+    __syncthreads();
+    if (threadIdx.x == 0) {                    // resident B operand: one TMA bulk copy per block
+        mbar_arrive_expect_tx(b_full, (uint32_t)NSG * C::B_SG);
+        for (int g = 0; g < NSG * C::CP; g++) tma_load_1d(smem + C::OFF_B + g * C::B_BLOCK, b_img + (size_t)g * C::B_BLOCK, C::B_BLOCK, b_full);
+    }
+}
+
+// Standardise the two rows a thread holds and split them into FP16 hi / lo A fragments ([chunk][row]).
+template <int D>
+__device__ __forceinline__ void tc_split_rows(const float2 (&xa)[D / 8], const float2 (&xb)[D / 8], const float* sh_s, const float* isc_s,
+                                              int qd, uint32_t (&zh)[D / 8][2], uint32_t (&zl)[D / 8][2]) {
+#pragma unroll
+    for (int j = 0; j < D / 8; j++) {
+        const float s0 = sh_s[8 * j + 2 * qd], s1 = sh_s[8 * j + 2 * qd + 1];
+        const float i0 = isc_s[8 * j + 2 * qd], i1 = isc_s[8 * j + 2 * qd + 1];
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            const float2 x = r ? xb[j] : xa[j];
+            const float z0 = __fmul_rn(__fsub_rn(x.x, s0), i0), z1 = __fmul_rn(__fsub_rn(x.y, s1), i1);
+            const __half2 h = __floats2half2_rn(z0, z1);
+            const float2 f = __half22float2(h);
+            zh[j][r] = *reinterpret_cast<const uint32_t*>(&h);
+            zl[j][r] = pack_half2(z0 - f.x, z1 - f.y);
+        }
+    }
+}
+
+// The base-2 logits of one 64-event tile against the resident clusters of the pass: per supergroup of 16 clusters and
+// block c of 8 output dimensions the k-steps that block needs (m64n128k16, A from registers), the squares summed over
+// the 8 columns of each cluster with a quad transpose.  lg[sg][u]: cluster sg * 16 + 8 (qd & 1) + 4 (qd >> 1) + (u >> 1),
+// row u & 1 (-inf for supergroups >= NSG).
+template <int D>
+__device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], const uint32_t (&zl)[D / 8][2], uint32_t bsm,
+                                               const float* ck_s, int NSG, int qd, uint32_t ones, float (&lg)[ECfg<D>::MAXSG][8]) {
+    using C = ECfg<D>;
+    constexpr int CP = C::CP;
+    constexpr uint32_t CH = C::N * 16;                        // bytes per B chunk
+#pragma unroll
+    for (int sg = 0; sg < C::MAXSG; sg++) {
+        if (sg >= NSG) {
+#pragma unroll
+            for (int u = 0; u < 8; u++) lg[sg][u] = -INFINITY;
+            continue;
+        }
+        float sq[32];                                      // sums of squares: [cluster 0..15][row]
+#pragma unroll
+        for (int u = 0; u < 32; u++) sq[u] = 0.f;
+#pragma unroll
+        for (int c = 0; c < CP; c++) {
+            const uint32_t bb = bsm + (uint32_t)(sg * CP + c) * C::B_BLOCK;
+            float acc[64];
+#pragma unroll
+            for (int u = 0; u < 64; u++) acc[u] = 0.f;
+            wgmma_fence();
+            bool accum = false;
+#pragma unroll
+            for (int j = c; j < CP; j++) {                 // (Wh_j, Wl_j) x (zh_j, zh_j)
+                wgmma_m64n128k16_rs(acc, zh[j][0], zh[j][1], zh[j][0], zh[j][1], make_smem_desc(bb + j * CH, CP * CH, 128), accum);
+                accum = true;
+            }
+            // (Wh_j) x (zl_j) for j >= c, then v x ones, two at a time; a lone v step pairs with a zero A chunk
+#pragma unroll
+            for (int p = c; p < CP + 1; p += 2) {
+                const int x = p, y = p + 1;                // list items: j < CP -> Wh_j x zl_j, j == CP -> v x ones
+                if (y <= CP) {
+                    const uint32_t yc = y < CP ? (uint32_t)y : 2u * CP;
+                    const uint32_t a2 = y < CP ? zl[y < CP ? y : 0][0] : ones, a3 = y < CP ? zl[y < CP ? y : 0][1] : ones;
+                    wgmma_m64n128k16_rs(acc, zl[x][0], zl[x][1], a2, a3, make_smem_desc(bb + x * CH, (yc - x) * CH, 128), true);
+                } else {                                   // x == CP: v alone, paired with chunk c under a zero A chunk
+                    wgmma_m64n128k16_rs(acc, 0u, 0u, ones, ones, make_smem_desc(bb + c * CH, (2 * CP - c) * CH, 128), true);
+                }
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+#pragma unroll
+            for (int i = 0; i < 16; i++) {
+                sq[2 * i] = fmaf(acc[4 * i], acc[4 * i], fmaf(acc[4 * i + 1], acc[4 * i + 1], sq[2 * i]));
+                sq[2 * i + 1] = fmaf(acc[4 * i + 2], acc[4 * i + 2], fmaf(acc[4 * i + 3], acc[4 * i + 3], sq[2 * i + 1]));
+            }
+        }
+        // sum over the quad (the 8 columns of a cluster are spread over its 4 lanes), transposing as it goes:
+        // lane qd ends with clusters cb .. cb+3 of the supergroup, cb = 8 (qd & 1) + 4 (qd >> 1), both rows
+        float w[16];
+        const bool b1 = qd & 1, b2 = (qd >> 1) & 1;
+#pragma unroll
+        for (int u = 0; u < 16; u++) {
+            const float send = b1 ? sq[u] : sq[16 + u], keep = b1 ? sq[16 + u] : sq[u];
+            w[u] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+        }
+#pragma unroll
+        for (int u = 0; u < 8; u++) {
+            const float send = b2 ? w[u] : w[8 + u], keep = b2 ? w[8 + u] : w[u];
+            const float qv = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+            const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
+            lg[sg][u] = fmaf(ck_s[64 + k], qv, ck_s[k]);
+        }
+    }
+}
+
 template <int D>
 __global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
 estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
@@ -545,16 +659,7 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
     const int gid = lane >> 2, qd = lane & 3;
     const int ntiles = (n + 63) / 64;
 
-    if (threadIdx.x == 0) { mbar_init(b_full, 1); fence_mbar_init(); }
-    // base-2 logits in the epilogue: l2 = ck * log2(e) + (-0.5 * log2(e) / scale_k^2) * |scale_k * y|^2   (the per-cluster
-    // power-of-two scale_k keeps the FP16 whitening factors in range whatever the cluster's width, see bimg_cluster)
-    if (threadIdx.x < 64) { ck_s[threadIdx.x] = ck[threadIdx.x] * 1.4426950408889634f; ck_s[64 + threadIdx.x] = ck[64 + threadIdx.x]; }
-    if (threadIdx.x < D) { sh_s[threadIdx.x] = shift_f[threadIdx.x]; isc_s[threadIdx.x] = inv_scale_f[threadIdx.x]; }
-    __syncthreads();
-    if (threadIdx.x == 0) {                    // resident B operand: one TMA bulk copy per block
-        mbar_arrive_expect_tx(b_full, (uint32_t)NSG * C::B_SG);
-        for (int g = 0; g < NSG * CP; g++) tma_load_1d(smem + C::OFF_B + g * C::B_BLOCK, b_img + (size_t)g * C::B_BLOCK, C::B_BLOCK, b_full);
-    }
+    tc_stage_operand<D>(smem, b_img, ck, shift_f, inv_scale_f, NSG);
 
     // rows r0 = 16 warp + gid and r1 = r0 + 8 of each 64-event tile; K positions 2 qd, 2 qd + 1 of every 8-wide chunk
     const int r0 = warp * 16 + gid;
@@ -572,91 +677,18 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
     if (t < ntiles) load_rows(t);
     const uint32_t ones = qd == 0 ? 0x3C003C00u : 0u;         // chunk {1, 1, 0 ...}: K elements 0 and 1 are held by qd == 0
     const uint32_t bsm = smem_u32(smem + C::OFF_B);
-    constexpr uint32_t CH = C::N * 16;                        // bytes per B chunk
     double ll_acc = 0.0;
     constexpr float kLn2 = 0.6931471805599453f;
     mbar_wait(b_full, 0);
 
     for (; t < ntiles; t += stride) {
         uint32_t zh[CP][2], zl[CP][2];                         // [chunk][row]: FP16 pairs, hi and lo parts
-#pragma unroll
-        for (int j = 0; j < CP; j++) {
-            const float s0 = sh_s[8 * j + 2 * qd], s1 = sh_s[8 * j + 2 * qd + 1];
-            const float i0 = isc_s[8 * j + 2 * qd], i1 = isc_s[8 * j + 2 * qd + 1];
-#pragma unroll
-            for (int r = 0; r < 2; r++) {
-                const float2 x = r ? xb[j] : xa[j];
-                const float z0 = __fmul_rn(__fsub_rn(x.x, s0), i0), z1 = __fmul_rn(__fsub_rn(x.y, s1), i1);
-                const __half2 h = __floats2half2_rn(z0, z1);
-                const float2 f = __half22float2(h);
-                zh[j][r] = *reinterpret_cast<const uint32_t*>(&h);
-                zl[j][r] = pack_half2(z0 - f.x, z1 - f.y);
-            }
-        }
+        tc_split_rows<D>(xa, xb, sh_s, isc_s, qd, zh, zl);
         const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
         if (t + stride < ntiles) load_rows(t + stride);
 
         float lg[C::MAXSG][8];                                 // base-2 logits: [supergroup][4 clusters x 2 rows]
-#pragma unroll
-        for (int sg = 0; sg < C::MAXSG; sg++) {
-            if (sg >= NSG) {
-#pragma unroll
-                for (int u = 0; u < 8; u++) lg[sg][u] = -INFINITY;
-                continue;
-            }
-            float sq[32];                                      // sums of squares: [cluster 0..15][row]
-#pragma unroll
-            for (int u = 0; u < 32; u++) sq[u] = 0.f;
-#pragma unroll
-            for (int c = 0; c < CP; c++) {
-                const uint32_t bb = bsm + (uint32_t)(sg * CP + c) * C::B_BLOCK;
-                float acc[64];
-#pragma unroll
-                for (int u = 0; u < 64; u++) acc[u] = 0.f;
-                wgmma_fence();
-                bool accum = false;
-#pragma unroll
-                for (int j = c; j < CP; j++) {                 // (Wh_j, Wl_j) x (zh_j, zh_j)
-                    wgmma_m64n128k16_rs(acc, zh[j][0], zh[j][1], zh[j][0], zh[j][1], make_smem_desc(bb + j * CH, CP * CH, 128), accum);
-                    accum = true;
-                }
-                // (Wh_j) x (zl_j) for j >= c, then v x ones, two at a time; a lone v step pairs with a zero A chunk
-#pragma unroll
-                for (int p = c; p < CP + 1; p += 2) {
-                    const int x = p, y = p + 1;                // list items: j < CP -> Wh_j x zl_j, j == CP -> v x ones
-                    if (y <= CP) {
-                        const uint32_t yc = y < CP ? (uint32_t)y : 2u * CP;
-                        const uint32_t a2 = y < CP ? zl[y < CP ? y : 0][0] : ones, a3 = y < CP ? zl[y < CP ? y : 0][1] : ones;
-                        wgmma_m64n128k16_rs(acc, zl[x][0], zl[x][1], a2, a3, make_smem_desc(bb + x * CH, (yc - x) * CH, 128), true);
-                    } else {                                   // x == CP: v alone, paired with chunk c under a zero A chunk
-                        wgmma_m64n128k16_rs(acc, 0u, 0u, ones, ones, make_smem_desc(bb + c * CH, (2 * CP - c) * CH, 128), true);
-                    }
-                }
-                wgmma_commit();
-                wgmma_wait_all();
-#pragma unroll
-                for (int i = 0; i < 16; i++) {
-                    sq[2 * i] = fmaf(acc[4 * i], acc[4 * i], fmaf(acc[4 * i + 1], acc[4 * i + 1], sq[2 * i]));
-                    sq[2 * i + 1] = fmaf(acc[4 * i + 2], acc[4 * i + 2], fmaf(acc[4 * i + 3], acc[4 * i + 3], sq[2 * i + 1]));
-                }
-            }
-            // sum over the quad (the 8 columns of a cluster are spread over its 4 lanes), transposing as it goes:
-            // lane qd ends with clusters cb .. cb+3 of the supergroup, cb = 8 (qd & 1) + 4 (qd >> 1), both rows
-            float w[16];
-            const bool b1 = qd & 1, b2 = (qd >> 1) & 1;
-#pragma unroll
-            for (int u = 0; u < 16; u++) {
-                const float send = b1 ? sq[u] : sq[16 + u], keep = b1 ? sq[16 + u] : sq[u];
-                w[u] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
-            }
-#pragma unroll
-            for (int u = 0; u < 8; u++) {
-                const float send = b2 ? w[u] : w[8 + u], keep = b2 ? w[8 + u] : w[u];
-                const float qv = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-                const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
-                lg[sg][u] = fmaf(ck_s[64 + k], qv, ck_s[k]);
-            }
-        }
+        tc_tile_logits<D>(zh, zl, bsm, ck_s, NSG, qd, ones, lg);
         // log-sum-exp over the clusters (estep2, gaussian_kernel.cu:481-503), per row: this lane's 16 logits, then the quad
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -734,6 +766,158 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
     }
 }
 
+// ===========================================================================
+// Scoring of new events (gmm_score): the E-step's operand path and logits (tc_stage_operand / tc_split_rows /
+// tc_tile_logits), with an epilogue that stores 12 B per event instead of 4 K: the label (argmax of the posterior,
+// lowest k on ties, -1 when every logit is NaN), the top responsibility and the log-density (the E-step's denominator).
+// Events are read from a chunk `x_aos` [n][D] of the caller's batch.
+//   K <= 64: one launch (pass 0, last).  max_resp = ex2(l_max - M) * (1 / S), the E-step's operations for the stored
+//            responsibility of that cluster, so it is bit-identical to it.
+//   K > 64:  P launches for P passes of 64 clusters.  Passes 0 .. P-2 keep a per-event running (log-denominator, best
+//            base-2 logit, best k) in run_*; the log-denominator is joined as the E-step's mode 2 joins it and an earlier
+//            pass wins ties.  The last pass joins, stores the outputs and max_resp = exp(l_best - denominator).
+// Every pass flags the chunk (*flag = 1) when an event has a coordinate that is not finite or lies beyond 2^14 global
+// standard deviations (the bound tc_estep_range_ok applies to the training data: the FP16 event operand overflows).
+// ===========================================================================
+template <int D>
+__global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
+score_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
+                const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, int n, int K, int NSG, int kbase,
+                int pass, int last, float* run_den, float* run_bl, int* run_bk, int* __restrict__ labels,
+                float* __restrict__ max_resp, float* __restrict__ logp, double* __restrict__ ll_out, int* __restrict__ flag) {
+    using C = ECfg<D>;
+    constexpr int CP = C::CP;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
+    const float* ck_s = reinterpret_cast<const float*>(smem + C::OFF_CK);
+    const float* sh_s = reinterpret_cast<const float*>(smem + C::OFF_SH);
+    const float* isc_s = sh_s + 32;
+
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int gid = lane >> 2, qd = lane & 3;
+    const int ntiles = (n + 63) / 64;
+    tc_stage_operand<D>(smem, b_img, ck, shift_f, inv_scale_f, NSG);
+
+    const int r0 = warp * 16 + gid;
+    float2 xa[CP], xb[CP];
+    auto load_rows = [&](int t) {
+        const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
+#pragma unroll
+        for (int j = 0; j < CP; j++) {
+            xa[j] = e0 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e0 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+            xb[j] = e1 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e1 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+        }
+    };
+    const int stride = (int)gridDim.x * C::NWG;
+    int t = (int)blockIdx.x * C::NWG + wg;
+    if (t < ntiles) load_rows(t);
+    const uint32_t ones = qd == 0 ? 0x3C003C00u : 0u;
+    const uint32_t bsm = smem_u32(smem + C::OFF_B);
+    double ll_acc = 0.0;
+    constexpr float kLn2 = 0.6931471805599453f, kLog2e = 1.4426950408889634f;
+    bool out_of_range = false;
+    mbar_wait(b_full, 0);
+
+    for (; t < ntiles; t += stride) {
+        const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
+#pragma unroll
+        for (int j = 0; j < CP; j++)
+#pragma unroll
+            for (int r = 0; r < 2; r++) {
+                const float2 x = r ? xb[j] : xa[j];
+                const float z0 = __fmul_rn(__fsub_rn(x.x, sh_s[8 * j + 2 * qd]), isc_s[8 * j + 2 * qd]);
+                const float z1 = __fmul_rn(__fsub_rn(x.y, sh_s[8 * j + 2 * qd + 1]), isc_s[8 * j + 2 * qd + 1]);
+                out_of_range |= (r ? e1 : e0) < n && (!(fabsf(z0) <= 16384.0f) || !(fabsf(z1) <= 16384.0f));
+            }
+        uint32_t zh[CP][2], zl[CP][2];
+        tc_split_rows<D>(xa, xb, sh_s, isc_s, qd, zh, zl);
+        if (t + stride < ntiles) load_rows(t + stride);
+
+        float lg[C::MAXSG][8];
+        tc_tile_logits<D>(zh, zl, bsm, ck_s, NSG, qd, ones, lg);
+
+        // per row: the E-step's max (fmaxf) and the arg-max over the pass's clusters, this lane's 16 logits in increasing
+        // k, then the quad with (value, index) pairs; lowest k on ties, NaN logits never win
+        float mx[2] = {-INFINITY, -INFINITY}, bl[2] = {-INFINITY, -INFINITY};
+        int bk[2] = {-1, -1};
+#pragma unroll
+        for (int sg = 0; sg < C::MAXSG; sg++)
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const float l = lg[sg][u];
+                const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
+                mx[u & 1] = fmaxf(mx[u & 1], l);
+                if (k < K && (l > bl[u & 1] || (bk[u & 1] < 0 && l == l))) { bl[u & 1] = l; bk[u & 1] = kbase + k; }
+            }
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+            mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+#pragma unroll
+            for (int o = 1; o <= 2; o <<= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, bl[r], o);
+                const int ok = __shfl_xor_sync(0xffffffffu, bk[r], o);
+                if (ok >= 0 && (bk[r] < 0 || ov > bl[r] || (ov == bl[r] && ok < bk[r]))) { bl[r] = ov; bk[r] = ok; }
+            }
+        }
+        // the denominator exactly as the E-step forms it
+        float sm[2] = {0.f, 0.f};
+#pragma unroll
+        for (int sg = 0; sg < C::MAXSG; sg++)
+#pragma unroll
+            for (int u = 0; u < 8; u++) sm[u & 1] += ex2_approx(lg[sg][u] - mx[u & 1]);
+        const long long er[2] = {e0, e1};
+        float dx[2] = {0.f, 0.f}, pbl[2] = {0.f, 0.f};
+        int pbk[2] = {-1, -1};
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            sm[r] += __shfl_xor_sync(0xffffffffu, sm[r], 1);
+            sm[r] += __shfl_xor_sync(0xffffffffu, sm[r], 2);
+            // the running state is updated in place: every lane reads before any writes
+            if (pass > 0 && er[r] < n) { dx[r] = run_den[er[r]]; pbl[r] = run_bl[er[r]]; pbk[r] = run_bk[er[r]]; }
+        }
+        __syncwarp();
+#pragma unroll
+        for (int r = 0; r < 2; r++) {
+            float denom = fmaf(mx[r], kLn2, logf(sm[r]));
+            float mr = ex2_approx(bl[r] - mx[r]) * (1.0f / sm[r]);
+            if (pass > 0) {
+                const float g = fmaxf(denom, dx[r]);
+                const float tot = g + logf(__expf(denom - g) + __expf(dx[r] - g));
+                // max_resp with the operations of the E-step's stored value: its mode 2 for a winner of this (last) pass,
+                // its mode 3 for a winner of an earlier one (the product rounded on its own)
+                if (bk[r] >= 0 && (pbk[r] < 0 || bl[r] > pbl[r])) {           // an earlier pass wins ties
+                    const float sc = (1.0f / sm[r]) * __expf(denom - tot);
+                    mr = ex2_approx(bl[r] - mx[r]) * sc;
+                } else {
+                    bl[r] = pbl[r]; bk[r] = pbk[r];
+                    mr = ex2_approx(bl[r] - __fmul_rn(tot, kLog2e));
+                }
+                denom = tot;
+            }
+            if (qd == 0 && er[r] < n) {
+                if (last) {
+                    labels[er[r]] = bk[r];
+                    max_resp[er[r]] = bk[r] >= 0 ? mr : __int_as_float(0x7fc00000);
+                    logp[er[r]] = denom;
+                    ll_acc += (double)denom;
+                } else {
+                    run_den[er[r]] = denom; run_bl[er[r]] = bl[r]; run_bk[er[r]] = bk[r];
+                }
+            }
+        }
+    }
+    if (__any_sync(0xffffffffu, out_of_range) && lane == 0) *flag = 1;
+    if (last) {
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 16);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 8);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 4);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 2);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 1);
+        if (lane == 0) atomicAdd(ll_out, ll_acc);
+    }
+}
+
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
@@ -773,7 +957,7 @@ struct TcState {
     int e_NG = 0;
     int host_threads = 8;
     // cudaFuncAttributeMaxDynamicSharedMemorySize is per device: the "already set" flags live with the (per-device) state
-    bool attr_estep = false, attr_mstep = false;
+    bool attr_estep = false, attr_mstep = false, attr_score = false;
     double h_shift[GMM_MAX_DIMENSIONS] = {0}, h_scale[GMM_MAX_DIMENSIONS] = {0};
 };
 
@@ -1438,6 +1622,41 @@ int tc_launch_estep(TcState* t, int K, double* d_ll, cudaStream_t stream) {
         case 16: return launch_estep_d<16>(t, K, d_ll, stream);
         case 24: return launch_estep_d<24>(t, K, d_ll, stream);
         default: return fail(GMM_ERR_ARG, "tensor E-step: unsupported D");
+    }
+}
+
+template <int D>
+static int launch_score_d(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream) {
+    using C = ECfg<D>;
+    if (!t->attr_score) {
+        TC_CUDA_TRY(cudaFuncSetAttribute(score_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        t->attr_score = true;
+    }
+    const int ntiles = (io.n + 127) / 128;
+    int grid = t->num_sms;
+    if (grid > ntiles) grid = ntiles;
+    if (grid < 1) grid = 1;
+    const int NP = (K + 63) / 64;
+    if (NP > 1 && !(io.run_den && io.run_bl && io.run_bk)) return fail(GMM_ERR_STATE, "tensor scoring: no running state for K > 64");
+    for (int p = 0; p < NP; p++) {
+        const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
+        score_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
+            io.x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f, io.n, Kp,
+            (Kp + C::GB - 1) / C::GB, 64 * p, p, p + 1 == NP, io.run_den, io.run_bl, io.run_bk, io.labels, io.max_resp, io.logp, io.ll,
+            io.flag);
+        TC_CUDA_TRY(cudaGetLastError());
+    }
+    return GMM_OK;
+}
+
+int tc_launch_score(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream) {
+    if (!t || !t->emap_ok) return fail(GMM_ERR_STATE, "tensor scoring not initialised for this shape");
+    if (io.n <= 0) return GMM_OK;
+    switch (t->D) {
+        case 8: return launch_score_d<8>(t, K, io, stream);
+        case 16: return launch_score_d<16>(t, K, io, stream);
+        case 24: return launch_score_d<24>(t, K, io, stream);
+        default: return fail(GMM_ERR_ARG, "tensor scoring: unsupported D");
     }
 }
 

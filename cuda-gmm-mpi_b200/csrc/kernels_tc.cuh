@@ -38,6 +38,22 @@ int  tc_params_cluster(TcState*, const clusters_t* host, int k, int K);
 int  tc_params_cluster_w(TcState*, const clusters_t* host, int k, int K, const double* W);
 int  tc_params_commit(TcState*, int K, int bad, cudaStream_t stream);
 int  tc_launch_estep(TcState*, int K, double* d_ll, cudaStream_t stream);
+// Scoring of a chunk of new events ([n][D] on the device) against the resident operand of the current parameters
+// (score_tc_kernel): labels / max_resp / logp per event, ll += sum of logp, *flag = 1 when an event is outside the FP16
+// operand range.  run_*: per-event running state of the passes, n entries each (needed for K > 64 only).
+struct TcScoreIo {
+    const float* x;
+    int n;
+    int* labels;
+    float* max_resp;
+    float* logp;
+    double* ll;
+    int* flag;
+    float* run_den;
+    float* run_bl;
+    int* run_bk;
+};
+int  tc_launch_score(TcState*, int K, const TcScoreIo& io, cudaStream_t stream);
 // Device-side M-step finalisation: reduced statistics -> parameter set `d_set` (floats, tc_param_set_floats(); arrays at
 // tc_param_set_off(which = 0 N, 1 pi, 2 constant, 3 means, 4 R, 5 Rinv), stride Kmax) + the E-step operand, no host round
 // trip.  d_ll[0] receives the log-likelihood slot of the statistics.  d_bad[0] = first iteration (`iter`) that met a cluster

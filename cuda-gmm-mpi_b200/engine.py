@@ -77,6 +77,8 @@ def load_library():
     L.gmm_em_iterations.argtypes = [C.c_void_p, C.c_int, C.c_int, _FP]
     L.gmm_get_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_get_fit_profile.argtypes = [C.c_void_p, _DP]
+    L.gmm_score.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, _DP]
+    L.gmm_get_score_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
@@ -274,6 +276,26 @@ class Engine:
         keys = ("estep_ms", "mstep_ms", "constants_host_ms", "allreduce_ms", "upload_ms", "mstep_tensor_launches", "iterations",
                 "mstep_simt_launches")
         return dict(zip(keys, list(out)[:8]))
+
+    def score(self, K, events, labels=True, max_resp=True, logp=True):
+        """Assign and score new events (gmm_score) against the current K-cluster parameters.
+        Returns (labels int32, max_resp float32, logp float32, loglik) with None for outputs not asked for."""
+        ev = np.ascontiguousarray(events, np.float32)
+        if ev.ndim != 2 or ev.shape[1] != self.D:
+            raise ValueError(f"events must be [n][{self.D}], got {ev.shape}")
+        n = ev.shape[0]
+        lab = np.empty(n, np.int32) if labels else None
+        mr = np.empty(n, np.float32) if max_resp else None
+        lp = np.empty(n, np.float32) if logp else None
+        ptr = lambda a: a.ctypes.data if a is not None and a.size else None  # noqa: E731
+        ll = C.c_double()
+        _check(self.lib.gmm_score(self.h, K, ptr(ev), n, ptr(lab), ptr(mr), ptr(lp), C.byref(ll)))
+        return lab, mr, lp, ll.value
+
+    def score_profile(self, reset=False):
+        out = (C.c_double * 4)()
+        _check(self.lib.gmm_get_score_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1], tensor_chunks=int(out[2]), simt_chunks=int(out[3]))
 
     def fit_profile(self):
         out = (C.c_double * 4)()

@@ -123,7 +123,9 @@ int  gmm_comm_rank(const gmm_ctx*, int* rank, int* nranks);
  * through the host path and stay on it; 0 = host finalisation every iteration,
  * invert_matrix.cpp semantics; env GMM_FINALIZE=host|device sets the default),
  * "finalize_fault_iter" (tests: that iteration of the next batch reports a
- * failure although nothing is wrong, -1 = never).  Options have to be set
+ * failure although nothing is wrong, -1 = never), "score_chunk" (events per
+ * chunk that gmm_score streams through its pinned and device buffers;
+ * default 1048576, at most 2^28).  Options have to be set
  * identically on every rank of a communicator.  Unknown keys are an
  * error (GMM_ERR_ARG).  Every E-step materialises the memberships on the
  * device (the reference's behaviour); they reach the host only through
@@ -172,6 +174,35 @@ int  gmm_em(gmm_ctx*, int K, int min_iters, int max_iters, float epsilon,
  * gmm_estep()/gmm_em() for the same K.  Returns the global log-likelihood of
  * the last E-step.  This is the unit bench.py times.                        */
 int  gmm_em_iterations(gmm_ctx*, int K, int iters, float* loglik_out);
+
+/* ---- using a fitted mixture (sklearn's predict / score_samples) ---------
+ * Evaluate n events (host, row-major [n][D], NOT the context's shard) against
+ * the parameter set the next gmm_estep(ctx, K) would use.  Per event:
+ *   labels[i]   = argmax_k of the posterior (lowest k on ties, -1 if every
+ *                 logit is NaN),
+ *   max_resp[i] = that posterior (NaN when labels[i] = -1),
+ *   logp[i]     = ln sum_k pi_k N(x_i | k) (the E-step's log-denominator).
+ * Any of the three output pointers may be NULL.  *loglik_out (may be NULL) =
+ * sum of logp in double over this call, THIS context only (no collective).
+ * The kernels are the ones the E-step would use (wgmma for D in {8, 16, 24}
+ * when its operand serves the parameters, else SIMT); a chunk holding an event
+ * beyond 2^14 standard deviations of the training data (or not finite) is
+ * re-scored by the SIMT kernel, or fails with GMM_ERR_STATE under
+ * GMM_PATH_TENSOR.  On the training shard the outputs equal the E-step's
+ * (max_resp bit for bit at K <= 64).  The batch streams through two pinned
+ * buffers in chunks of option "score_chunk" events; nothing of the EM state
+ * (memberships, statistics, log-likelihood, gmm_get_profile) changes.
+ * Errors: K outside [1, Kmax], n < 0 or events_aos == NULL with n > 0 ->
+ * GMM_ERR_ARG; K != the K of the current parameters, or a call between
+ * gmm_mstep and gmm_constants (half-updated parameters) -> GMM_ERR_STATE.
+ * After gmm_fit, score against the best model with
+ * gmm_set_clusters(ctx, ideal_K, saved) followed by gmm_score.               */
+int  gmm_score(gmm_ctx*, int K, const float* events_aos, long long n,
+               int* labels, float* max_resp, float* logp, double* loglik_out);
+/* Since the last reset: out[0] score-kernel ms, out[1] wall ms inside
+ * gmm_score, out[2] chunks scored by the wgmma kernel, out[3] chunks scored
+ * by the SIMT kernel (including re-scored ones, which out[2] then omits).   */
+int  gmm_get_score_profile(gmm_ctx*, double out[4], int reset);
 
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
