@@ -307,6 +307,43 @@ struct ScoreBuffers {
     }
 };
 
+// gmm_score_stats' own buffers (its input stage is gmm_score's two pinned slots and device chunks): ONE compute-side chunk
+// (the kernels of consecutive chunks are serialised on the compute stream), the statistics it adds up, the range flag and,
+// on the first call that asks for memberships, their pinned mirror.
+struct ScoreStatsBuffers {
+    long long cap = 0;                          // events per chunk
+    size_t pitch = 0;                           // row pitch in floats of the SoA copies and the responsibilities (multiple of 32)
+    float* d_z = nullptr;                       // [D][pitch] standardised SoA copy (tensor M-step)
+    float* d_xs = nullptr;                      // [D][pitch] raw SoA copy (SIMT kernels)
+    float* d_memb = nullptr;                    // [8 ceil(Kmax / 8)][pitch] responsibilities of the chunk
+    float* h_memb = nullptr;                    // pinned [Kmax][cap]
+    double* d_stats = nullptr;                  // [Kmax F + 1]
+    double* h_stats = nullptr;                  // pinned
+    int* d_flag = nullptr;
+    int* h_flag = nullptr;                      // pinned
+    cudaEvent_t ev_flag = nullptr;
+    cudaEvent_t p0[2] = {nullptr, nullptr}, p1[2] = {nullptr, nullptr}, k0[2] = {nullptr, nullptr}, k1[2] = {nullptr, nullptr};
+    double kernel_ms = 0, wall_ms = 0, wait_ms = 0;   // gmm_get_score_stats_profile
+    long long e_tensor = 0, e_simt = 0, m_tensor = 0, m_simt = 0;
+    void release_chunk() {
+        cudaFree(d_z); cudaFree(d_xs); cudaFree(d_memb);
+        if (h_memb) cudaFreeHost(h_memb);
+        d_z = d_xs = d_memb = h_memb = nullptr;
+        cap = 0; pitch = 0;
+    }
+    void destroy() {
+        release_chunk();
+        cudaFree(d_stats); cudaFree(d_flag);
+        if (h_stats) cudaFreeHost(h_stats);
+        if (h_flag) cudaFreeHost(h_flag);
+        d_stats = h_stats = nullptr; d_flag = h_flag = nullptr;
+        if (ev_flag) { cudaEventDestroy(ev_flag); ev_flag = nullptr; }
+        for (int b = 0; b < 2; b++)
+            for (cudaEvent_t* e : {&p0[b], &p1[b], &k0[b], &k1[b]})
+                if (*e) { cudaEventDestroy(*e); *e = nullptr; }
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -377,7 +414,8 @@ struct gmm_ctx {
     int fin_fault_iter = -1;     // option "finalize_fault_iter" (tests): that iteration of the next batch reports a failure
     bool params_partial = false; // gmm_mstep has updated N, means, R but not yet Rinv / constants / the operand (upload_params clears)
     ScoreBuffers score;          // gmm_score: streaming buffers, allocated on first use
-    long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score
+    long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score / gmm_score_stats
+    ScoreStatsBuffers sstats;    // gmm_score_stats: chunk buffers, allocated on first use
 };
 
 namespace gmm {
@@ -519,16 +557,16 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
 }
 
 // ---- kernel dispatch -------------------------------------------------------
+// SIMT E-step over n events of the SoA copy xs [D][pitch] into memb [K][pitch] (the shard's, or a gmm_score_stats chunk's)
 template <int D>
-static void launch_estep_simt_d(gmm_ctx* c, int K) {
-    const int blocks = (c->n + kEstepThreads - 1) / kEstepThreads;
-    estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(c->d_x_soa, c->memb_pitch, c->n, K, c->d_epack, c->d_memb, c->memb_pitch,
-                                                                 c->d_stats + (size_t)K * c->F);
+static void launch_estep_simt_d(gmm_ctx* c, int K, const float* xs, int n, float* memb, size_t pitch, double* ll) {
+    const int blocks = (n + kEstepThreads - 1) / kEstepThreads;
+    estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, c->d_epack, memb, pitch, ll);
 }
-static int launch_estep_simt(gmm_ctx* c, int K) {
-    if (c->n == 0) return GMM_OK;
+static int launch_estep_simt_on(gmm_ctx* c, int K, const float* xs, int n, float* memb, size_t pitch, double* ll) {
+    if (n == 0) return GMM_OK;
     switch (c->D) {
-#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K); break;
+#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K, xs, n, memb, pitch, ll); break;
         GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
         GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
         GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
@@ -538,6 +576,9 @@ static int launch_estep_simt(gmm_ctx* c, int K) {
     }
     CUDA_TRY(cudaGetLastError());
     return GMM_OK;
+}
+static int launch_estep_simt(gmm_ctx* c, int K) {
+    return launch_estep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F);
 }
 
 template <int D>
@@ -560,8 +601,9 @@ static int launch_score_simt(gmm_ctx* c, int K, const TcScoreIo& io) {
     return GMM_OK;
 }
 
+// FP64 SIMT M-step over n events of the SoA copy xs and the responsibilities memb (both [..][pitch]), adding into stats
 template <int JMAX, int CPT>
-static int launch_mstep_simt_t(gmm_ctx* c, int K) {
+static int launch_mstep_simt_t(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats) {
     constexpr int FP = 16 * JMAX, KT = 16 * CPT, GS = KT + 2;
     const size_t smem = sizeof(double) * (size_t)(kMstepTE * FP + kMstepTE * GS + kMstepTE * GMM_MAX_DIMENSIONS) +
                         sizeof(short) * 2 * FP;
@@ -572,36 +614,40 @@ static int launch_mstep_simt_t(gmm_ctx* c, int K) {
         if (c->device < 64) attr_set[c->device] = true;
     }
     int gx = c->num_sms;
-    int per = (c->n + gx - 1) / gx;
+    int per = (n + gx - 1) / gx;
     per = (per + kMstepTE - 1) / kMstepTE * kMstepTE;
     if (per < kMstepTE) per = kMstepTE;
-    gx = (c->n + per - 1) / per;
+    gx = (n + per - 1) / per;
     dim3 grid(gx, (K + KT - 1) / KT);
-    mstep_simt_kernel<JMAX, CPT><<<grid, kMstepThreads, smem, c->stream>>>(c->d_x_soa, c->memb_pitch, c->n, c->D, K, c->d_memb, c->memb_pitch,
-                                                                           c->d_shift, c->d_stats, per);
+    mstep_simt_kernel<JMAX, CPT><<<grid, kMstepThreads, smem, c->stream>>>(xs, pitch, n, c->D, K, memb, pitch, c->d_shift, stats, per);
     CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
-static int launch_mstep_simt(gmm_ctx* c, int K) {
-    if (c->n == 0) return GMM_OK;
+static int launch_mstep_simt_on(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats) {
+    if (n == 0) return GMM_OK;
     const int F = c->F;
     const int cpt = K <= 16 ? 1 : (K <= 32 ? 2 : 4);
+#define GMM_MS(j, p) return launch_mstep_simt_t<j, p>(c, K, xs, n, memb, pitch, stats)
     if (F <= 48) {
-        if (cpt == 1) return launch_mstep_simt_t<3, 1>(c, K);
-        if (cpt == 2) return launch_mstep_simt_t<3, 2>(c, K);
-        return launch_mstep_simt_t<3, 4>(c, K);
+        if (cpt == 1) GMM_MS(3, 1);
+        if (cpt == 2) GMM_MS(3, 2);
+        GMM_MS(3, 4);
     } else if (F <= 160) {
-        if (cpt == 1) return launch_mstep_simt_t<10, 1>(c, K);
-        if (cpt == 2) return launch_mstep_simt_t<10, 2>(c, K);
-        return launch_mstep_simt_t<10, 4>(c, K);
+        if (cpt == 1) GMM_MS(10, 1);
+        if (cpt == 2) GMM_MS(10, 2);
+        GMM_MS(10, 4);
     } else if (F <= 336) {
-        if (cpt == 1) return launch_mstep_simt_t<21, 1>(c, K);
-        if (cpt == 2) return launch_mstep_simt_t<21, 2>(c, K);
-        return launch_mstep_simt_t<21, 4>(c, K);
+        if (cpt == 1) GMM_MS(21, 1);
+        if (cpt == 2) GMM_MS(21, 2);
+        GMM_MS(21, 4);
     } else {
-        if (cpt == 1) return launch_mstep_simt_t<36, 1>(c, K);
-        return launch_mstep_simt_t<36, 2>(c, K);
+        if (cpt == 1) GMM_MS(36, 1);
+        GMM_MS(36, 2);
     }
+#undef GMM_MS
+}
+static int launch_mstep_simt(gmm_ctx* c, int K) {
+    return launch_mstep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats);
 }
 
 static int zero_stats(gmm_ctx* c, int K) {
@@ -898,6 +944,7 @@ void gmm_destroy(gmm_ctx* c) {
     if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
     tc_destroy(c->tc);
     c->score.destroy();
+    c->sstats.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -1514,6 +1561,180 @@ int gmm_get_score_profile(gmm_ctx* c, double out[4], int reset) {
     ScoreBuffers& s = c->score;
     out[0] = s.kernel_ms; out[1] = s.wall_ms; out[2] = (double)s.tensor_chunks; out[3] = (double)s.simt_chunks;
     if (reset) { s.kernel_ms = s.wall_ms = 0; s.tensor_chunks = s.simt_chunks = 0; }
+    return GMM_OK;
+}
+
+// ---- E-step + M-step statistics of new events ---------------------------------------------------------------------------
+static int score_stats_buffers(gmm_ctx* c, bool with_memberships) {
+    ScoreStatsBuffers& t = c->sstats;
+    if (!t.ev_flag) {
+        CUDA_TRY(cudaEventCreateWithFlags(&t.ev_flag, cudaEventDisableTiming));
+        for (int b = 0; b < 2; b++)
+            for (cudaEvent_t* e : {&t.p0[b], &t.p1[b], &t.k0[b], &t.k1[b]}) CUDA_TRY(cudaEventCreate(e));
+        CUDA_TRY(cudaMalloc(&t.d_stats, sizeof(double) * ((size_t)c->Kmax * c->F + 1)));
+        CUDA_TRY(cudaMallocHost(&t.h_stats, sizeof(double) * ((size_t)c->Kmax * c->F + 1)));
+        CUDA_TRY(cudaMalloc(&t.d_flag, sizeof(int)));
+        CUDA_TRY(cudaMallocHost(&t.h_flag, sizeof(int)));
+    }
+    const long long want = c->score_chunk;
+    if (t.cap < want) {
+        t.release_chunk();
+        const size_t pitch = ((size_t)want + 31) / 32 * 32, rows = (size_t)(c->Kmax + 7) / 8 * 8;
+        CUDA_TRY(cudaMalloc(&t.d_z, sizeof(float) * pitch * c->D));
+        CUDA_TRY(cudaMalloc(&t.d_xs, sizeof(float) * pitch * c->D));
+        CUDA_TRY(cudaMalloc(&t.d_memb, sizeof(float) * pitch * rows));
+        // rows above K that no E-step of this call writes are read by the tensor M-step's 32-cluster boxes (their columns
+        // are discarded): keep them finite
+        CUDA_TRY(cudaMemsetAsync(t.d_memb, 0, sizeof(float) * pitch * rows, c->stream));
+        t.cap = want;
+        t.pitch = pitch;
+    }
+    if (with_memberships && !t.h_memb) CUDA_TRY(cudaMallocHost(&t.h_memb, sizeof(float) * (size_t)c->Kmax * t.cap));
+    return GMM_OK;
+}
+
+// Per chunk i (slot b = i & 1 of gmm_score's input stage), in order on the compute stream: prep kernel (SoA copies + range
+// flag) -> flag to the host, while chunk i + 1 is staged and its H2D issued -> the kernels the flag allows -> E-step into the
+// chunk's responsibilities -> M-step adding into the call's statistics -> (memberships) pitched D2H and rows to the caller.
+static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bool with_stats, float* memberships) {
+    ScoreBuffers& s = c->score;
+    ScoreStatsBuffers& t = c->sstats;
+    const int D = c->D;
+    const size_t KF = (size_t)K * c->F;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
+    const bool e_tensor = c->estep_tensor_ready;
+    const bool m_tensor = with_stats && use_tensor_mstep(c, K);
+    const bool raw_always = !e_tensor || (with_stats && !m_tensor);   // the context's own selection puts a SIMT kernel on every chunk
+    const float* shift_f = (e_tensor || m_tensor) ? tc_shift_f(c->tc) : nullptr;
+    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
+    if ((e_tensor || m_tensor) && !shift_f) return fail(GMM_ERR_STATE, "gmm_score_stats: the tensor kernels have no centre");
+    bool epack_ready = !e_tensor;          // while the tensor operand serves the parameters d_epack is not maintained
+    CUDA_TRY(cudaMemsetAsync(t.d_stats, 0, sizeof(double) * (KF + 1), c->stream));
+    auto rows_of = [&](long long i) { return (int)std::min(chunk, n - i * chunk); };
+    auto stage = [&](long long i) -> int {
+        const int b = (int)(i & 1), m = rows_of(i);
+        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
+        std::memcpy(s.h_in[b], ev + (size_t)(i * chunk) * D, sizeof(float) * (size_t)m * D);
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the device chunk's previous readers are done with it
+        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyHostToDevice, s.copy));
+        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
+        return GMM_OK;
+    };
+    auto collect = [&](int b) {                                   // timings of a chunk whose kernels have finished
+        float a = 0, k = 0, w = 0;
+        if (cudaEventElapsedTime(&a, t.p0[b], t.p1[b]) == cudaSuccess && cudaEventElapsedTime(&k, t.k0[b], t.k1[b]) == cudaSuccess)
+            t.kernel_ms += (double)a + (double)k;
+        if (cudaEventElapsedTime(&w, t.p1[b], t.k0[b]) == cudaSuccess) t.wait_ms += w;
+    };
+    if (nchunks > 0)
+        if (int rc = stage(0)) return rc;
+    for (long long i = 0; i < nchunks; i++) {
+        const int b = (int)(i & 1), m = rows_of(i);
+        const long long e0 = i * chunk;
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
+        CUDA_TRY(cudaMemsetAsync(t.d_flag, 0, sizeof(int), c->stream));
+        CUDA_TRY(cudaEventRecord(t.p0[b], c->stream));
+        score_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(
+            s.d_in[b], m, D, shift_f, shift_f ? tc_inv_scale_f(c->tc) : nullptr, zb, m_tensor ? t.d_z : nullptr,
+            raw_always ? t.d_xs : nullptr, t.pitch, t.d_flag);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaEventRecord(t.p1[b], c->stream));
+        CUDA_TRY(cudaMemcpyAsync(t.h_flag, t.d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaEventRecord(t.ev_flag, c->stream));
+        if (i + 1 < nchunks)
+            if (int rc = stage(i + 1)) return rc;
+        CUDA_TRY(cudaEventSynchronize(t.ev_flag));
+        if (i > 0) collect(b ^ 1);                                // (the prep of chunk i ran after chunk i - 1's kernels)
+        const int flag = *t.h_flag;
+        if (flag & kScoreStatsNotFinite) return fail(GMM_ERR_ARG, "gmm_score_stats: an event has a coordinate that is not finite");
+        const bool ce = e_tensor && !(flag & kScoreStatsBeyondFp16);
+        const bool cm = m_tensor && !(flag & kScoreStatsBeyondZb);
+        if (e_tensor && !ce && estep_path_of(c) == GMM_PATH_TENSOR)
+            return fail(GMM_ERR_STATE, "gmm_score_stats: an event lies beyond 2^14 standard deviations (the tensor E-step's FP16 "
+                                       "operand range) and estep_path is GMM_PATH_TENSOR");
+        if (m_tensor && !cm && mstep_path_of(c) == GMM_PATH_TENSOR)
+            return fail(GMM_ERR_STATE, "gmm_score_stats: an event lies beyond the tensor M-step's fixed-point range (|z| >= the "
+                                       "training data's bound) and mstep_path is GMM_PATH_TENSOR");
+        if (!ce && !epack_ready) {
+            build_epack(K, D, &c->host, c->h_epack);
+            CUDA_TRY(cudaMemcpyAsync(c->d_epack, c->h_epack, sizeof(float) * (size_t)K * epack_stride(D), cudaMemcpyHostToDevice, c->stream));
+            epack_ready = true;
+        }
+        CUDA_TRY(cudaEventRecord(t.k0[b], c->stream));
+        if (!raw_always && (!ce || (with_stats && !cm))) {       // a fallback of this chunk only: its raw SoA copy now
+            transpose_aos_to_soa_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], t.d_xs, t.pitch, m, D);
+            CUDA_TRY(cudaGetLastError());
+        }
+        int rc = ce ? tc_launch_estep_on(c->tc, K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
+                    : launch_estep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
+        if (rc) return rc;
+        (ce ? t.e_tensor : t.e_simt)++;
+        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
+        if (with_stats) {
+            rc = cm ? tc_launch_mstep_on(c->tc, K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
+                    : launch_mstep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats);
+            if (rc) return rc;
+            (cm ? t.m_tensor : t.m_simt)++;
+        }
+        CUDA_TRY(cudaEventRecord(t.k1[b], c->stream));
+        if (memberships) {
+            CUDA_TRY(cudaMemcpy2DAsync(t.h_memb, sizeof(float) * (size_t)m, t.d_memb, sizeof(float) * t.pitch, sizeof(float) * (size_t)m, K,
+                                       cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(cudaStreamSynchronize(c->stream));
+            for (int k = 0; k < K; k++)
+                std::memcpy(memberships + (size_t)k * n + e0, t.h_memb + (size_t)k * m, sizeof(float) * (size_t)m);
+        }
+    }
+    if (with_stats) CUDA_TRY(cudaMemcpyAsync(t.h_stats, t.d_stats, sizeof(double) * (KF + 1), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (nchunks > 0) collect((int)((nchunks - 1) & 1));
+    return GMM_OK;
+}
+
+int gmm_score_stats(gmm_ctx* c, int K, const float* events_aos, long long n, double* stats_out, double* shift_out, float* memberships) {
+    if (int rc = check_K(c, K, "gmm_score_stats")) return rc;
+    if (n < 0 || (n > 0 && !events_aos)) return fail(GMM_ERR_ARG, "gmm_score_stats: bad events (n < 0, or no rows)");
+    if (!stats_out && !memberships) return fail(GMM_ERR_ARG, "gmm_score_stats: neither statistics nor memberships requested");
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_score_stats: parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, "gmm_score_stats: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!c->have_shift) {
+        // the centre comes from the global column moments, an all-reduce over the ranks: never issued from here
+        if (c->nranks > 1)
+            return fail(GMM_ERR_STATE, "gmm_score_stats: the context's centre is not fixed yet (run gmm_mstep or gmm_em first on every rank)");
+        if (int rc = ensure_moments(c)) return rc;
+    }
+    const size_t len = (size_t)K * c->F + 1;
+    int rc = GMM_OK;
+    if (n > 0) {
+        rc = score_buffers(c);
+        if (rc == GMM_OK) rc = score_stats_buffers(c, memberships != nullptr);
+        if (rc == GMM_OK) rc = score_stats_batch(c, K, events_aos, n, stats_out != nullptr, memberships);
+        // nothing of this call may still be in flight when it returns (also after a failure)
+        const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
+        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = fail(GMM_ERR_CUDA, std::string("gmm_score_stats: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    if (rc == GMM_OK) {
+        if (stats_out) {
+            if (n > 0) std::memcpy(stats_out, c->sstats.h_stats, sizeof(double) * len);
+            else std::fill(stats_out, stats_out + len, 0.0);
+        }
+        if (shift_out) std::memcpy(shift_out, c->shift, sizeof(double) * (size_t)c->D);
+    }
+    c->sstats.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_get_score_stats_profile(gmm_ctx* c, double out[7], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_score_stats_profile: bad argument");
+    ScoreStatsBuffers& t = c->sstats;
+    out[0] = t.kernel_ms; out[1] = t.wall_ms;
+    out[2] = (double)t.e_tensor; out[3] = (double)t.e_simt; out[4] = (double)t.m_tensor; out[5] = (double)t.m_simt;
+    out[6] = t.wait_ms;
+    if (reset) { t.kernel_ms = t.wall_ms = t.wait_ms = 0; t.e_tensor = t.e_simt = t.m_tensor = t.m_simt = 0; }
     return GMM_OK;
 }
 

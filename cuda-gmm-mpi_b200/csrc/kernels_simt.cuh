@@ -297,6 +297,44 @@ __global__ void transpose_aos_to_soa_kernel(const float* __restrict__ aos, float
     }
 }
 
+// Chunk preparation of gmm_score_stats: ONE pass over a chunk's AoS rows [n][D] (D <= 32) that writes
+//   z_soa[d][e] = (x - shift_f) * inv_scale_f   the operations of standardise_soa_kernel, so z is bit-identical to the
+//                                               resident copy the tensor M-step reads (when z_soa != NULL);
+//   x_soa[d][e] = x                             the raw copy the SIMT kernels read (when x_soa != NULL);
+//   *flag |= 1 an event with a coordinate that is not finite, 2 a |z_d| beyond 2^14 (the tensor E-step's FP16 event operand),
+//            4 a |z_d| >= zb (the tensor M-step's fixed-point quanta: 11 + 6 + 7 bits hold for |z| < zb only).
+// Bits 2 and 4 need shift_f / inv_scale_f (NULL: not tested).  Block (32, 8): a 32-event tile read as one contiguous run of
+// 32 * D floats, written as D rows of 32 events.
+constexpr int kScoreStatsNotFinite = 1, kScoreStatsBeyondFp16 = 2, kScoreStatsBeyondZb = 4;
+__global__ void __launch_bounds__(256)
+score_stats_prep_kernel(const float* __restrict__ aos, int n, int D, const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f,
+                        float zb, float* __restrict__ z_soa, float* __restrict__ x_soa, size_t pitch, int* __restrict__ flag) {
+    __shared__ float tile[32][33];
+    const int e0 = blockIdx.x * 32;
+    const int rows = min(32, n - e0);
+    const int tid = threadIdx.y * 32 + threadIdx.x;
+    const float* src = aos + (size_t)e0 * D;
+    for (int i = tid; i < rows * D; i += 256) tile[i / D][i % D] = src[i];
+    __syncthreads();
+    const int e = e0 + threadIdx.x;
+    int bits = 0;
+    if (threadIdx.x < rows) {
+        for (int d = threadIdx.y; d < D; d += 8) {
+            const float x = tile[threadIdx.x][d];
+            if (!isfinite(x)) bits |= kScoreStatsNotFinite;
+            if (x_soa) x_soa[(size_t)d * pitch + e] = x;
+            if (shift_f) {
+                const float z = __fmul_rn(__fsub_rn(x, shift_f[d]), inv_scale_f[d]);
+                if (!(fabsf(z) <= 16384.0f)) bits |= kScoreStatsBeyondFp16;
+                if (!(fabsf(z) < zb)) bits |= kScoreStatsBeyondZb;
+                if (z_soa) z_soa[(size_t)d * pitch + e] = z;
+            }
+        }
+    }
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (bits && threadIdx.x == 0) atomicOr(flag, bits);
+}
+
 // Column sums for seeding: out[d] += sum x, out[D+d] += sum x^2 (double); column extremes:
 // out[2D+d] = max x, out[3D+d] = max (-x) (initialised to -DBL_MAX by the caller).
 // Replaces mvtmeans / averageVariance (gaussian_kernel.cu:54-102), which scan

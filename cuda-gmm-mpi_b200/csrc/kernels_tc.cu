@@ -940,6 +940,11 @@ struct TcState {
     float zmax[GMM_MAX_DIMENSIONS] = {0};    // power-of-two bound of |z_d| over the whole data set
     MMagic magic{0.f, 0.f};          // rounding constants of the coordinate / product rows
     int3* d_rowmap = nullptr;        // [MT * 128] operand row -> (packed statistic, dimension i, dimension j)
+    CUtensorMap tm_cx{}, tm_cg{};    // tc_launch_mstep_on: maps over the caller's chunk buffers, for cmap_n events
+    const void* cmap_z = nullptr;
+    const void* cmap_g = nullptr;
+    size_t cmap_pitch = 0;
+    int cmap_n = -1;
     // E-step
     CUtensorMap tm_x128{};
     bool emap_ok = false;
@@ -1583,46 +1588,57 @@ int tc_launch_finalize(TcState* t, int K, const double* d_stats, const float* d_
 }
 
 template <int D>
-static int launch_estep_d(TcState* t, int K, double* d_ll, cudaStream_t stream) {
+static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, cudaStream_t stream) {
     using C = ECfg<D>;
     static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
     if (!t->attr_estep) {
         TC_CUDA_TRY(cudaFuncSetAttribute(estep_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_estep = true;
     }
-    const int ntiles = (t->n + 127) / 128;
+    const int ntiles = (n + 127) / 128;
     int grid = t->num_sms;
     if (grid > ntiles) grid = ntiles;
     if (grid < 1) grid = 1;
     const int NP = (K + 63) / 64;
-    if (NP > 1 && !t->d_den) return fail(GMM_ERR_STATE, "tensor E-step: context was created for at most 64 clusters");
+    if (NP > 1 && !den) return fail(GMM_ERR_STATE, "tensor E-step: context was created for at most 64 clusters");
     // P passes of 64 clusters: log-denominators of passes 0 .. P-2 (mode 1), then the last pass writes its final
     // responsibilities and the events' total log-denominators (mode 2, or mode 0 when P = 1), then passes 0 .. P-2 write
     // theirs against those totals (mode 3): 2P - 1 launches, every responsibility stored once
     auto launch = [&](int p, int mode, const float* den_in, float* den_out) {
         const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
         estep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
-            t->d_x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f,
-            t->d_memb + (size_t)(64 * p) * t->memb_pitch, t->memb_pitch, t->n, Kp, (Kp + C::GB - 1) / C::GB, d_ll, mode, den_in, den_out);
+            x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f,
+            memb + (size_t)(64 * p) * pitch, pitch, n, Kp, (Kp + C::GB - 1) / C::GB, d_ll, mode, den_in, den_out);
         return cudaGetLastError();
     };
     if (NP == 1) TC_CUDA_TRY(launch(0, 0, nullptr, nullptr));
     else {
-        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 1, p ? t->d_den : nullptr, t->d_den));
-        TC_CUDA_TRY(launch(NP - 1, 2, t->d_den, t->d_den));
-        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 3, t->d_den, nullptr));
+        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 1, p ? den : nullptr, den));
+        TC_CUDA_TRY(launch(NP - 1, 2, den, den));
+        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 3, den, nullptr));
     }
     return GMM_OK;
 }
 
-int tc_launch_estep(TcState* t, int K, double* d_ll, cudaStream_t stream) {
+static int launch_estep_any(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, cudaStream_t stream) {
     if (!t || !t->emap_ok) return fail(GMM_ERR_STATE, "tensor E-step not initialised for this shape");
     switch (t->D) {
-        case 8: return launch_estep_d<8>(t, K, d_ll, stream);
-        case 16: return launch_estep_d<16>(t, K, d_ll, stream);
-        case 24: return launch_estep_d<24>(t, K, d_ll, stream);
+        case 8: return launch_estep_d<8>(t, K, x, n, memb, pitch, den, d_ll, stream);
+        case 16: return launch_estep_d<16>(t, K, x, n, memb, pitch, den, d_ll, stream);
+        case 24: return launch_estep_d<24>(t, K, x, n, memb, pitch, den, d_ll, stream);
         default: return fail(GMM_ERR_ARG, "tensor E-step: unsupported D");
     }
+}
+
+int tc_launch_estep(TcState* t, int K, double* d_ll, cudaStream_t stream) {
+    if (!t) return fail(GMM_ERR_STATE, "tensor E-step not initialised for this shape");
+    return launch_estep_any(t, K, t->d_x, t->n, t->d_memb, t->memb_pitch, t->d_den, d_ll, stream);
+}
+
+int tc_launch_estep_on(TcState* t, int K, const float* d_x_aos, int n, float* d_memb, size_t pitch, float* d_den, double* d_ll,
+                       cudaStream_t stream) {
+    if (n <= 0) return GMM_OK;
+    return launch_estep_any(t, K, d_x_aos, n, d_memb, pitch, d_den, d_ll, stream);
 }
 
 template <int D>
@@ -1661,7 +1677,7 @@ int tc_launch_score(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream)
 }
 
 template <int D>
-static int launch_mstep_d(TcState* t, int K, double* d_stats, cudaStream_t stream) {
+static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, cudaStream_t stream) {
     using C = MCfg<D>;
     static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
     if (!t->attr_mstep) {
@@ -1669,32 +1685,58 @@ static int launch_mstep_d(TcState* t, int K, double* d_stats, cudaStream_t strea
         t->attr_mstep = true;
     }
     int gx = t->num_sms;
-    int per = (t->n + gx - 1) / gx;
+    int per = (n + gx - 1) / gx;
     per = (per + kTE - 1) / kTE * kTE;
-    gx = (t->n + per - 1) / per;
+    gx = (n + per - 1) / per;
     const int gy = (K + kNCL - 1) / kNCL;
     if ((size_t)gx * gy * C::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
     dim3 grid(gx, gy);
-    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(t->tm_x, t->tm_g, t->n, t->d_scratch, per, t->magic);
+    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tm_x, tm_g, n, t->d_scratch, per, t->magic);
     TC_CUDA_TRY(cudaGetLastError());
     mstep_tc_finalize_kernel<<<C::NCHUNK * 8, 256, 0, stream>>>(t->d_scratch, gx, C::MT, K, C::F, t->d_rowmap, t->d_scale, d_stats);
     TC_CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
 
-int tc_launch_mstep(TcState* t, int K, double* d_stats, cudaStream_t stream) {
+static int launch_mstep_any(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, cudaStream_t stream) {
     if (!t || !t->maps_ok) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
     if (!t->have_shift) return fail(GMM_ERR_STATE, "tensor-core M-step needs gmm_seed (shift/scale) first");
     if (!t->mstep_ready) return fail(GMM_ERR_STATE, "tensor-core M-step: the data range exceeds the fixed-point operand budget");
     switch (t->D) {
-        case 4: return launch_mstep_d<4>(t, K, d_stats, stream);
-        case 8: return launch_mstep_d<8>(t, K, d_stats, stream);
-        case 12: return launch_mstep_d<12>(t, K, d_stats, stream);
-        case 16: return launch_mstep_d<16>(t, K, d_stats, stream);
-        case 20: return launch_mstep_d<20>(t, K, d_stats, stream);
-        case 24: return launch_mstep_d<24>(t, K, d_stats, stream);
+        case 4: return launch_mstep_d<4>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 8: return launch_mstep_d<8>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 12: return launch_mstep_d<12>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 16: return launch_mstep_d<16>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 20: return launch_mstep_d<20>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 24: return launch_mstep_d<24>(t, K, tm_x, tm_g, n, d_stats, stream);
         default: return fail(GMM_ERR_ARG, "tensor-core M-step: unsupported D");
     }
+}
+
+int tc_launch_mstep(TcState* t, int K, double* d_stats, cudaStream_t stream) {
+    if (!t) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
+    return launch_mstep_any(t, K, t->tm_x, t->tm_g, t->n, d_stats, stream);
+}
+
+int tc_launch_mstep_on(TcState* t, int K, const float* d_z, const float* d_memb, size_t pitch, int n, double* d_stats, cudaStream_t stream) {
+    if (n <= 0) return GMM_OK;
+    if (!t || !t->maps_ok) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
+    if (t->cmap_z != d_z || t->cmap_g != d_memb || t->cmap_pitch != pitch || t->cmap_n != n) {
+        t->cmap_n = -1;
+        if (int rc = make_map_2d(&t->tm_cx, d_z, (uint64_t)n, (uint64_t)t->D, (uint64_t)pitch * 4, kTE, (uint32_t)t->D)) return rc;
+        if (int rc = make_map_2d(&t->tm_cg, d_memb, (uint64_t)n, (uint64_t)t->Kmax, (uint64_t)pitch * 4, kTE, kNCL, /*swizzle128=*/true)) return rc;
+        t->cmap_z = d_z; t->cmap_g = d_memb; t->cmap_pitch = pitch; t->cmap_n = n;
+    }
+    return launch_mstep_any(t, K, t->tm_cx, t->tm_cg, n, d_stats, stream);
+}
+
+const float* tc_shift_f(const TcState* t) { return t && t->have_shift ? t->d_shift_f : nullptr; }
+const float* tc_inv_scale_f(const TcState* t) { return t && t->have_shift ? t->d_inv_scale_f : nullptr; }
+float tc_mstep_zbound(const TcState* t) {
+    float zb = 0.f;
+    if (t)
+        for (int d = 0; d < t->D; d++) zb = std::fmax(zb, t->zmax[d]);
+    return zb;
 }
 
 }  // namespace gmm

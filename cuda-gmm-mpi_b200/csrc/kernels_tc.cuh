@@ -68,4 +68,20 @@ int  tc_launch_finalize(TcState*, int K, const double* d_stats, const float* d_a
 // Accumulates sum_n g[k][n] * phi_f(x_n - shift) into d_stats[k*F + f] (double, original units).
 int  tc_launch_mstep(TcState*, int K, double* d_stats, cudaStream_t stream);
 
+// The same two steps on caller-owned buffers (gmm_score_stats: chunks of new events, nothing of the state's buffers is
+// written except the M-step's per-launch scratch).  pitch: row pitch in floats of memb (and of z), a multiple of 32.
+//   estep: events [n][D] (device, AoS) -> memb [8 * ceil(K / 8)][pitch]; den: [n] floats of running log-denominator
+//          (K > 64 only); *d_ll += sum of the events' log-denominators.
+//   mstep: standardised SoA copy z [D][pitch] (tc_shift_f / tc_inv_scale_f) and memb [>= Kmax rows][pitch] of n events;
+//          adds into d_stats[0 .. K*F).  The tensor maps are encoded with n as their event extent (TMA's zero fill masks
+//          the tail), re-encoded only when the buffers or n change.
+int  tc_launch_estep_on(TcState*, int K, const float* d_x_aos, int n, float* d_memb, size_t pitch, float* d_den, double* d_ll,
+                        cudaStream_t stream);
+int  tc_launch_mstep_on(TcState*, int K, const float* d_z, const float* d_memb, size_t pitch, int n, double* d_stats, cudaStream_t stream);
+// Device copies of the float centre and inverse scale the tensor kernels use (NULL before tc_set_shift_scale), and the
+// power-of-two bound zb of |z| the M-step's fixed-point quanta were set from (max over the dimensions).
+const float* tc_shift_f(const TcState*);
+const float* tc_inv_scale_f(const TcState*);
+float tc_mstep_zbound(const TcState*);
+
 }  // namespace gmm

@@ -79,6 +79,8 @@ def load_library():
     L.gmm_get_fit_profile.argtypes = [C.c_void_p, _DP]
     L.gmm_score.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p, _DP]
     L.gmm_get_score_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_score_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gmm_get_score_stats_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
@@ -296,6 +298,28 @@ class Engine:
         out = (C.c_double * 4)()
         _check(self.lib.gmm_get_score_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], wall_ms=out[1], tensor_chunks=int(out[2]), simt_chunks=int(out[3]))
+
+    def score_stats(self, K, events, stats=True, memberships=False):
+        """E-step + M-step statistics of new events (gmm_score_stats) under the current K-cluster parameters.
+        Returns (stats [K*F+1] float64 or None, shift [D] float64, memberships [K][n] float32 or None).
+        host_finalize(stats, shift, cl, K) turns the statistics into N, pi, means, R, Rinv and constants
+        (regularised by cl.avgvar: set it to 0 for the raw per-sample covariances)."""
+        ev = np.ascontiguousarray(events, np.float32)
+        if ev.ndim != 2 or ev.shape[1] != self.D:
+            raise ValueError(f"events must be [n][{self.D}], got {ev.shape}")
+        n = ev.shape[0]
+        st = np.empty(stats_len(K, self.D), np.float64) if stats else None
+        sh = np.empty(self.D, np.float64)
+        mb = np.empty((K, n), np.float32) if memberships else None
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        _check(self.lib.gmm_score_stats(self.h, K, ev.ctypes.data if n else None, n, ptr(st), ptr(sh), ptr(mb)))
+        return st, sh, mb
+
+    def score_stats_profile(self, reset=False):
+        out = (C.c_double * 7)()
+        _check(self.lib.gmm_get_score_stats_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1], estep_tensor_chunks=int(out[2]), estep_simt_chunks=int(out[3]),
+                    mstep_tensor_chunks=int(out[4]), mstep_simt_chunks=int(out[5]), flag_wait_ms=out[6])
 
     def fit_profile(self):
         out = (C.c_double * 4)()

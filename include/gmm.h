@@ -204,6 +204,46 @@ int  gmm_score(gmm_ctx*, int K, const float* events_aos, long long n,
  * by the SIMT kernel (including re-scored ones, which out[2] then omits).   */
 int  gmm_get_score_profile(gmm_ctx*, double out[4], int reset);
 
+/* E-step + M-step statistics of n new events (host, row-major [n][D], NOT
+ * the context's shard) under the parameter set the next gmm_estep(ctx, K)
+ * would use.  No collective; nothing of the EM state changes (memberships,
+ * statistics, log-likelihood, gmm_get_profile, gmm_get_score_profile).
+ *   stats_out   [gmm_stats_len(K, D)] doubles: S0 | S1 | S2 per cluster about
+ *               the context's centre (the packed layout of gmm_host_finalize),
+ *               then the sum of the events' log-densities.  Overwritten, not
+ *               accumulated.  May be NULL (then no M-step work is done).
+ *   shift_out   [D] the centre s the statistics are about (the float-rounded
+ *               value the kernels use); may be NULL.
+ *   memberships [K][n] cluster-major (the clusters_t layout, so
+ *               gmm_write_results can write them); may be NULL.
+ * At least one of stats_out / memberships must be non-NULL.  Statistics of
+ * several calls (batches, ranks) about the same centre add up: summed and
+ * passed to gmm_host_finalize, then gmm_set_clusters, they make one EM
+ * iteration over data that never has to fit on the device.
+ * Kernels: those the context's own steps would use, chosen per chunk of option
+ * "score_chunk" events.  A chunk with an event beyond 2^14 standard
+ * deviations runs the SIMT E-step; one with an event at or beyond the
+ * training data's power-of-two bound zb (the tensor M-step's fixed-point
+ * range) runs the FP64 SIMT M-step; either fails with GMM_ERR_STATE when the
+ * step concerned is forced to GMM_PATH_TENSOR.  On the training shard, in one
+ * chunk, the memberships equal gmm_estep's bit for bit, and so do the
+ * statistics gmm_mstep's wgmma M-step forms.
+ * Errors: K outside [1, Kmax], n < 0, events_aos == NULL with n > 0, both
+ * outputs NULL, or a coordinate that is not finite -> GMM_ERR_ARG; K != the K
+ * of the current parameters, a call between gmm_mstep and gmm_constants, or a
+ * multi-rank context whose centre is not fixed yet (a SIMT-only context
+ * before its first gmm_mstep / gmm_em) -> GMM_ERR_STATE.  n = 0 gives zero
+ * statistics and fills shift_out.                                            */
+int  gmm_score_stats(gmm_ctx*, int K, const float* events_aos, long long n,
+                     double* stats_out, double* shift_out, float* memberships);
+/* Since the last reset: out[0] kernel ms (prep + E + M), out[1] wall ms,
+ * out[2] / out[3] chunks whose responsibilities came from the wgmma / SIMT
+ * E-step, out[4] / out[5] chunks whose statistics came from the wgmma /
+ * FP64 SIMT M-step, out[6] ms the compute stream stood between a chunk's prep
+ * kernel and its E-step: the range-flag round trip to the host plus the
+ * host's staging of the next chunk, which is issued before the flag is read. */
+int  gmm_get_score_stats_profile(gmm_ctx*, double out[7], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce

@@ -7,7 +7,12 @@ rate through gmm_score (4 D bytes in and 12 bytes out per event over PCIe, plus 
 pinned stages: expected to be bound by those copies), and the E-step's time at the same shape from gmm_get_profile.
 Prints the card's name, power limit and maximum SM clock (read-only nvidia-smi query) first.
 
-    python scripts/bench_score.py [--n 10000000] [--iters 5] [--repeats 3]
+--mode stats times gmm_score_stats instead, once with statistics only and once with memberships as well: the kernel time
+(prep + E-step + M-step) per 10M events, the host-to-host rate (4 D bytes in per event, plus 4 K bytes out with
+memberships), the per-chunk wait of the compute stream for the range flag, and the resident E-step + M-step time at the
+same shape from gmm_get_profile.
+
+    python scripts/bench_score.py [--mode score|stats] [--n 10000000] [--iters 5] [--repeats 3]
 """
 import argparse
 import json
@@ -59,11 +64,48 @@ def bench_shape(pkg, train, fresh, K, iters, repeats):
                 estep_ms_per_10M=round(estep_ms * 1e7 / train.shape[0], 3))
 
 
+def bench_stats_shape(pkg, train, fresh, K, iters, repeats):
+    n, D = fresh.shape
+    with pkg.Engine(train, K) as eng:
+        eng.seed(K)
+        eng.estep(K)
+        eng.em_iterations(K, iters)
+        eng.profile(reset=True)
+        for _ in range(repeats):
+            eng.estep(K)
+            eng.mstep(K)
+            eng.constants(K)
+        prof = eng.profile()
+        estep_ms, mstep_ms = prof["estep_ms"] / repeats, prof["mstep_ms"] / repeats
+        eng.score_stats(K, fresh[: min(n, 1 << 20)], memberships=True)     # warm-up: buffers, pinned mirror, attributes
+        out = dict(D=D, K=K, resident_estep_ms_per_10M=round(estep_ms * 1e7 / train.shape[0], 3),
+                   resident_mstep_ms_per_10M=round(mstep_ms * 1e7 / train.shape[0], 3))
+        for memb in (False, True):
+            kern, wall, wait, nchunks = [], [], [], 0
+            for _ in range(repeats):
+                eng.score_stats_profile(reset=True)
+                t0 = time.perf_counter()
+                eng.score_stats(K, fresh, memberships=memb)
+                wall.append(time.perf_counter() - t0)
+                p = eng.score_stats_profile()
+                kern.append(p["kernel_ms"])
+                wait.append(p["flag_wait_ms"])
+                nchunks = p["estep_tensor_chunks"] + p["estep_simt_chunks"]
+                path = f"E {'wgmma' if not p['estep_simt_chunks'] else 'SIMT/mixed'}, M {'wgmma' if not p['mstep_simt_chunks'] else 'FP64/mixed'}"
+            tag = "memb" if memb else "stats"
+            out[f"{tag}_path"] = path
+            out[f"{tag}_kernel_ms_per_10M"] = round(float(np.median(kern)) * 1e7 / n, 3)
+            out[f"{tag}_host_to_host_events_per_s"] = round(n / float(np.median(wall)))
+            out[f"{tag}_flag_wait_ms_per_chunk"] = round(float(np.median(wait)) / max(nchunks, 1), 4)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--n", type=int, default=10_000_000)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--mode", default="score", choices=["score", "stats"])
     a = ap.parse_args()
     pkg = entry.load_package()
     pkg.load_library()
@@ -75,7 +117,8 @@ def main():
             data = {D: (np.ascontiguousarray(both[:a.n]), np.ascontiguousarray(both[a.n:]))}
             del both
         train, fresh = data[D]
-        print(json.dumps(bench_shape(pkg, train, fresh, K, a.iters, a.repeats)), flush=True)
+        bench = bench_shape if a.mode == "score" else bench_stats_shape
+        print(json.dumps(bench(pkg, train, fresh, K, a.iters, a.repeats)), flush=True)
 
 
 if __name__ == "__main__":
