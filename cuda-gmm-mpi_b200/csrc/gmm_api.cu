@@ -31,6 +31,7 @@
 #include "../../include/gmm.h"
 #include "host_math.h"
 #include "kernels_simt.cuh"
+#include "kernels_seed.cuh"
 #include "kernels_tc.cuh"
 
 namespace gmm {
@@ -344,6 +345,36 @@ struct ScoreStatsBuffers {
     }
 };
 
+// gmm_seed_kmeans' buffers: allocated on its first call (the shard's size is fixed), freed by gmm_destroy.
+struct KmeansBuffers {
+    bool ready = false;
+    int nb = 0, nba = 0, nxfer = 0;             // blocks of the k-means++ kernels / of the assignment; slots of d_xfer
+    double* d_d2 = nullptr;                     // [n] squared distance to the nearest chosen centre
+    int* d_labels = nullptr;                    // [n] Lloyd labels
+    double* d_bsum = nullptr;                   // [nb] per-block sums of d2
+    double* d_bpot = nullptr;                   // [nb][kSeedMaxCand] per-block candidate potentials
+    int* d_bchanged = nullptr;                  // [nba] changed labels per assignment block
+    double* d_binertia = nullptr;               // [nba] distances per assignment block
+    float* d_cand = nullptr;                    // [kSeedMaxCand][D] candidate rows
+    SeedPick* d_pick = nullptr;                 // [kSeedMaxCand]
+    int* d_pick_idx = nullptr;                  // [kSeedMaxCand]
+    float* d_centres = nullptr;                 // [Kmax][D]
+    double* d_xfer = nullptr;                   // [nranks][16] zero-padded per-rank values
+    double* h_bsum = nullptr;                   // pinned mirrors
+    double* h_bpot = nullptr;
+    int* h_bchanged = nullptr;
+    double* h_binertia = nullptr;
+    SeedPick* h_pick = nullptr;
+    double* h_xfer = nullptr;
+    void destroy() {
+        cudaFree(d_d2); cudaFree(d_labels); cudaFree(d_bsum); cudaFree(d_bpot); cudaFree(d_bchanged); cudaFree(d_binertia);
+        cudaFree(d_cand); cudaFree(d_pick); cudaFree(d_pick_idx); cudaFree(d_centres); cudaFree(d_xfer);
+        for (void* p : {(void*)h_bsum, (void*)h_bpot, (void*)h_bchanged, (void*)h_binertia, (void*)h_pick, (void*)h_xfer})
+            if (p) cudaFreeHost(p);
+        *this = KmeansBuffers();
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -416,6 +447,7 @@ struct gmm_ctx {
     ScoreBuffers score;          // gmm_score: streaming buffers, allocated on first use
     long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score / gmm_score_stats
     ScoreStatsBuffers sstats;    // gmm_score_stats: chunk buffers, allocated on first use
+    KmeansBuffers kmeans;        // gmm_seed_kmeans: allocated on first use
 };
 
 namespace gmm {
@@ -945,6 +977,7 @@ void gmm_destroy(gmm_ctx* c) {
     tc_destroy(c->tc);
     c->score.destroy();
     c->sstats.destroy();
+    c->kmeans.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -1735,6 +1768,286 @@ int gmm_get_score_stats_profile(gmm_ctx* c, double out[7], int reset) {
     out[2] = (double)t.e_tensor; out[3] = (double)t.e_simt; out[4] = (double)t.m_tensor; out[5] = (double)t.m_simt;
     out[6] = t.wait_ms;
     if (reset) { t.kernel_ms = t.wall_ms = t.wait_ms = 0; t.e_tensor = t.e_simt = t.m_tensor = t.m_simt = 0; }
+    return GMM_OK;
+}
+
+// ---- k-means++ and Lloyd seeding ------------------------------------------------------------------------------------------
+static int kmeans_buffers(gmm_ctx* c) {
+    KmeansBuffers& b = c->kmeans;
+    if (b.ready) return GMM_OK;
+    const size_t n = (size_t)std::max(c->n, 1), D = (size_t)c->D;
+    b.nb = (int)((n + kSeedBlockEvents - 1) / kSeedBlockEvents);
+    b.nba = (int)((n + kAssignThreads - 1) / kAssignThreads);
+    b.nxfer = 16 * c->nranks;
+    CUDA_TRY(cudaMalloc(&b.d_d2, sizeof(double) * n));
+    CUDA_TRY(cudaMalloc(&b.d_labels, sizeof(int) * n));
+    CUDA_TRY(cudaMalloc(&b.d_bsum, sizeof(double) * b.nb));
+    CUDA_TRY(cudaMalloc(&b.d_bpot, sizeof(double) * b.nb * kSeedMaxCand));
+    CUDA_TRY(cudaMalloc(&b.d_bchanged, sizeof(int) * b.nba));
+    CUDA_TRY(cudaMalloc(&b.d_binertia, sizeof(double) * b.nba));
+    CUDA_TRY(cudaMalloc(&b.d_cand, sizeof(float) * kSeedMaxCand * D));
+    CUDA_TRY(cudaMalloc(&b.d_pick, sizeof(SeedPick) * kSeedMaxCand));
+    CUDA_TRY(cudaMalloc(&b.d_pick_idx, sizeof(int) * kSeedMaxCand));
+    CUDA_TRY(cudaMalloc(&b.d_centres, sizeof(float) * (size_t)c->Kmax * D));
+    CUDA_TRY(cudaMalloc(&b.d_xfer, sizeof(double) * b.nxfer));
+    CUDA_TRY(cudaMallocHost(&b.h_bsum, sizeof(double) * b.nb));
+    CUDA_TRY(cudaMallocHost(&b.h_bpot, sizeof(double) * b.nb * kSeedMaxCand));
+    CUDA_TRY(cudaMallocHost(&b.h_bchanged, sizeof(int) * b.nba));
+    CUDA_TRY(cudaMallocHost(&b.h_binertia, sizeof(double) * b.nba));
+    CUDA_TRY(cudaMallocHost(&b.h_pick, sizeof(SeedPick) * kSeedMaxCand));
+    CUDA_TRY(cudaMallocHost(&b.h_xfer, sizeof(double) * b.nxfer));
+    b.ready = true;
+    return GMM_OK;
+}
+
+// Every rank's m (<= 16) values on every host: one all-reduce of a zero-padded [nranks][m] vector (each slot has one
+// non-zero contributor, so the sum is exact).  Callers add the ranks' values in rank order: every rank forms the same bits.
+static int kmeans_rank_values(gmm_ctx* c, const double* mine, int m, std::vector<double>& all) {
+    KmeansBuffers& b = c->kmeans;
+    all.assign((size_t)c->nranks * m, 0.0);
+    std::copy(mine, mine + m, all.begin() + (size_t)c->rank * m);
+    if (c->nranks == 1) return GMM_OK;
+    const size_t len = (size_t)c->nranks * m;
+    std::copy(all.begin(), all.end(), b.h_xfer);
+    CUDA_TRY(cudaMemcpyAsync(b.d_xfer, b.h_xfer, sizeof(double) * len, cudaMemcpyHostToDevice, c->stream));
+    ncclResult_t r = nccl().AllReduce(b.d_xfer, b.d_xfer, len, ncclDouble, ncclSum, c->comm, c->stream);
+    if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+    CUDA_TRY(cudaMemcpyAsync(b.h_xfer, b.d_xfer, sizeof(double) * len, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    std::copy(b.h_xfer, b.h_xfer + len, all.begin());
+    return GMM_OK;
+}
+
+// Sum of `count` floats over the ranks (rows that only their owner filled in, zeros elsewhere).
+static int kmeans_sum_rows(gmm_ctx* c, float* d_rows, size_t count) {
+    if (c->nranks == 1) return GMM_OK;
+    ncclResult_t r = nccl().AllReduce(d_rows, d_rows, count, ncclFloat, ncclSum, c->comm, c->stream);
+    if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+    return GMM_OK;
+}
+
+#define GMM_SEED_DISPATCH(D, CALL)                                                                                         \
+    switch (D) {                                                                                                           \
+        GMM_SEED_CASE(1, CALL) GMM_SEED_CASE(2, CALL) GMM_SEED_CASE(3, CALL) GMM_SEED_CASE(4, CALL)                      \
+        GMM_SEED_CASE(5, CALL) GMM_SEED_CASE(6, CALL) GMM_SEED_CASE(7, CALL) GMM_SEED_CASE(8, CALL)                      \
+        GMM_SEED_CASE(9, CALL) GMM_SEED_CASE(10, CALL) GMM_SEED_CASE(11, CALL) GMM_SEED_CASE(12, CALL)                   \
+        GMM_SEED_CASE(13, CALL) GMM_SEED_CASE(14, CALL) GMM_SEED_CASE(15, CALL) GMM_SEED_CASE(16, CALL)                  \
+        GMM_SEED_CASE(17, CALL) GMM_SEED_CASE(18, CALL) GMM_SEED_CASE(19, CALL) GMM_SEED_CASE(20, CALL)                  \
+        GMM_SEED_CASE(21, CALL) GMM_SEED_CASE(22, CALL) GMM_SEED_CASE(23, CALL) GMM_SEED_CASE(24, CALL)                  \
+        GMM_SEED_CASE(25, CALL) GMM_SEED_CASE(26, CALL) GMM_SEED_CASE(27, CALL) GMM_SEED_CASE(28, CALL)                  \
+        GMM_SEED_CASE(29, CALL) GMM_SEED_CASE(30, CALL) GMM_SEED_CASE(31, CALL) GMM_SEED_CASE(32, CALL)                  \
+        default: return fail(GMM_ERR_ARG, "unsupported dimension count");                                                 \
+    }
+#define GMM_SEED_CASE(d, CALL) case d: CALL(d); break;
+
+static int kmeanspp_update(gmm_ctx* c, const float* d_centre, bool first) {
+    KmeansBuffers& b = c->kmeans;
+    if (c->n == 0) return GMM_OK;
+#define GMM_CALL(d) kmeanspp_update_kernel<d><<<b.nb, kSeedThreads, 0, c->stream>>>(c->d_x_soa, c->memb_pitch, c->n, d_centre, \
+                                                                                      first ? 1 : 0, b.d_d2, b.d_bsum)
+    GMM_SEED_DISPATCH(c->D, GMM_CALL)
+#undef GMM_CALL
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+
+static int kmeanspp_potential(gmm_ctx* c, int L) {
+    KmeansBuffers& b = c->kmeans;
+    if (c->n == 0) return GMM_OK;
+#define GMM_CALL(d) kmeanspp_potential_kernel<d><<<b.nb, kSeedThreads, 0, c->stream>>>(c->d_x_soa, c->memb_pitch, c->n, b.d_cand, L, \
+                                                                                         b.d_d2, b.d_bpot)
+    GMM_SEED_DISPATCH(c->D, GMM_CALL)
+#undef GMM_CALL
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+
+static int kmeans_assign_launch(gmm_ctx* c, int K, int Kw) {
+    KmeansBuffers& b = c->kmeans;
+    if (c->n == 0) return GMM_OK;
+#define GMM_CALL(d) kmeans_assign_kernel<d><<<b.nba, kAssignThreads, 0, c->stream>>>(c->d_x_soa, c->memb_pitch, c->n, b.d_centres, K, \
+                                                                                       Kw, c->d_memb, c->memb_pitch, b.d_labels,    \
+                                                                                       b.d_bchanged, b.d_binertia)
+    GMM_SEED_DISPATCH(c->D, GMM_CALL)
+#undef GMM_CALL
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+#undef GMM_SEED_CASE
+#undef GMM_SEED_DISPATCH
+
+// splitmix64; each draw u = (next >> 11) * 2^-53 in [0, 1).  Every rank draws the same sequence.
+struct SplitMix64 {
+    unsigned long long s;
+    double uniform() {
+        unsigned long long z = (s += 0x9E3779B97F4A7C15ULL);
+        z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ULL;
+        z = (z ^ (z >> 27)) * 0x94D049BB133111EBULL;
+        z ^= z >> 31;
+        return (double)(z >> 11) * 0x1.0p-53;
+    }
+};
+
+// Greedy k-means++ (sklearn's rule) into kmeans.d_centres [K][D].  Per round: block sums of d2 -> host, T summed in rank
+// then block order; L = 2 + floor(ln K) targets u T, each resolved on the rank that owns it (first event whose inclusive
+// prefix exceeds the target; if rounding leaves none, the last event with d2 > 0); the candidates' potentials
+// sum min(d2, d(x, c_l)) all-reduced; the lowest potential wins (lowest l on ties); d2 takes the winner in.
+static int kmeanspp_run(gmm_ctx* c, int K, unsigned long long seed) {
+    KmeansBuffers& b = c->kmeans;
+    const int D = c->D, L = std::min(kSeedMaxCand, 2 + (int)std::floor(std::log((double)K)));
+    SplitMix64 rng{seed};
+    const long long g0 = std::min((long long)(rng.uniform() * (double)c->n_global), c->n_global - 1);
+    CUDA_TRY(cudaMemsetAsync(b.d_centres, 0, sizeof(float) * (size_t)K * D, c->stream));
+    if (g0 >= c->offset && g0 < c->offset + c->n)
+        CUDA_TRY(cudaMemcpyAsync(b.d_centres, c->d_x_aos + (size_t)(g0 - c->offset) * D, sizeof(float) * D, cudaMemcpyDeviceToDevice, c->stream));
+    if (int rc = kmeans_sum_rows(c, b.d_centres, (size_t)D)) return rc;
+    if (K > 1)
+        if (int rc = kmeanspp_update(c, b.d_centres, true)) return rc;
+    std::vector<double> all, prefix((size_t)b.nb);
+    for (int k = 1; k < K; k++) {
+        // T: this rank's block sums in block order, then the ranks in rank order
+        if (c->n > 0) CUDA_TRY(cudaMemcpyAsync(b.h_bsum, b.d_bsum, sizeof(double) * b.nb, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));
+        const int nb = c->n > 0 ? b.nb : 0;
+        double Tr = 0.0;
+        for (int i = 0; i < nb; i++) Tr += b.h_bsum[i];
+        if (int rc = kmeans_rank_values(c, &Tr, 1, all)) return rc;
+        double T = 0.0, base = 0.0;
+        std::vector<double> Q((size_t)c->nranks);
+        for (int r = 0; r < c->nranks; r++) {
+            if (r == c->rank) base = T;
+            T += all[(size_t)r];
+            Q[(size_t)r] = T;
+        }
+        if (!(T > 0.0)) {                                  // fewer distinct events than K: the rest repeat the first centre
+            for (int j = k; j < K; j++)
+                CUDA_TRY(cudaMemcpyAsync(b.d_centres + (size_t)j * D, b.d_centres, sizeof(float) * D, cudaMemcpyDeviceToDevice, c->stream));
+            break;
+        }
+        {                                                  // this rank's inclusive block prefixes, continuing from the ranks before it
+            double run = base;
+            for (int i = 0; i < nb; i++) prefix[(size_t)i] = (run += b.h_bsum[i]);
+        }
+        int last_block = -1;                               // last block of this rank with a positive sum
+        for (int i = nb - 1; i >= 0 && last_block < 0; i--)
+            if (b.h_bsum[i] > 0.0) last_block = i;
+        int last_rank = -1;
+        for (int r = c->nranks - 1; r >= 0 && last_rank < 0; r--)
+            if (all[(size_t)r] > 0.0) last_rank = r;
+        for (int l = 0; l < L; l++) {
+            const double t = rng.uniform() * T;
+            SeedPick p{-1, 0, 0.0, 0.0};
+            int owner = -1;
+            for (int r = 0; r < c->nranks && owner < 0; r++)
+                if (Q[(size_t)r] > t) owner = r;
+            const bool fallback = owner < 0;
+            if (fallback) owner = last_rank;
+            if (owner == c->rank) {
+                const int blk = fallback ? nb : (int)(std::upper_bound(prefix.begin(), prefix.begin() + nb, t) - prefix.begin());
+                if (blk < nb) { p.block = blk; p.start = blk > 0 ? prefix[(size_t)blk - 1] : base; p.target = t; }
+                else { p.block = last_block; p.start = 0.0; p.target = INFINITY; }
+            }
+            b.h_pick[l] = p;
+        }
+        CUDA_TRY(cudaMemcpyAsync(b.d_pick, b.h_pick, sizeof(SeedPick) * L, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(cudaMemsetAsync(b.d_cand, 0, sizeof(float) * (size_t)L * D, c->stream));
+        if (c->n > 0) {
+            kmeanspp_pick_kernel<<<L, 32, 0, c->stream>>>(b.d_d2, c->n, b.d_pick, c->d_x_aos, D, b.d_cand, b.d_pick_idx);
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (int rc = kmeans_sum_rows(c, b.d_cand, (size_t)L * D)) return rc;
+        if (int rc = kmeanspp_potential(c, L)) return rc;
+        if (c->n > 0) CUDA_TRY(cudaMemcpyAsync(b.h_bpot, b.d_bpot, sizeof(double) * b.nb * kSeedMaxCand, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));
+        double pot[kSeedMaxCand] = {0};
+        for (int i = 0; i < nb; i++)
+            for (int l = 0; l < L; l++) pot[l] += b.h_bpot[(size_t)i * kSeedMaxCand + l];
+        if (int rc = kmeans_rank_values(c, pot, L, all)) return rc;
+        int best = 0;
+        double best_pot = INFINITY;
+        for (int l = 0; l < L; l++) {
+            double s = 0.0;
+            for (int r = 0; r < c->nranks; r++) s += all[(size_t)r * L + l];
+            if (s < best_pot) { best_pot = s; best = l; }
+        }
+        CUDA_TRY(cudaMemcpyAsync(b.d_centres + (size_t)k * D, b.d_cand + (size_t)best * D, sizeof(float) * D, cudaMemcpyDeviceToDevice, c->stream));
+        if (k + 1 < K)
+            if (int rc = kmeanspp_update(c, b.d_centres + (size_t)k * D, false)) return rc;
+    }
+    return GMM_OK;
+}
+
+// One Lloyd assignment to kmeans.d_centres: one-hot rows into d_memb, labels; global changed count and inertia.
+static int kmeans_assign(gmm_ctx* c, int K, long long* changed, double* inertia) {
+    KmeansBuffers& b = c->kmeans;
+    const int Kw = std::min((c->Kmax + 7) / 8 * 8, (K + 31) / 32 * 32);
+    if (int rc = kmeans_assign_launch(c, K, Kw)) return rc;
+    if (c->n > 0) {
+        CUDA_TRY(cudaMemcpyAsync(b.h_bchanged, b.d_bchanged, sizeof(int) * b.nba, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaMemcpyAsync(b.h_binertia, b.d_binertia, sizeof(double) * b.nba, cudaMemcpyDeviceToHost, c->stream));
+    }
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    double mine[2] = {0.0, 0.0};
+    if (c->n > 0)
+        for (int i = 0; i < b.nba; i++) { mine[0] += (double)b.h_bchanged[i]; mine[1] += b.h_binertia[i]; }
+    std::vector<double> all;
+    if (int rc = kmeans_rank_values(c, mine, 2, all)) return rc;
+    double ch = 0.0, in = 0.0;
+    for (int r = 0; r < c->nranks; r++) { ch += all[(size_t)r * 2]; in += all[(size_t)r * 2 + 1]; }
+    *changed = (long long)ch;
+    *inertia = in;
+    return GMM_OK;
+}
+
+int gmm_seed_kmeans(gmm_ctx* c, int K, int max_iter, unsigned long long seed, clusters_t* host_out, float* centres_out,
+                    int* iters_out, double* inertia_out) {
+    if (int rc = check_K(c, K, "gmm_seed_kmeans")) return rc;
+    if ((long long)K > c->n_global) return fail(GMM_ERR_ARG, "gmm_seed_kmeans: K exceeds the number of events");
+    if (max_iter < 0) return fail(GMM_ERR_ARG, "gmm_seed_kmeans: max_iter < 0");
+    CUDA_TRY(cudaSetDevice(c->device));
+    if (int rc = ensure_moments(c)) return rc;             // centre and avgvar fixed before the first M-step
+    if (int rc = kmeans_buffers(c)) return rc;
+    KmeansBuffers& b = c->kmeans;
+    const int D = c->D, F = c->F;
+    c->memb_valid = false;
+    if (int rc = kmeanspp_run(c, K, seed)) return rc;
+    std::vector<float> cent((size_t)K * D);
+    CUDA_TRY(cudaMemcpyAsync(cent.data(), b.d_centres, sizeof(float) * cent.size(), cudaMemcpyDeviceToHost, c->stream));
+    if (c->n > 0) CUDA_TRY(cudaMemsetAsync(b.d_labels, 0xff, sizeof(int) * (size_t)c->n, c->stream));   // -1: every label changes once
+    if (int rc = zero_stats(c, K)) return rc;
+    // Lloyd: assignment + M-step on its one-hot memberships; the centre update is shift + S1 / S0 (S0 = 0 keeps the centre)
+    long long changed = 0;
+    double inertia = 0.0;
+    if (int rc = kmeans_assign(c, K, &changed, &inertia)) return rc;
+    if (int rc = run_mstep_accumulate(c, K)) return rc;
+    if (int rc = reduce_stats_to_host(c, K)) return rc;
+    int iters = 0;
+    while (iters < max_iter) {
+        for (int k = 0; k < K; k++) {
+            const double* s = c->h_stats + (size_t)k * F;
+            if (s[0] != 0.0)
+                for (int d = 0; d < D; d++) cent[(size_t)k * D + d] = (float)(c->shift[d] + s[1 + d] / s[0]);
+        }
+        CUDA_TRY(cudaMemcpyAsync(b.d_centres, cent.data(), sizeof(float) * cent.size(), cudaMemcpyHostToDevice, c->stream));
+        iters++;
+        if (int rc = kmeans_assign(c, K, &changed, &inertia)) return rc;
+        if (changed == 0) break;                           // same labels: the last M-step's statistics still hold
+        if (int rc = run_mstep_accumulate(c, K)) return rc;
+        if (int rc = reduce_stats_to_host(c, K)) return rc;
+    }
+    // the mixture of the final assignment: avgvar as gmm_seed sets it, then the M-step finalisation and the constants;
+    // uploaded as gmm_set_clusters uploads parameters
+    seed_from_moments(c->sum_x, c->sum_x2, c->n_global, D, K, cent.data(), &c->host);
+    finalize_from_stats(c->h_stats, c->shift, K, D, &c->host, c->host_threads, /*with_constants=*/false);
+    constants_from_R(K, D, &c->host, c->host_threads);
+    if (int rc = upload_params(c, K)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    c->memb_valid = false;
+    collect_all(c);
+    if (host_out) copy_params(host_out, &c->host, K, D);
+    if (centres_out) std::memcpy(centres_out, cent.data(), sizeof(float) * cent.size());
+    if (iters_out) *iters_out = iters;
+    if (inertia_out) *inertia_out = inertia;
     return GMM_OK;
 }
 

@@ -68,6 +68,7 @@ def load_library():
     L.gmm_comm_rank.argtypes = [C.c_void_p, _IP, _IP]
     L.gmm_set_option.argtypes = [C.c_void_p, C.c_char_p, C.c_double]
     L.gmm_seed.argtypes = [C.c_void_p, C.c_int, _CP]
+    L.gmm_seed_kmeans.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_ulonglong, _CP, _FP, _IP, _DP]
     L.gmm_set_clusters.argtypes = [C.c_void_p, C.c_int, _CP]
     L.gmm_get_clusters.argtypes = [C.c_void_p, C.c_int, _CP, C.c_int]
     L.gmm_estep.argtypes = [C.c_void_p, C.c_int, _FP]
@@ -240,6 +241,17 @@ class Engine:
         s = out.struct()
         _check(self.lib.gmm_seed(self.h, K, C.byref(s)))
         return out
+
+    def seed_kmeans(self, K, max_iter=300, seed=0, out=None):
+        """k-means++ + Lloyd initialisation (gmm_seed_kmeans): sklearn's init_params='kmeans' mixture.
+        Returns (clusters, centres [K][D] float32, Lloyd centre updates, inertia)."""
+        out = out or self.new_clusters()
+        s = out.struct()
+        cent = np.empty((K, self.D), np.float32)
+        it, inertia = C.c_int(), C.c_double()
+        _check(self.lib.gmm_seed_kmeans(self.h, K, max_iter, C.c_ulonglong(seed & 0xFFFFFFFFFFFFFFFF), C.byref(s),
+                                        cent.ctypes.data_as(_FP), C.byref(it), C.byref(inertia)))
+        return out, cent, it.value, inertia.value
 
     def set_clusters(self, K, cl):
         s = cl.struct()

@@ -139,6 +139,41 @@ int  gmm_set_option(gmm_ctx*, const char* key, double value);
  * host_out (all arrays except memberships) and uploads it.                 */
 int  gmm_seed(gmm_ctx*, int K, clusters_t* host_out);
 
+/* k-means++ (greedy) seeding + at most max_iter Lloyd iterations on the context's events,
+ * then ONE M-step on the one-hot memberships of the final assignment: the mixture
+ * sklearn's init_params='kmeans' starts EM from.  Collective (all ranks, same arguments).
+ * Leaves the context as gmm_seed does: current parameters for K = the returned ones,
+ * no valid memberships; gmm_em / gmm_estep / gmm_score may follow.
+ *   host_out     all clusters_t arrays except memberships (may be NULL)
+ *   centres_out  [K][D] the centres of the final assignment (may be NULL)
+ *   iters_out    Lloyd centre updates performed (may be NULL)
+ *   inertia_out  sum over all events of the squared distance to the assigned centre (may be NULL)
+ * Semantics (reproducible bit for bit in float64 numpy):
+ *   - draws: splitmix64 from `seed`, u = (next() >> 11) * 2^-53, on the host, the same on
+ *     every rank.  First centre: global event min(floor(u n_global), n_global - 1).
+ *   - d(x, c) = sum_d (double(x_d) - double(c_d))^2 in dimension order, no FMA; d2[i] = min
+ *     over the chosen centres.  Block sums of d2 add blocks of 1024 consecutive events of a
+ *     shard in index order; T and the running prefix add the block sums in block order and
+ *     the shards in rank order.
+ *   - each further centre: L = 2 + floor(ln K) draws, targets u_l T; candidate l = the first
+ *     event whose inclusive prefix of d2 exceeds u_l T (rounding leaving none: the last event
+ *     with d2 > 0); the candidate of smallest potential sum min(d2, d(x, c_l)) wins, lowest l
+ *     on ties.  T = 0 (fewer distinct events than K): the remaining centres repeat the first.
+ *   - Lloyd: nearest centre in FP32 (sum of (x - c)^2, ties to the lowest k); the centre
+ *     update is shift + S1/S0 of the context's own M-step (wgmma or FP64 SIMT, as gmm_mstep
+ *     chooses; counted in gmm_get_profile's launch counters); S0 = 0 keeps the centre.  Stops
+ *     after max_iter updates or when an assignment changes no label.  max_iter = 0: the
+ *     k-means++ centres, one assignment, one M-step (sklearn's 'k-means++' init).
+ *   - result: N, pi, means, R, Rinv, constant from the last M-step's statistics with avgvar
+ *     from the global variance as gmm_seed sets it (clusters without events: the N < 0.5
+ *     rules), uploaded as gmm_set_clusters uploads them.  Overwrites the device memberships.
+ * Device memory: 12 bytes per event (allocated on the first call, freed by gmm_destroy).
+ * Errors: K outside [1, Kmax], K > n_global or max_iter < 0 -> GMM_ERR_ARG; a failed
+ * collective -> GMM_ERR_NCCL.  The k-means++ centres are deterministic for a seed; so is the
+ * rest where the wgmma M-step runs (the FP64 SIMT M-step adds with atomics in varying order). */
+int  gmm_seed_kmeans(gmm_ctx*, int K, int max_iter, unsigned long long seed,
+                     clusters_t* host_out, float* centres_out, int* iters_out, double* inertia_out);
+
 /* H2D of N,pi,constant,avgvar,means,R,Rinv (gaussian.cu:446-452, 935-941). */
 int  gmm_set_clusters(gmm_ctx*, int K, const clusters_t* host_in);
 
