@@ -31,6 +31,7 @@
 #include "../../include/gmm.h"
 #include "host_math.h"
 #include "kernels_simt.cuh"
+#include "kernels_sample.cuh"
 #include "kernels_seed.cuh"
 #include "kernels_tc.cuh"
 
@@ -375,6 +376,19 @@ struct KmeansBuffers {
     }
 };
 
+// gmm_sample's parameter block (kernels_sample.cuh layout, sized for Kmax) and its pinned staging: allocated on the first
+// call, freed by gmm_destroy.  Its chunks stream through gmm_score's slots.
+struct SampleBuffers {
+    double* d_block = nullptr;
+    char* h_block = nullptr;
+    double kernel_ms = 0, wall_ms = 0;          // gmm_get_sample_profile
+    void destroy() {
+        cudaFree(d_block);
+        if (h_block) cudaFreeHost(h_block);
+        d_block = nullptr; h_block = nullptr;
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -448,6 +462,7 @@ struct gmm_ctx {
     long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score / gmm_score_stats
     ScoreStatsBuffers sstats;    // gmm_score_stats: chunk buffers, allocated on first use
     KmeansBuffers kmeans;        // gmm_seed_kmeans: allocated on first use
+    SampleBuffers sample;        // gmm_sample: parameter block, allocated on first use
 };
 
 namespace gmm {
@@ -978,6 +993,7 @@ void gmm_destroy(gmm_ctx* c) {
     c->score.destroy();
     c->sstats.destroy();
     c->kmeans.destroy();
+    c->sample.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -1873,8 +1889,6 @@ static int kmeans_assign_launch(gmm_ctx* c, int K, int Kw) {
     CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
-#undef GMM_SEED_CASE
-#undef GMM_SEED_DISPATCH
 
 // splitmix64; each draw u = (next >> 11) * 2^-53 in [0, 1).  Every rank draws the same sequence.
 struct SplitMix64 {
@@ -2048,6 +2062,136 @@ int gmm_seed_kmeans(gmm_ctx* c, int K, int max_iter, unsigned long long seed, cl
     if (centres_out) std::memcpy(centres_out, cent.data(), sizeof(float) * cent.size());
     if (iters_out) *iters_out = iters;
     if (inertia_out) *inertia_out = inertia;
+    return GMM_OK;
+}
+
+// ---- sampling from the mixture ------------------------------------------------------------------------------------------
+// The parameter block of the current K clusters (kernels_sample.cuh layout) in the pinned staging, with the checks of
+// gmm.h in cluster order.  *klast = the last cluster with pi > 0.
+static int sample_params(gmm_ctx* c, int K, int* klast) {
+    const int D = c->D, REC = sample_rec_floats(D);
+    double* cum = reinterpret_cast<double*>(c->sample.h_block);
+    float* rec = reinterpret_cast<float*>(cum + sample_cum_len(K));
+    double run = 0.0;
+    *klast = -1;
+    for (int k = 0; k < K; k++) {
+        const float p = c->host.pi[k];
+        if (!(p >= 0.0f) || !std::isfinite(p))
+            return fail(GMM_ERR_STATE, "gmm_sample: pi of cluster " + std::to_string(k) + " is negative or not finite");
+        double U[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS], ld;
+        if (!reverse_cholesky(c->host.R + (size_t)k * D * D, D, U, &ld))
+            return fail(GMM_ERR_STATE, "gmm_sample: R of cluster " + std::to_string(k) + " is not positive definite");
+        run += (double)p;
+        cum[k] = run;
+        if (p > 0.0f) *klast = k;
+        float* r = rec + (size_t)k * REC;
+        int e = 0;
+        for (int d = 0; d < D; d++) {
+            r[e++] = c->host.means[(size_t)k * D + d];
+            for (int j = d; j < D; j++) r[e++] = (float)U[d][j];
+        }
+        for (; e < REC; e++) r[e] = 0.0f;
+    }
+    if (!(run > 0.0)) return fail(GMM_ERR_STATE, "gmm_sample: the mixing weights pi sum to zero");
+    return GMM_OK;
+}
+
+// Chunks of c->score_chunk events through gmm_score's slots: sample_kernel writes slot i & 1's device chunk (rows) and
+// label area, the copy stream brings them to the slot's pinned stages, the host copies them to the caller's arrays.  The
+// order is score_batch's: chunk i is issued before chunk i - 1 is handed over, so chunk i's kernel runs while chunk
+// i - 1's D2H and the host copy of chunk i - 2 proceed.
+static int sample_batch(gmm_ctx* c, int K, int klast, unsigned long long seed, long long first, long long n, float* events,
+                        int* labels) {
+    ScoreBuffers& s = c->score;
+    const int D = c->D;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
+    CUDA_TRY(cudaMemcpyAsync(c->sample.d_block, c->sample.h_block, sample_block_bytes(K, D), cudaMemcpyHostToDevice, c->stream));
+    // the parameters go to shared memory when they fit beside the output tile with two blocks per SM (D = 24: K <= 66)
+    const size_t staged = sample_tile_bytes(D) + sample_block_bytes(K, D);
+    const int stage = staged <= (size_t)kSampleStageBytes ? 1 : 0;
+    const size_t smem = stage ? staged : sample_tile_bytes(D);
+    int per_sm = 0;
+#define GMM_CALL(d)                                                                                                   \
+    do {                                                                                                              \
+        CUDA_TRY(cudaFuncSetAttribute(sample_kernel<d>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, sample_kernel<d>, kSampleThreads, smem));    \
+    } while (0)
+    GMM_SEED_DISPATCH(D, GMM_CALL)
+#undef GMM_CALL
+    const long long max_grid = (long long)std::max(per_sm, 1) * c->num_sms;
+    auto labels_of = [&](char* base) { return reinterpret_cast<int*>(base + ScoreBuffers::kHeader); };
+    auto issue = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        const int grid = (int)std::min<long long>((m + kSampleThreads - 1) / kSampleThreads, max_grid);
+        int* d_lab = labels_of(s.d_out[b]);
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous chunk has left the device
+        CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
+#define GMM_CALL(d) \
+    sample_kernel<d><<<grid, kSampleThreads, smem, c->stream>>>(c->sample.d_block, K, klast, stage, seed, first + e0, m, s.d_in[b], d_lab)
+        GMM_SEED_DISPATCH(D, GMM_CALL)
+#undef GMM_CALL
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
+        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
+        CUDA_TRY(cudaMemcpyAsync(s.h_in[b], s.d_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyDeviceToHost, s.copy));
+        if (labels) CUDA_TRY(cudaMemcpyAsync(labels_of(s.h_out[b]), d_lab, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
+        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
+        return GMM_OK;
+    };
+    auto finish = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) c->sample.kernel_ms += ms;
+        std::memcpy(events + (size_t)e0 * D, s.h_in[b], sizeof(float) * (size_t)m * D);
+        if (labels) std::memcpy(labels + e0, labels_of(s.h_out[b]), sizeof(int) * (size_t)m);
+        return GMM_OK;
+    };
+    for (long long i = 0; i < nchunks; i++) {
+        if (int rc = issue(i)) return rc;
+        if (i > 0)
+            if (int rc = finish(i - 1)) return rc;
+    }
+    return finish(nchunks - 1);
+}
+#undef GMM_SEED_CASE
+#undef GMM_SEED_DISPATCH
+
+int gmm_sample(gmm_ctx* c, int K, long long n, unsigned long long seed, long long first, float* events_out, int* labels_out) {
+    if (int rc = check_K(c, K, "gmm_sample")) return rc;
+    if (n < 0 || first < 0 || first > (1LL << 62) - n || (n > 0 && !events_out))
+        return fail(GMM_ERR_ARG, "gmm_sample: bad range or output (n < 0, first < 0, first + n > 2^62, or no event array)");
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_sample: parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, "gmm_sample: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    SampleBuffers& sb = c->sample;
+    if (!sb.d_block) CUDA_TRY(cudaMalloc(&sb.d_block, sample_block_bytes(c->Kmax, c->D)));
+    if (!sb.h_block) CUDA_TRY(cudaMallocHost(&sb.h_block, sample_block_bytes(c->Kmax, c->D)));
+    int klast = 0;
+    int rc = sample_params(c, K, &klast);
+    if (rc == GMM_OK && n > 0) {
+        rc = score_buffers(c);
+        if (rc == GMM_OK) rc = sample_batch(c, K, klast, seed, first, n, events_out, labels_out);
+        // nothing of this call may still be in flight when it returns (also after a failure)
+        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
+        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = fail(GMM_ERR_CUDA, std::string("gmm_sample: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    sb.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_get_sample_profile(gmm_ctx* c, double out[2], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_sample_profile: bad argument");
+    out[0] = c->sample.kernel_ms; out[1] = c->sample.wall_ms;
+    if (reset) c->sample.kernel_ms = c->sample.wall_ms = 0;
     return GMM_OK;
 }
 

@@ -87,9 +87,7 @@ void constants_cluster(int k, int D, clusters_t* c) {
 // two finalisations produce bit-identical factors and E-step operands.
 #pragma GCC push_options
 #pragma GCC optimize("fp-contract=off")
-bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out */) {
-    double U[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS];
-    const float* R = c->R + (size_t)k * D * D;
+bool reverse_cholesky(const float* R, int D, double (*U)[GMM_MAX_DIMENSIONS], double* ld_out) {
     double ld = 0.0;
     for (int j = D - 1; j >= 0; j--) {
         double d = R[j * D + j];
@@ -104,6 +102,14 @@ bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out 
             U[i][j] = v * rp;
         }
     }
+    *ld_out = ld;
+    return true;
+}
+
+bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out */) {
+    double U[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS];
+    double ld;
+    if (!reverse_cholesky(c->R + (size_t)k * D * D, D, U, &ld)) return false;
     // W = U^-1 (upper triangular), column by column: W[i][j] = -(sum_{m=i+1..j} U[i][m] W[m][j]) / U[i][i]
     for (int j = 0; j < D; j++) {
         for (int i = D - 1; i > j; i--) W[i * D + j] = 0.0;

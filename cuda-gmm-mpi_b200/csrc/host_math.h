@@ -35,6 +35,10 @@ void constants_cluster(int k, int D, clusters_t* c);
 // Same results for a symmetric positive definite R from one (reverse) Cholesky factorisation; also returns the
 // upper-triangular W with Rinv = W^T W.  false = not positive definite, nothing written (use constants_cluster).
 bool constants_cluster_spd(int k, int D, clusters_t* c, double* W);
+// The factorisation behind it: R = U U^T with U upper triangular, in double from the float R [D][D] (row-major, the
+// off-diagonal pairs averaged), pivots from the last one up; *ld = sum ln U_jj.  Only U's upper triangle is written.
+// false = not positive definite (a pivot <= 0 or not finite).
+bool reverse_cholesky(const float* R, int D, double (*U)[GMM_MAX_DIMENSIONS], double* ld);
 // N, mean and covariance of ONE cluster from the packed statistics (the loop body of finalize_from_stats).
 void finalize_cluster(const double* stats, const double* shift, int k, int D, clusters_t* c);
 void mixing_weights(int K, clusters_t* c);

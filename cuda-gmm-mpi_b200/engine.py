@@ -82,6 +82,8 @@ def load_library():
     L.gmm_get_score_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_score_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_void_p]
     L.gmm_get_score_stats_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_sample.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_ulonglong, C.c_longlong, C.c_void_p, C.c_void_p]
+    L.gmm_get_sample_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
@@ -332,6 +334,21 @@ class Engine:
         _check(self.lib.gmm_get_score_stats_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], wall_ms=out[1], estep_tensor_chunks=int(out[2]), estep_simt_chunks=int(out[3]),
                     mstep_tensor_chunks=int(out[4]), mstep_simt_chunks=int(out[5]), flag_wait_ms=out[6])
+
+    def sample(self, K, n, seed=0, first=0, labels=True):
+        """Draw events first .. first + n - 1 of the sample `seed` from the current K-cluster mixture (gmm_sample).
+        Returns (events float32 [n][D], labels int32 [n] or None)."""
+        n = int(n)
+        ev = np.empty((max(n, 0), self.D), np.float32)
+        lab = np.empty(max(n, 0), np.int32) if labels else None
+        _check(self.lib.gmm_sample(self.h, K, n, C.c_ulonglong(seed & 0xFFFFFFFFFFFFFFFF), first,
+                                   ev.ctypes.data if ev.size else None, lab.ctypes.data if lab is not None and lab.size else None))
+        return ev, lab
+
+    def sample_profile(self, reset=False):
+        out = (C.c_double * 2)()
+        _check(self.lib.gmm_get_sample_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1])
 
     def fit_profile(self):
         out = (C.c_double * 4)()

@@ -279,6 +279,42 @@ int  gmm_score_stats(gmm_ctx*, int K, const float* events_aos, long long n,
  * host's staging of the next chunk, which is issued before the flag is read. */
 int  gmm_get_score_stats_profile(gmm_ctx*, double out[7], int reset);
 
+/* Draw n events from the mixture (sklearn's sample(n)): events_out [n][D] row-major, labels_out [n] the
+ * component of each event (may be NULL).  The parameters are the set the next gmm_estep(ctx, K) would use:
+ * pi, means and R of the context's host copy.  No collective; nothing of the EM state changes (memberships,
+ * statistics, log-likelihood, gmm_get_profile, gmm_get_score_profile, gmm_get_score_stats_profile).
+ * Event i of the call is the event of global index g = first + i, a function of (parameters, seed, g)
+ * alone: options "path" and "score_chunk" and the number of ranks do not change it, and calls (first, n1)
+ * and (first + n1, n2) give the bits of one call (first, n1 + n2) — ranks or batches split one sample so.
+ * Semantics (restated in float64 numpy by tests/_sample_ref.py):
+ *   - words: Philox4x32-10 (Salmon et al. 2011, the Random123 definition), key (lo32(seed), hi32(seed));
+ *     block j of event g uses counter (lo32(g), hi32(g), j, 0); the event's words are block 0's four
+ *     words (x, y, z, w), then block 1's, and so on.
+ *   - component: u = ((w0 >> 5) 2^26 + (w1 >> 6)) 2^-53 (53 bits, [0, 1)).  C_k = running sum in double
+ *     of the float pi in cluster order, T = C_{K-1}; the label is the first k with u*T < C_k (product
+ *     rounded in double), or, if rounding leaves none, the last k with pi_k > 0.  A cluster with pi = 0
+ *     is never drawn; one that carries the reference's pi = 1e-10 (N < 0.5) is drawn with that weight.
+ *   - normals: pair p = 0 .. ceil(D/2) - 1 uses words a = w_{2+2p}, b = w_{3+2p}, in float:
+ *     u1 = ((float)a + 0.5f) 2^-32 in (0, 1], r = sqrtf(-2 logf(u1)) (at most ~6.8),
+ *     (s, c) = sincospif((float)b 2^-31), z_{2p} = r c, z_{2p+1} = r s (the last s dropped for odd D).
+ *     Conversions round to nearest; no fast-math approximations.
+ *   - event: x = mu_k + U_k z, with U_k the upper-triangular factor R_k = U_k U_k^T that the host
+ *     finalisation computes in double from the float R (off-diagonal pairs averaged, pivots from the last
+ *     one up), rounded to float: x_d = fmaf-accumulation of U_dj z_j for j = d .. D-1 onto mu_d, in float.
+ *   This is sklearn's distribution, except that events come i.i.d. in index order where sklearn sorts
+ *   them by component.
+ * The kernel writes chunks of option "score_chunk" events through gmm_score's two device chunks and pinned
+ * stages; the parameter block ([K] double + [K][D + D(D+1)/2] float, padded) is allocated for Kmax on the
+ * first call and freed by gmm_destroy.
+ * Errors: K outside [1, Kmax], n < 0, first < 0, first + n > 2^62, or events_out == NULL with n > 0 ->
+ * GMM_ERR_ARG; K != the K of the current parameters, a call between gmm_mstep and gmm_constants, a cluster
+ * whose R is not positive definite, a pi that is negative or not finite (the first such cluster is named
+ * in the message), or T <= 0 -> GMM_ERR_STATE.  n = 0 returns GMM_OK and writes nothing.              */
+int  gmm_sample(gmm_ctx*, int K, long long n, unsigned long long seed, long long first,
+                float* events_out, int* labels_out);
+/* Since the last reset: out[0] sampling-kernel ms, out[1] wall ms inside gmm_sample.                   */
+int  gmm_get_sample_profile(gmm_ctx*, double out[2], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
