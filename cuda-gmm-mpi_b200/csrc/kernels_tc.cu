@@ -490,11 +490,11 @@ mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, 
 // memory: each thread converts its own rows straight into wgmma A fragments
 // (register operand), so one k-step may pair ANY two B chunks (start + LBO).
 //
-// One persistent CTA per SM, NWG independent warpgroups; each takes 64-event tiles in turn and per supergroup of 16
-// clusters and block c of 8 output dimensions issues the k-steps that block needs (m64n128k16, A from registers),
-// then squares and sums the 8 columns of each cluster (a quad of lanes holds them), the log-sum-exp over the
-// clusters (again within the quad) and writes the responsibilities and the log-likelihood.  The warpgroups
-// interleave, so one's MMAs overlap another's epilogue.
+// One persistent CTA per SM, NWG independent warpgroups; each takes 64-event tiles in turn.  Per supergroup of 16 clusters,
+// block c of 8 output dimensions and half of the supergroup it issues the k-steps that block needs (m64n64k16, A from
+// registers) as one MMA group, and squares and sums the 8 columns of each cluster (a quad of lanes holds them) while the
+// next group runs (tc_tile_logits); then the log-sum-exp over the clusters (again within the quad), the responsibilities
+// and the log-likelihood.  The other warpgroup's MMAs cover this one's log-sum-exp and stores.
 // ===========================================================================
 
 // Block structure.  W is upper triangular, so the 8 output columns d in [8c, 8c+8) of a cluster
@@ -516,9 +516,16 @@ template <int D> struct ECfg {
     static constexpr int OFF_SH = OFF_CK + 512;               // float[32] shift, float[32] inverse scale
     static constexpr int OFF_BAR = OFF_SH + 256;
     static constexpr int SMEM_BYTES = OFF_BAR + 64;
-    static constexpr int NWG = 2;                             // warpgroups per CTA (255 registers each: no spills at D = 24)
+    static constexpr int NWG = 2;                             // warpgroups per CTA (up to 255 registers each, no spills)
     static constexpr int THREADS = 128 * NWG;
 };
+
+// Timing variants of the E-step for scripts/prof_estep.py (`make variant DEFS=-DGMM_ESTEP_CUT=n`); the default build is 0.
+//   1  MMA only: the accumulators feed one sum per block, no squares, log-sum-exp, exp, log or stores (results are wrong)
+//   2  no stores: the full epilogue, but the responsibilities are not written
+#ifndef GMM_ESTEP_CUT
+#define GMM_ESTEP_CUT 0
+#endif
 
 // ---- pieces shared by estep_tc_kernel and score_tc_kernel (same operand path, different epilogues) ----------------
 // Shared-memory staging of one pass: constants, shift / inverse scale, and the resident B image (one TMA bulk copy per
@@ -562,16 +569,53 @@ __device__ __forceinline__ void tc_split_rows(const float2 (&xa)[D / 8], const f
     }
 }
 
-// The base-2 logits of one 64-event tile against the resident clusters of the pass: per supergroup of 16 clusters and
-// block c of 8 output dimensions the k-steps that block needs (m64n128k16, A from registers), the squares summed over
-// the 8 columns of each cluster with a quad transpose.  lg[sg][u]: cluster sg * 16 + 8 (qd & 1) + 4 (qd >> 1) + (u >> 1),
-// row u & 1 (-inf for supergroups >= NSG).
+// One MMA group of a tile: half h (clusters 8h .. 8h+7 of the supergroup whose B image starts at bsg, N = 64) of block c,
+// i.e. the k-steps that block needs (m64n64k16, A from registers), into a 32-register accumulator.  The first k-step
+// overwrites it (scale-d = 0).  The caller commits.
 template <int D>
-__device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], const uint32_t (&zl)[D / 8][2], uint32_t bsm,
-                                               const float* ck_s, int NSG, int qd, uint32_t ones, float (&lg)[ECfg<D>::MAXSG][8]) {
+__device__ __forceinline__ void tc_issue_group(float (&acc)[32], const uint32_t (&zh)[D / 8][2], const uint32_t (&zl)[D / 8][2],
+                                               uint32_t bsg, int c, int h, uint32_t ones) {
     using C = ECfg<D>;
     constexpr int CP = C::CP;
-    constexpr uint32_t CH = C::N * 16;                        // bytes per B chunk
+    constexpr uint32_t CH = C::N * 16;                        // bytes per B chunk (128 rows of 16 B)
+    const uint32_t bb = bsg + (uint32_t)c * C::B_BLOCK + (uint32_t)h * (CH / 2);
+    wgmma_fence();
+#pragma unroll
+    for (int j = c; j < CP; j++)                              // (Wh_j, Wl_j) x (zh_j, zh_j)
+        wgmma_m64n64k16_rs(acc, zh[j][0], zh[j][1], zh[j][0], zh[j][1], make_smem_desc(bb + j * CH, CP * CH, 128), j > c);
+    // (Wh_j) x (zl_j) for j >= c, then v x ones, two at a time; a lone v step pairs with a zero A chunk
+#pragma unroll
+    for (int p = c; p < CP + 1; p += 2) {
+        const int x = p, y = p + 1;                           // list items: j < CP -> Wh_j x zl_j, j == CP -> v x ones
+        if (y <= CP) {
+            const uint32_t yc = y < CP ? (uint32_t)y : 2u * CP;
+            const uint32_t a2 = y < CP ? zl[y < CP ? y : 0][0] : ones, a3 = y < CP ? zl[y < CP ? y : 0][1] : ones;
+            wgmma_m64n64k16_rs(acc, zl[x][0], zl[x][1], a2, a3, make_smem_desc(bb + x * CH, (yc - x) * CH, 128), true);
+        } else {                                              // x == CP: v alone, paired with chunk c under a zero A chunk
+            wgmma_m64n64k16_rs(acc, 0u, 0u, ones, ones, make_smem_desc(bb + c * CH, (2 * CP - c) * CH, 128), true);
+        }
+    }
+}
+
+// The base-2 logits of one 64-event tile against the resident clusters of the pass: per supergroup of 16 clusters, block
+// c of 8 output dimensions and half h of the supergroup's clusters the k-steps that block needs (one MMA group), the
+// squares summed over the 8 columns of each cluster with a quad transpose.  lg[sg][u]: cluster sg * 16 + 8 (qd & 1) +
+// 4 (qd >> 1) + (u >> 1), row u & 1 (-inf for supergroups >= NSG).
+// Software pipeline: the groups (sg, c, h) form one sequence over a ring of two accumulators (group (sg, c, h) in acc[h]);
+// group i + 1 is issued and committed before group i is waited for and squared, so this warpgroup always has MMAs queued
+// while it squares and transposes; only the tile's last group is waited for with nothing behind it.  No group stays in
+// flight across tiles: the register A operand zh / zl of the next tile could not be written while this tile's last group
+// still reads it, and ptxas serialises every wgmma when a pending group is carried around the tile loop.
+// NSG (resident supergroups of the pass) is a template parameter: with a wgmma issue or a wait<1> under a run-time branch
+// on it, ptxas serialises every wgmma of the kernel (C7514).
+template <int D, int NSG>
+__device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], const uint32_t (&zl)[D / 8][2], uint32_t bsm,
+                                               const float* ck_s, int qd, uint32_t ones, float (&lg)[ECfg<D>::MAXSG][8]) {
+    using C = ECfg<D>;
+    constexpr int CP = C::CP;
+    float acc[2][32];
+    tc_issue_group<D>(acc[0], zh, zl, bsm, 0, 0, ones);
+    wgmma_commit();
 #pragma unroll
     for (int sg = 0; sg < C::MAXSG; sg++) {
         if (sg >= NSG) {
@@ -579,42 +623,43 @@ __device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], c
             for (int u = 0; u < 8; u++) lg[sg][u] = -INFINITY;
             continue;
         }
+        const uint32_t bsg = bsm + (uint32_t)sg * C::B_SG;
         float sq[32];                                      // sums of squares: [cluster 0..15][row]
 #pragma unroll
         for (int u = 0; u < 32; u++) sq[u] = 0.f;
 #pragma unroll
         for (int c = 0; c < CP; c++) {
-            const uint32_t bb = bsm + (uint32_t)(sg * CP + c) * C::B_BLOCK;
-            float acc[64];
 #pragma unroll
-            for (int u = 0; u < 64; u++) acc[u] = 0.f;
-            wgmma_fence();
-            bool accum = false;
-#pragma unroll
-            for (int j = c; j < CP; j++) {                 // (Wh_j, Wl_j) x (zh_j, zh_j)
-                wgmma_m64n128k16_rs(acc, zh[j][0], zh[j][1], zh[j][0], zh[j][1], make_smem_desc(bb + j * CH, CP * CH, 128), accum);
-                accum = true;
-            }
-            // (Wh_j) x (zl_j) for j >= c, then v x ones, two at a time; a lone v step pairs with a zero A chunk
-#pragma unroll
-            for (int p = c; p < CP + 1; p += 2) {
-                const int x = p, y = p + 1;                // list items: j < CP -> Wh_j x zl_j, j == CP -> v x ones
-                if (y <= CP) {
-                    const uint32_t yc = y < CP ? (uint32_t)y : 2u * CP;
-                    const uint32_t a2 = y < CP ? zl[y < CP ? y : 0][0] : ones, a3 = y < CP ? zl[y < CP ? y : 0][1] : ones;
-                    wgmma_m64n128k16_rs(acc, zl[x][0], zl[x][1], a2, a3, make_smem_desc(bb + x * CH, (yc - x) * CH, 128), true);
-                } else {                                   // x == CP: v alone, paired with chunk c under a zero A chunk
-                    wgmma_m64n128k16_rs(acc, 0u, 0u, ones, ones, make_smem_desc(bb + c * CH, (2 * CP - c) * CH, 128), true);
+            for (int h = 0; h < 2; h++) {
+                // queue the next group of the sequence, then wait for this one (all conditions are compile-time)
+                if (sg + 1 == NSG && c + 1 == CP && h == 1) {
+                    wgmma_wait<0>();
+                } else {
+                    if (h == 0) tc_issue_group<D>(acc[1], zh, zl, bsg, c, 1, ones);
+                    else if (c + 1 < CP) tc_issue_group<D>(acc[0], zh, zl, bsg, c + 1, 0, ones);
+                    else tc_issue_group<D>(acc[0], zh, zl, bsg + C::B_SG, 0, 0, ones);
+                    wgmma_commit();
+                    wgmma_wait<1>();
                 }
-            }
-            wgmma_commit();
-            wgmma_wait_all();
+                wgmma_pin(acc[h]);
+                const float(&a)[32] = acc[h];
+#if GMM_ESTEP_CUT == 1
+                sq[0] += a[0];
+#else
 #pragma unroll
-            for (int i = 0; i < 16; i++) {
-                sq[2 * i] = fmaf(acc[4 * i], acc[4 * i], fmaf(acc[4 * i + 1], acc[4 * i + 1], sq[2 * i]));
-                sq[2 * i + 1] = fmaf(acc[4 * i + 2], acc[4 * i + 2], fmaf(acc[4 * i + 3], acc[4 * i + 3], sq[2 * i + 1]));
+                for (int i = 0; i < 8; i++) {
+                    float& s0 = sq[16 * h + 2 * i];
+                    float& s1 = sq[16 * h + 2 * i + 1];
+                    s0 = fmaf(a[4 * i], a[4 * i], fmaf(a[4 * i + 1], a[4 * i + 1], s0));
+                    s1 = fmaf(a[4 * i + 2], a[4 * i + 2], fmaf(a[4 * i + 3], a[4 * i + 3], s1));
+                }
+#endif
             }
         }
+#if GMM_ESTEP_CUT == 1
+        for (int u = 0; u < 8; u++) lg[sg][u] = sq[0];
+        continue;
+#endif
         // sum over the quad (the 8 columns of a cluster are spread over its 4 lanes), transposing as it goes:
         // lane qd ends with clusters cb .. cb+3 of the supergroup, cb = 8 (qd & 1) + 4 (qd >> 1), both rows
         float w[16];
@@ -634,13 +679,12 @@ __device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], c
     }
 }
 
-template <int D>
+template <int D, int NSG>
 __global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
 estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
                 const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float* __restrict__ memb,
-                size_t pitch, int n, int K, int NSG, double* __restrict__ ll_out, int mode, const float* den_in,
-                float* den_out) {
-    // K / NSG / b_img / ck / memb describe ONE pass of at most 64 clusters.  More than 64 clusters take 2P - 1 launches
+                size_t pitch, int n, int K, double* __restrict__ ll_out, int mode, const float* den_in, float* den_out) {
+    // K / NSG (= ceil(K / 16)) / b_img / ck / memb describe ONE pass of at most 64 clusters.  More than 64 clusters take 2P - 1 launches
     // for P passes, and every responsibility is written exactly once:
     //   mode 1 (passes 0 .. P-2)  log-denominator only: den_out[e] = ln(sum_k exp(logit)) (+ den_in[e] in log space), no stores
     //   mode 2 (pass P-1)         its own log-sum-exp joined with den_in[e] (all other passes): final responsibilities of this
@@ -688,7 +732,11 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
         if (t + stride < ntiles) load_rows(t + stride);
 
         float lg[C::MAXSG][8];                                 // base-2 logits: [supergroup][4 clusters x 2 rows]
-        tc_tile_logits<D>(zh, zl, bsm, ck_s, NSG, qd, ones, lg);
+        tc_tile_logits<D, NSG>(zh, zl, bsm, ck_s, qd, ones, lg);
+#if GMM_ESTEP_CUT == 1
+        for (int sg = 0; sg < C::MAXSG; sg++) ll_acc += (double)lg[sg][0];
+        continue;
+#endif
         // log-sum-exp over the clusters (estep2, gaussian_kernel.cu:481-503), per row: this lane's 16 logits, then the quad
         float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
@@ -742,7 +790,7 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
                 if (qd == 0 && er[r] < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
             }
         }
-        if (mode != 1) {
+        if (mode != 1 && GMM_ESTEP_CUT != 2) {
             // Rows [K, 8*ceil(K/8)) are written too (zeros of the padding clusters): the buffer is allocated in
             // multiples of 8 rows.
 #pragma unroll
@@ -779,10 +827,10 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
 // Every pass flags the chunk (*flag = 1) when an event has a coordinate that is not finite or lies beyond 2^14 global
 // standard deviations (the bound tc_estep_range_ok applies to the training data: the FP16 event operand overflows).
 // ===========================================================================
-template <int D>
+template <int D, int NSG>
 __global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
 score_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
-                const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, int n, int K, int NSG, int kbase,
+                const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, int n, int K, int kbase,
                 int pass, int last, float* run_den, float* run_bl, int* run_bk, int* __restrict__ labels,
                 float* __restrict__ max_resp, float* __restrict__ logp, double* __restrict__ ll_out, int* __restrict__ flag) {
     using C = ECfg<D>;
@@ -834,7 +882,7 @@ score_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
         if (t + stride < ntiles) load_rows(t + stride);
 
         float lg[C::MAXSG][8];
-        tc_tile_logits<D>(zh, zl, bsm, ck_s, NSG, qd, ones, lg);
+        tc_tile_logits<D, NSG>(zh, zl, bsm, ck_s, qd, ones, lg);
 
         // per row: the E-step's max (fmaxf) and the arg-max over the pass's clusters, this lane's 16 logits in increasing
         // k, then the quad with (value, index) pairs; lowest k on ties, NaN logits never win
@@ -1591,8 +1639,13 @@ template <int D>
 static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, cudaStream_t stream) {
     using C = ECfg<D>;
     static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
+    // one instance per number of resident supergroups (1 .. 4) of a pass
+    static void (*const kern[C::MAXSG])(const float*, const uint8_t*, const float*, const float*, const float*, float*, size_t, int, int,
+                                        double*, int, const float*, float*) = {estep_tc_kernel<D, 1>, estep_tc_kernel<D, 2>,
+                                                                              estep_tc_kernel<D, 3>, estep_tc_kernel<D, 4>};
+    static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_estep) {
-        TC_CUDA_TRY(cudaFuncSetAttribute(estep_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_estep = true;
     }
     const int ntiles = (n + 127) / 128;
@@ -1606,9 +1659,9 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
     // theirs against those totals (mode 3): 2P - 1 launches, every responsibility stored once
     auto launch = [&](int p, int mode, const float* den_in, float* den_out) {
         const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
-        estep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
+        kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
             x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f,
-            memb + (size_t)(64 * p) * pitch, pitch, n, Kp, (Kp + C::GB - 1) / C::GB, d_ll, mode, den_in, den_out);
+            memb + (size_t)(64 * p) * pitch, pitch, n, Kp, d_ll, mode, den_in, den_out);
         return cudaGetLastError();
     };
     if (NP == 1) TC_CUDA_TRY(launch(0, 0, nullptr, nullptr));
@@ -1644,8 +1697,12 @@ int tc_launch_estep_on(TcState* t, int K, const float* d_x_aos, int n, float* d_
 template <int D>
 static int launch_score_d(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream) {
     using C = ECfg<D>;
+    static void (*const kern[C::MAXSG])(const float*, const uint8_t*, const float*, const float*, const float*, int, int, int, int, int,
+                                        float*, float*, int*, int*, float*, float*, double*, int*) = {
+        score_tc_kernel<D, 1>, score_tc_kernel<D, 2>, score_tc_kernel<D, 3>, score_tc_kernel<D, 4>};
+    static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_score) {
-        TC_CUDA_TRY(cudaFuncSetAttribute(score_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_score = true;
     }
     const int ntiles = (io.n + 127) / 128;
@@ -1656,9 +1713,8 @@ static int launch_score_d(TcState* t, int K, const TcScoreIo& io, cudaStream_t s
     if (NP > 1 && !(io.run_den && io.run_bl && io.run_bk)) return fail(GMM_ERR_STATE, "tensor scoring: no running state for K > 64");
     for (int p = 0; p < NP; p++) {
         const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
-        score_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
-            io.x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f, io.n, Kp,
-            (Kp + C::GB - 1) / C::GB, 64 * p, p, p + 1 == NP, io.run_den, io.run_bl, io.run_bk, io.labels, io.max_resp, io.logp, io.ll,
+        kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
+            io.x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f, io.n, Kp, 64 * p, p, p + 1 == NP, io.run_den, io.run_bl, io.run_bk, io.labels, io.max_resp, io.logp, io.ll,
             io.flag);
         TC_CUDA_TRY(cudaGetLastError());
     }
