@@ -31,6 +31,7 @@
 #include "../../include/gmm.h"
 #include "host_math.h"
 #include "kernels_simt.cuh"
+#include "kernels_condition.cuh"
 #include "kernels_sample.cuh"
 #include "kernels_seed.cuh"
 #include "kernels_tc.cuh"
@@ -389,6 +390,33 @@ struct SampleBuffers {
     }
 };
 
+// gmm_condition's parameter block (sized for Kmax and the largest record any observed set of this D needs) and its
+// pinned mirror, allocated on the first call; per slot of gmm_score's two, the imputations of a chunk (device and pinned:
+// cond_mean [chunk][NM] then cond_var [chunk][NM]), allocated on the first imputing call and grown with chunk x NM, never
+// shrunk.  All freed by gmm_destroy.  Its chunks stream through gmm_score's slots.
+struct ConditionBuffers {
+    float* d_block = nullptr;
+    float* h_block = nullptr;
+    float* d_imp[2] = {nullptr, nullptr};
+    float* h_imp[2] = {nullptr, nullptr};
+    size_t imp_floats = 0;                      // floats per slot
+    double kernel_ms = 0, wall_ms = 0;          // gmm_get_condition_profile
+    void release_imp() {
+        for (int s = 0; s < 2; s++) {
+            cudaFree(d_imp[s]);
+            if (h_imp[s]) cudaFreeHost(h_imp[s]);
+            d_imp[s] = h_imp[s] = nullptr;
+        }
+        imp_floats = 0;
+    }
+    void destroy() {
+        release_imp();
+        cudaFree(d_block);
+        if (h_block) cudaFreeHost(h_block);
+        d_block = h_block = nullptr;
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -463,6 +491,7 @@ struct gmm_ctx {
     ScoreStatsBuffers sstats;    // gmm_score_stats: chunk buffers, allocated on first use
     KmeansBuffers kmeans;        // gmm_seed_kmeans: allocated on first use
     SampleBuffers sample;        // gmm_sample: parameter block, allocated on first use
+    ConditionBuffers cond;       // gmm_condition: parameter block and imputation buffers, allocated on first use
 };
 
 namespace gmm {
@@ -628,15 +657,17 @@ static int launch_estep_simt(gmm_ctx* c, int K) {
     return launch_estep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F);
 }
 
+// SIMT scoring of io.n rows of D coordinates against the epack records `epack` (gmm_score: the context's D and d_epack;
+// gmm_condition: the observed dimensions and its marginal block)
 template <int D>
-static void launch_score_simt_d(gmm_ctx* c, int K, const TcScoreIo& io) {
-    score_simt_kernel<D><<<(io.n + kEstepThreads - 1) / kEstepThreads, kEstepThreads, 0, c->stream>>>(io.x, io.n, K, c->d_epack, io.labels,
+static void launch_score_simt_d(gmm_ctx* c, int K, const float* epack, const TcScoreIo& io) {
+    score_simt_kernel<D><<<(io.n + kEstepThreads - 1) / kEstepThreads, kEstepThreads, 0, c->stream>>>(io.x, io.n, K, epack, io.labels,
                                                                                                      io.max_resp, io.logp, io.ll);
 }
-static int launch_score_simt(gmm_ctx* c, int K, const TcScoreIo& io) {
+static int launch_score_simt(gmm_ctx* c, int D, int K, const float* epack, const TcScoreIo& io) {
     if (io.n <= 0) return GMM_OK;
-    switch (c->D) {
-#define GMM_CASE(d) case d: launch_score_simt_d<d>(c, K, io); break;
+    switch (D) {
+#define GMM_CASE(d) case d: launch_score_simt_d<d>(c, K, epack, io); break;
         GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
         GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
         GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
@@ -994,6 +1025,7 @@ void gmm_destroy(gmm_ctx* c) {
     c->sstats.destroy();
     c->kmeans.destroy();
     c->sample.destroy();
+    c->cond.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -1512,7 +1544,7 @@ static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, int* lab
         if (!on_tensor)
             if (int rc = ensure_epack()) return rc;
         CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
-        int rc = on_tensor ? tc_launch_score(c->tc, K, io, c->stream) : launch_score_simt(c, K, io);
+        int rc = on_tensor ? tc_launch_score(c->tc, K, io, c->stream) : launch_score_simt(c, D, K, c->d_epack, io);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
         (on_tensor ? s.tensor_chunks : s.simt_chunks)++;
@@ -2192,6 +2224,227 @@ int gmm_get_sample_profile(gmm_ctx* c, double out[2], int reset) {
     if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_sample_profile: bad argument");
     out[0] = c->sample.kernel_ms; out[1] = c->sample.wall_ms;
     if (reset) c->sample.kernel_ms = c->sample.wall_ms = 0;
+    return GMM_OK;
+}
+
+// ---- events measured on a subset of the dimensions ----------------------------------------------------------------------
+// Floats of one cluster's record in gmm_condition's block: the marginal epack record (no imputation), or the
+// kernels_condition.cuh record.
+static int condition_rec_floats(int n_obs, int nm, bool impute) {
+    return impute ? cond_rec_floats(cond_round4(n_obs), cond_round4(nm)) : epack_stride(n_obs);
+}
+static size_t condition_block_floats(int Kmax, int D) {
+    int rec = epack_stride(D);
+    for (int o = 1; o < D; o++) rec = std::max(rec, condition_rec_floats(o, D - o, true));
+    return (size_t)Kmax * rec;
+}
+
+// The parameter block of the current K clusters in the pinned mirror (gmm.h): the marginal set (mu_O, P_O, constant_O,
+// pi) goes through build_epack, at n_obs dimensions for score_simt_kernel, or zero-padded to a multiple of 4 and followed
+// by mu_M, G and c for condition_simt_kernel.  With nm = 0 the marginal set is the context's own arrays.
+static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const int* mis, int nm, bool impute) {
+    const int D = c->D;
+    float* block = c->cond.h_block;
+    if (nm == 0) {
+        build_epack(K, D, &c->host, block);
+        return GMM_OK;
+    }
+    const int DO = impute ? cond_round4(n_obs) : n_obs, NM = cond_round4(nm);
+    std::vector<float> mo((size_t)K * DO, 0.0f), po((size_t)K * DO * DO, 0.0f), co(K), g((size_t)K * nm * n_obs), cv((size_t)K * nm);
+    std::atomic<int> first_bad{K};
+    const std::function<void(int)> per_cluster = [&](int k) {
+        std::vector<float> p((size_t)n_obs * n_obs);
+        if (!condition_cluster(&c->host, k, D, obs, n_obs, mis, nm, p.data(), &co[k], &g[(size_t)k * nm * n_obs], &cv[(size_t)k * nm])) {
+            int cur = first_bad.load();
+            while (k < cur && !first_bad.compare_exchange_weak(cur, k)) {}
+            return;
+        }
+        for (int a = 0; a < n_obs; a++) {
+            mo[(size_t)k * DO + a] = c->host.means[(size_t)k * D + obs[a]];
+            for (int b = 0; b < n_obs; b++) po[(size_t)k * DO * DO + a * DO + b] = p[(size_t)a * n_obs + b];
+        }
+    };
+    if (K >= 8) {
+        if (!c->pool) c->pool = new HostPool(c->host_threads);
+        else c->pool->resize(c->host_threads);
+        c->pool->run(K, per_cluster);
+    } else {
+        for (int k = 0; k < K; k++) per_cluster(k);
+    }
+    if (first_bad.load() < K)
+        return fail(GMM_ERR_STATE, "gmm_condition: the block P_MM of cluster " + std::to_string(first_bad.load()) +
+                                       " (inverse covariance on the missing dimensions) is not positive definite");
+    clusters_t marg{};
+    marg.means = mo.data(); marg.Rinv = po.data(); marg.constant = co.data(); marg.pi = c->host.pi;
+    if (!impute) {
+        build_epack(K, DO, &marg, block);
+        return GMM_OK;
+    }
+    const int EP = epack_stride(DO), REC = condition_rec_floats(n_obs, nm, true);
+    std::vector<float> ep((size_t)K * EP);
+    build_epack(K, DO, &marg, ep.data());
+    std::memset(block, 0, sizeof(float) * (size_t)K * REC);
+    for (int k = 0; k < K; k++) {
+        float* r = block + (size_t)k * REC;
+        std::memcpy(r, &ep[(size_t)k * EP], sizeof(float) * EP);
+        float* mu = r + EP;
+        float* G = mu + NM;
+        float* cvar = G + (size_t)NM * DO;
+        for (int d = 0; d < nm; d++) {
+            mu[d] = c->host.means[(size_t)k * D + mis[d]];
+            for (int o = 0; o < n_obs; o++) G[d * DO + o] = g[((size_t)k * nm + d) * n_obs + o];
+            cvar[d] = cv[(size_t)k * nm + d];
+        }
+    }
+    return GMM_OK;
+}
+
+// condition_simt_kernel<NO, NM> for the observed / imputed counts rounded up to multiples of 4 (NO + NM <= 36: 36 instances)
+static int launch_condition(gmm_ctx* c, int n_obs, int nm, int K, const float* block, const TcScoreIo& io, float* mean, float* var) {
+    if (io.n <= 0) return GMM_OK;
+    const int grid = (io.n + kEstepThreads - 1) / kEstepThreads;
+    switch (cond_round4(n_obs) / 4 * 16 + cond_round4(nm) / 4) {
+#define GMM_CASE(a, b)                                                                                                          \
+    case (a) * 16 + (b):                                                                                                        \
+        condition_simt_kernel<4 * (a), 4 * (b)><<<grid, kEstepThreads, 0, c->stream>>>(io.x, io.n, n_obs, nm, K, block, io.labels, \
+                                                                                      io.max_resp, io.logp, io.ll, mean, var);  \
+        break;
+        GMM_CASE(1, 1) GMM_CASE(1, 2) GMM_CASE(1, 3) GMM_CASE(1, 4) GMM_CASE(1, 5) GMM_CASE(1, 6) GMM_CASE(1, 7) GMM_CASE(1, 8)
+        GMM_CASE(2, 1) GMM_CASE(2, 2) GMM_CASE(2, 3) GMM_CASE(2, 4) GMM_CASE(2, 5) GMM_CASE(2, 6) GMM_CASE(2, 7)
+        GMM_CASE(3, 1) GMM_CASE(3, 2) GMM_CASE(3, 3) GMM_CASE(3, 4) GMM_CASE(3, 5) GMM_CASE(3, 6)
+        GMM_CASE(4, 1) GMM_CASE(4, 2) GMM_CASE(4, 3) GMM_CASE(4, 4) GMM_CASE(4, 5)
+        GMM_CASE(5, 1) GMM_CASE(5, 2) GMM_CASE(5, 3) GMM_CASE(5, 4)
+        GMM_CASE(6, 1) GMM_CASE(6, 2) GMM_CASE(6, 3)
+        GMM_CASE(7, 1) GMM_CASE(7, 2)
+        GMM_CASE(8, 1)
+#undef GMM_CASE
+        default: return fail(GMM_ERR_ARG, "gmm_condition: unsupported split of the dimensions");
+    }
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+
+// Chunks of c->score_chunk events through gmm_score's slots, in score_batch's order: host rows -> pinned stage -> (copy
+// stream) device chunk -> (compute stream) kernel -> (copy stream) outputs and imputations -> pinned mirrors -> caller's
+// arrays; chunk i is issued before chunk i - 1 is handed over.
+static int condition_batch(gmm_ctx* c, int K, int n_obs, int nm, bool impute, const float* ev, long long n, int* labels,
+                           float* max_resp, float* logp, float* cmean, float* cvar, double* ll_sum) {
+    ScoreBuffers& s = c->score;
+    ConditionBuffers& cb = c->cond;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
+    const size_t var_off = (size_t)chunk * nm;             // cond_var's offset in a slot's imputation buffer
+    CUDA_TRY(cudaMemcpyAsync(cb.d_block, cb.h_block, sizeof(float) * (size_t)K * condition_rec_floats(n_obs, nm, impute),
+                             cudaMemcpyHostToDevice, c->stream));
+    auto issue = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
+        std::memcpy(s.h_in[b], ev + (size_t)e0 * n_obs, sizeof(float) * (size_t)m * n_obs);
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the chunk buffer's previous kernel is done with it
+        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * n_obs, cudaMemcpyHostToDevice, s.copy));
+        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous outputs have left the device
+        const TcScoreIo dv = score_io(c, s.d_out[b], b, m), hv = score_io(c, s.h_out[b], b, m);
+        CUDA_TRY(cudaMemsetAsync(s.d_out[b], 0, ScoreBuffers::kHeader, c->stream));
+        CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
+        const int rc = impute ? launch_condition(c, n_obs, nm, K, cb.d_block, dv, cb.d_imp[b], cvar ? cb.d_imp[b] + var_off : nullptr)
+                              : launch_score_simt(c, n_obs, K, cb.d_block, dv);
+        if (rc) return rc;
+        CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
+        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
+        CUDA_TRY(cudaMemcpyAsync(s.h_out[b], s.d_out[b], ScoreBuffers::kHeader, cudaMemcpyDeviceToHost, s.copy));
+        if (labels) CUDA_TRY(cudaMemcpyAsync(hv.labels, dv.labels, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
+        if (max_resp) CUDA_TRY(cudaMemcpyAsync(hv.max_resp, dv.max_resp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
+        if (logp) CUDA_TRY(cudaMemcpyAsync(hv.logp, dv.logp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
+        if (impute && cmean)
+            CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b], cb.d_imp[b], sizeof(float) * (size_t)m * nm, cudaMemcpyDeviceToHost, s.copy));
+        if (impute && cvar)
+            CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b] + var_off, cb.d_imp[b] + var_off, sizeof(float) * (size_t)m * nm,
+                                     cudaMemcpyDeviceToHost, s.copy));
+        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
+        return GMM_OK;
+    };
+    auto finish = [&](long long i) -> int {
+        const int b = (int)(i & 1);
+        const long long e0 = i * chunk;
+        const int m = (int)std::min(chunk, n - e0);
+        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) cb.kernel_ms += ms;
+        const TcScoreIo hv = score_io(c, s.h_out[b], b, m);
+        *ll_sum += *hv.ll;
+        if (labels) std::memcpy(labels + e0, hv.labels, sizeof(int) * (size_t)m);
+        if (max_resp) std::memcpy(max_resp + e0, hv.max_resp, sizeof(float) * (size_t)m);
+        if (logp) std::memcpy(logp + e0, hv.logp, sizeof(float) * (size_t)m);
+        if (impute && cmean) std::memcpy(cmean + (size_t)e0 * nm, cb.h_imp[b], sizeof(float) * (size_t)m * nm);
+        if (impute && cvar) std::memcpy(cvar + (size_t)e0 * nm, cb.h_imp[b] + var_off, sizeof(float) * (size_t)m * nm);
+        return GMM_OK;
+    };
+    for (long long i = 0; i < nchunks; i++) {
+        if (int rc = issue(i)) return rc;
+        if (i > 0)
+            if (int rc = finish(i - 1)) return rc;
+    }
+    return finish(nchunks - 1);
+}
+
+int gmm_condition(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n, int* labels,
+                  float* max_resp, float* logp, float* cond_mean, float* cond_var, double* loglik_out) {
+    if (int rc = check_K(c, K, "gmm_condition")) return rc;
+    if (n < 0 || (n > 0 && !events_obs)) return fail(GMM_ERR_ARG, "gmm_condition: bad events (n < 0, or no rows)");
+    if (!obs_dims || n_obs < 1 || n_obs > c->D)
+        return fail(GMM_ERR_ARG, "gmm_condition: obs_dims must hold between 1 and D dimension indices");
+    for (int i = 0; i < n_obs; i++)
+        if (obs_dims[i] < 0 || obs_dims[i] >= c->D || (i > 0 && obs_dims[i] <= obs_dims[i - 1]))
+            return fail(GMM_ERR_ARG, "gmm_condition: obs_dims must be strictly increasing indices in [0, D)");
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_condition: parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, "gmm_condition: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    ConditionBuffers& cb = c->cond;
+    if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
+    if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
+    int mis[GMM_MAX_DIMENSIONS];
+    int nm = 0;
+    for (int d = 0, i = 0; d < c->D; d++) {
+        if (i < n_obs && obs_dims[i] == d) i++;
+        else mis[nm++] = d;
+    }
+    const bool impute = nm > 0 && (cond_mean || cond_var);
+    double ll = 0.0;
+    int rc = condition_params(c, K, obs_dims, n_obs, mis, nm, impute);
+    if (rc == GMM_OK && n > 0) {
+        rc = score_buffers(c);
+        const size_t want = 2 * (size_t)c->score_chunk * nm;
+        if (rc == GMM_OK && impute && cb.imp_floats < want) {
+            cb.release_imp();
+            for (int b = 0; b < 2 && rc == GMM_OK; b++) {
+                cudaError_t e = cudaMalloc(&cb.d_imp[b], sizeof(float) * want);
+                if (e == cudaSuccess) e = cudaMallocHost(&cb.h_imp[b], sizeof(float) * want);
+                if (e != cudaSuccess) rc = fail(GMM_ERR_CUDA, std::string("gmm_condition: imputation buffers: ") + cudaGetErrorString(e));
+            }
+            if (rc == GMM_OK) cb.imp_floats = want;
+            else cb.release_imp();
+        }
+        if (rc == GMM_OK) rc = condition_batch(c, K, n_obs, nm, impute, events_obs, n, labels, max_resp, logp, cond_mean, cond_var, &ll);
+        // nothing of this call may still be in flight when it returns (also after a failure)
+        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
+        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = fail(GMM_ERR_CUDA, std::string("gmm_condition: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        if (rc == GMM_OK && loglik_out) *loglik_out = ll;
+    }
+    cb.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_get_condition_profile(gmm_ctx* c, double out[2], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_condition_profile: bad argument");
+    out[0] = c->cond.kernel_ms; out[1] = c->cond.wall_ms;
+    if (reset) c->cond.kernel_ms = c->cond.wall_ms = 0;
     return GMM_OK;
 }
 

@@ -340,6 +340,61 @@ void build_epack(int K, int D, const clusters_t* c, float* out) {
     }
 }
 
+bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_obs, const int* mis, int nm, float* p_o,
+                       float* constant_o, float* g, float* cvar) {
+    constexpr int DM = GMM_MAX_DIMENSIONS;
+    const float* P = c->Rinv + (size_t)k * D * D;
+    auto S = [&](int i, int j) { return 0.5 * ((double)P[i * D + j] + (double)P[j * D + i]); };
+    double L[DM][DM], Y[DM][DM], Z[DM][DM], Li[DM][DM];
+    double ld = 0.0;
+    for (int j = 0; j < nm; j++) {                          // S_MM = L L^T
+        double s = S(mis[j], mis[j]);
+        for (int t = 0; t < j; t++) s -= L[j][t] * L[j][t];
+        if (!(s > 0.0) || !std::isfinite(s)) return false;
+        L[j][j] = std::sqrt(s);
+        ld += std::log(L[j][j]);
+        for (int i = j + 1; i < nm; i++) {
+            double v = S(mis[i], mis[j]);
+            for (int t = 0; t < j; t++) v -= L[i][t] * L[j][t];
+            L[i][j] = v / L[j][j];
+        }
+    }
+    for (int o = 0; o < n_obs; o++) {
+        for (int i = 0; i < nm; i++) {                      // Y = L^-1 S_MO
+            double v = S(mis[i], obs[o]);
+            for (int t = 0; t < i; t++) v -= L[i][t] * Y[t][o];
+            Y[i][o] = v / L[i][i];
+        }
+        for (int i = nm - 1; i >= 0; i--) {                 // Z = L^-T Y = S_MM^-1 S_MO
+            double v = Y[i][o];
+            for (int t = i + 1; t < nm; t++) v -= L[t][i] * Z[t][o];
+            Z[i][o] = v / L[i][i];
+        }
+    }
+    for (int a = 0; a < n_obs; a++)                         // S_OO - S_OM S_MM^-1 S_MO = S_OO - Y^T Y
+        for (int b = a; b < n_obs; b++) {
+            double v = S(obs[a], obs[b]);
+            for (int t = 0; t < nm; t++) v -= Y[t][a] * Y[t][b];
+            p_o[a * n_obs + b] = p_o[b * n_obs + a] = (float)v;
+        }
+    for (int j = 0; j < nm; j++) {                          // L^-1, lower triangular; S_MM^-1 = L^-T L^-1
+        Li[j][j] = 1.0 / L[j][j];
+        for (int i = j + 1; i < nm; i++) {
+            double v = 0.0;
+            for (int t = j; t < i; t++) v -= L[i][t] * Li[t][j];
+            Li[i][j] = v / L[i][i];
+        }
+    }
+    for (int d = 0; d < nm; d++) {
+        double v = 0.0;
+        for (int i = d; i < nm; i++) v += Li[i][d] * Li[i][d];
+        cvar[d] = (float)v;
+        for (int o = 0; o < n_obs; o++) g[d * n_obs + o] = (float)(-Z[d][o]);
+    }
+    *constant_o = (float)((double)c->constant[k] + 0.5 * nm * std::log(2.0 * M_PI) - ld);
+    return true;
+}
+
 }  // namespace gmm
 
 // ---------------------------------------------------------------------------

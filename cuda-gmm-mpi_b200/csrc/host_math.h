@@ -64,4 +64,14 @@ int reduce_order(clusters_t* c, int K, int D, int* c1, int* c2, int num_threads,
 int  epack_stride(int D);
 void build_epack(int K, int D, const clusters_t* c, float* out);
 
+// gmm_condition's parameters of cluster k (gmm.h): in double from the float Rinv of c, S = (Rinv + Rinv^T) / 2, split
+// into the observed dimensions obs[n_obs] and the missing ones mis[nm] (nm >= 1), rounded to float:
+//   p_o [n_obs][n_obs] = S_OO - S_OM S_MM^-1 S_MO    (marginal precision, symmetric)
+//   *constant_o        = constant + nm/2 ln 2 pi - 1/2 ln det S_MM
+//   g [nm][n_obs]      = -S_MM^-1 S_MO               (regression of the missing dimensions on dx_O)
+//   cvar [nm]          = diag(S_MM^-1)                (conditional variances)
+// S_MM is factorised once (Cholesky).  false = S_MM is not positive definite (a pivot <= 0 or not finite); nothing written.
+bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_obs, const int* mis, int nm, float* p_o,
+                       float* constant_o, float* g, float* cvar);
+
 }  // namespace gmm

@@ -104,18 +104,43 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
 }
 
 // ---------------------------------------------------------------------------
+// One cluster of the scoring loop, shared by score_simt_kernel and condition_simt_kernel (kernels_condition.cuh), on the
+// record p (epack layout) of cluster k: dx = x - mu and the logit l = constant + ln pi - q / 2 with the E-step's
+// operations, the running arg-max (lowest k on ties; NaN logits never win) and the online log-sum-exp.  It declares
+// dx[D] and l in the enclosing scope, where the caller reads them.  A macro rather than a function: expanded in place,
+// score_simt_kernel keeps the statements, and so the machine code, it had when they were written out in it (an inlined
+// function with reference parameters reorders ptxas's output).
+// ---------------------------------------------------------------------------
+#define GMM_SCORE_CLUSTER(D, x, p, k, dx, l, run_max, run_sum, best_l, best_k)                      \
+    float dx[D];                                                                                    \
+    _Pragma("unroll") for (int d_ = 0; d_ < (D); d_++) dx[d_] = x[d_] - p[d_];                      \
+    float q_ = 0.0f;                                                                                \
+    int idx_ = ((D) + 3) & ~3;                                                                      \
+    _Pragma("unroll") for (int i_ = 0; i_ < (D); i_++) {                                            \
+        float t_ = 0.0f;                                                                            \
+        _Pragma("unroll") for (int j_ = i_; j_ < (D); j_++) t_ = fmaf(p[idx_++], dx[j_], t_);       \
+        q_ = fmaf(dx[i_], t_, q_);                                                                  \
+    }                                                                                               \
+    const float l = fmaf(-0.5f, q_, p[(((D) + 3) & ~3) + (D) * ((D) + 1) / 2]);                     \
+    if (l > best_l || (best_k < 0 && l == l)) { best_l = l; best_k = k; }                           \
+    {                                                                                               \
+        const float m2_ = fmaxf(run_max, l);                                                        \
+        run_sum = run_sum * expf(run_max - m2_) + expf(l - m2_);                                    \
+        run_max = m2_;                                                                              \
+    }
+
+// ---------------------------------------------------------------------------
 // Scoring of new events (gmm_score) for every D and any K in one launch: the E-step above with the same cluster staging
 // and the same logit arithmetic, reading the caller's AoS chunk [n][D] directly, keeping an online log-sum-exp and a
 // running arg-max (lowest k on ties; NaN logits never win, -1 when every logit is NaN) and storing only the label,
 // max_resp = expf(l_max - denom) (bit-identical to the stored responsibility of estep_simt_kernel) and logp = denom.
+// gmm_condition runs it on its marginal parameters, with D = the number of observed dimensions.
 // ---------------------------------------------------------------------------
 template <int D>
 __global__ void __launch_bounds__(kEstepThreads)
 score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __restrict__ epack, int* __restrict__ labels,
                   float* __restrict__ max_resp, float* __restrict__ logp, double* __restrict__ ll_out) {
     constexpr int STRIDE = epack_stride_c(D);
-    constexpr int COEF = (D + 3) & ~3;
-    constexpr int NCOEF = D * (D + 1) / 2;
     __shared__ __align__(16) float sp[kEstepClusterChunk * STRIDE];
     __shared__ double sred[kEstepThreads / 32];
 
@@ -138,23 +163,7 @@ score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __
         __syncthreads();
         for (int kk = 0; kk < kc; kk++) {
             const float* p = sp + kk * STRIDE;
-            float dx[D];
-#pragma unroll
-            for (int d = 0; d < D; d++) dx[d] = x[d] - p[d];
-            float q = 0.0f;
-            int idx = COEF;
-#pragma unroll
-            for (int i = 0; i < D; i++) {
-                float t = 0.0f;
-#pragma unroll
-                for (int j = i; j < D; j++) t = fmaf(p[idx++], dx[j], t);
-                q = fmaf(dx[i], t, q);
-            }
-            const float l = fmaf(-0.5f, q, p[COEF + NCOEF]);
-            if (l > best_l || (best_k < 0 && l == l)) { best_l = l; best_k = k0 + kk; }
-            const float m2 = fmaxf(run_max, l);
-            run_sum = run_sum * expf(run_max - m2) + expf(l - m2);
-            run_max = m2;
+            GMM_SCORE_CLUSTER(D, x, p, k0 + kk, dx, l, run_max, run_sum, best_l, best_k)
         }
     }
     const float denom = run_max + logf(run_sum);

@@ -84,6 +84,9 @@ def load_library():
     L.gmm_get_score_stats_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_sample.argtypes = [C.c_void_p, C.c_int, C.c_longlong, C.c_ulonglong, C.c_longlong, C.c_void_p, C.c_void_p]
     L.gmm_get_sample_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_condition.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p, _DP]
+    L.gmm_get_condition_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
@@ -348,6 +351,32 @@ class Engine:
     def sample_profile(self, reset=False):
         out = (C.c_double * 2)()
         _check(self.lib.gmm_get_sample_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1])
+
+    def condition(self, K, obs_dims, events_obs, labels=True, max_resp=True, logp=True, mean=True, var=False):
+        """Score events measured on the dimensions obs_dims only and impute the others (gmm_condition) under the current
+        K-cluster parameters.  events_obs is [n][len(obs_dims)].  Returns (labels int32, max_resp float32, logp float32,
+        mean float32 [n][NM], var float32 [n][NM], loglik) with None for outputs not asked for; NM = D - len(obs_dims),
+        and mean / var are None when NM = 0."""
+        obs = np.ascontiguousarray(obs_dims, np.int32).reshape(-1)
+        ev = np.ascontiguousarray(events_obs, np.float32)
+        if ev.ndim != 2 or ev.shape[1] != obs.size:
+            raise ValueError(f"events_obs must be [n][{obs.size}], got {ev.shape}")
+        n, nm = ev.shape[0], self.D - obs.size
+        lab = np.empty(n, np.int32) if labels else None
+        mr = np.empty(n, np.float32) if max_resp else None
+        lp = np.empty(n, np.float32) if logp else None
+        cm = np.empty((n, nm), np.float32) if mean and nm > 0 else None
+        cv = np.empty((n, nm), np.float32) if var and nm > 0 else None
+        ptr = lambda a: a.ctypes.data if a is not None and a.size else None  # noqa: E731
+        ll = C.c_double(0.0)
+        _check(self.lib.gmm_condition(self.h, K, obs.ctypes.data if obs.size else None, int(obs.size), ptr(ev), n, ptr(lab),
+                                      ptr(mr), ptr(lp), ptr(cm), ptr(cv), C.byref(ll)))
+        return lab, mr, lp, cm, cv, ll.value
+
+    def condition_profile(self, reset=False):
+        out = (C.c_double * 2)()
+        _check(self.lib.gmm_get_condition_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], wall_ms=out[1])
 
     def fit_profile(self):

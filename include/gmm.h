@@ -315,6 +315,46 @@ int  gmm_sample(gmm_ctx*, int K, long long n, unsigned long long seed, long long
 /* Since the last reset: out[0] sampling-kernel ms, out[1] wall ms inside gmm_sample.                   */
 int  gmm_get_sample_profile(gmm_ctx*, double out[2], int reset);
 
+/* Score n events measured on a subset O of the dimensions, and impute the others, under the parameter set the next
+ * gmm_estep(ctx, K) would use (statistical file matching of panels that share a backbone; Gaussian-mixture regression).
+ *   obs_dims [n_obs]   strictly increasing indices in [0, D): the set O.  M = the other dimensions in increasing
+ *                      order, NM = D - n_obs of them.
+ *   events_obs         [n][n_obs] row-major, the coordinates of O in the order of obs_dims.
+ *   labels, max_resp, logp   as gmm_score defines them, for the MARGINAL mixture sum_k pi_k N(x_O | mu_kO, R_kOO).
+ *   cond_mean [n][NM]  E[x_M | x_O];  cond_var [n][NM]  the diagonal of Cov[x_M | x_O].  Ignored when NM = 0.
+ *   *loglik_out        sum of logp in double over this call, THIS context only.
+ * Every output pointer may be NULL.  No collective; nothing of the EM state changes (memberships, statistics,
+ * log-likelihood, the SIMT E-step's parameters, gmm_get_profile, gmm_get_score_profile, gmm_get_score_stats_profile,
+ * gmm_get_sample_profile).
+ * Semantics (restated in float64 numpy by tests/_condition_ref.py), from the float means, Rinv (P), constant and pi of
+ * the context's host copy, per cluster k:
+ *   - NM = 0: the marginal set is (means, Rinv, constant, pi) itself, so the outputs are gmm_score's SIMT kernel's.
+ *   - NM >= 1, in double: S = (P + P^T) / 2; S_MM = L L^T (Cholesky; a pivot <= 0 or not finite -> GMM_ERR_STATE);
+ *       P_O        = S_OO - S_OM S_MM^-1 S_MO                      (the inverse of R_OO)
+ *       constant_O = constant + (NM/2) ln 2 pi - (1/2) ln det S_MM  (ln det R_OO = ln det R + ln det P_MM)
+ *       G          = -S_MM^-1 S_MO  [NM][n_obs],   c_d = (S_MM^-1)_dd
+ *     each rounded to float.  The marginal set (mu_O, P_O, constant_O, pi) is packed as the SIMT E-step packs its
+ *     parameters (coefficients P_ii and P_ij + P_ji, constant_O + logf(pi) in float).
+ *   - scoring: gmm_score's SIMT kernel on the marginal set: dx = x_O - mu_kO, l_k = constant_O + ln pi_k - dx^T P_O dx / 2
+ *     in float, online log-sum-exp and arg-max.  Computing the imputations too changes no bit of labels, max_resp, logp.
+ *   - imputation, in float: m_k = mu_kM + G_k dx (G_k dx summed first), r_k = exp(l_k - logp);
+ *     cond_mean = sum_k r_k m_k,  cond_var = sum_k r_k (c_k + (m_k - cond_mean)^2), merged cluster by cluster with a
+ *     weighted running mean and sum of squares (West 1979), rescaled when the running maximum logit moves.
+ *   Events with a coordinate that is not finite give what gmm_score's SIMT kernel gives (label -1, NaN) and NaN
+ *   imputations.  The result of an event does not depend on the chunking or on the split into calls.
+ * Rows stream in chunks of option "score_chunk" events through gmm_score's two device chunks, pinned stages and copy
+ * stream.  A parameter block for Kmax clusters (at most 700 floats per cluster, at D = 32) and its pinned mirror are
+ * allocated on the first call; an imputing call adds per slot 2 x score_chunk x NM floats on the device and pinned,
+ * grown to the largest chunk x NM seen.  gmm_destroy frees them.
+ * Errors: K outside [1, Kmax], n < 0, events_obs == NULL with n > 0, obs_dims == NULL, n_obs outside [1, D], or indices
+ * that are not strictly increasing or out of range -> GMM_ERR_ARG; K != the K of the current parameters, a call between
+ * gmm_mstep and gmm_constants, or a cluster whose block P_MM is not positive definite (the first one is named in the
+ * message) -> GMM_ERR_STATE.  n = 0 returns GMM_OK after these checks and writes nothing, *loglik_out included.        */
+int  gmm_condition(gmm_ctx*, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n,
+                   int* labels, float* max_resp, float* logp, float* cond_mean, float* cond_var, double* loglik_out);
+/* Since the last reset: out[0] kernel ms, out[1] wall ms inside gmm_condition.                                        */
+int  gmm_get_condition_profile(gmm_ctx*, double out[2], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
