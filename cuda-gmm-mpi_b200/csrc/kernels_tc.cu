@@ -31,15 +31,14 @@
 //
 // Dataflow per CTA (persistent over a contiguous range of events, 32 clusters per CTA row of the grid):
 //   warp 0      TMA producer: tile [D][32 events] of the pre-standardised SoA copy z and raw
-//               responsibility tile [32 clusters][32 events] (2-D tensor maps, SWIZZLE_128B for
-//               the latter, zero fill out of bounds)
-//   warps 4-11  operand builders (two warpgroups on alternate tiles): form the products, split
-//               them, write the wgmma operand images (no-swizzle core-matrix layout)
-//   warpgroups 3 .. 2+MT  consumers, one per 128-row feature tile: per 32 events 2 x 2 x 3 m64n32k16 wgmma, committed
-//               as one group, with the accumulators in registers; a sub-tile's group is still running while the next
-//               sub-tile's MMAs are issued (three operand stages).  The exact group is drained every 128 events and the
-//               remainder group every 512 into FP32 round-to-nearest partial sums held in shared memory (one private
-//               slot per thread), written ONCE per CTA (no scratch zeroing, no atomics).
+//               responsibility tile [32 clusters][32 events] (2-D tensor maps, both SWIZZLE_128B, zero fill out of bounds)
+//   warps 1-3   split the responsibilities and write the wgmma B images gh / gl / gs (no-swizzle core-matrix layout)
+//   warpgroups 1 .. MT  consumers, one per 128-row feature tile: each thread builds the A fragments of its 4 feature rows
+//               (mstep_rows.h) from the raw z tile in registers — the feature operand never goes through shared memory —
+//               and per 32 events the warpgroup issues 2 x 2 x 3 m64n32k16 wgmma (A from registers), one group per
+//               64-row half, the group of one half running while the other half is built.  The exact group is drained
+//               every 128 events and the remainder group every 512 into FP32 round-to-nearest partial sums held in shared
+//               memory (one private slot per thread), written ONCE per CTA (no scratch zeroing, no atomics).
 // A second tiny kernel reduces the per-CTA partials in double and un-scales.
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -58,6 +57,7 @@
 
 #include "host_math.h"
 #include "kernels_tc.cuh"
+#include "mstep_rows.h"
 #include "tc_ptx.cuh"
 
 namespace gmm {
@@ -76,7 +76,7 @@ using namespace ptx;
 // ---------------------------------------------------------------------------
 constexpr int kTE = 32;          // events per sub-tile (MMA K extent per operand part)
 constexpr int kNCL = 32;         // clusters per CTA pass (N of the exact / remainder groups: register budget of the consumers)
-constexpr int kNST = 3;          // operand stages: one read by the in-flight MMAs, one built by each builder warpgroup
+constexpr int kNST = 3;          // responsibility operand stages
 constexpr int kNRAW = 4;         // raw (TMA) stages
 constexpr int kChunkSub = 4;     // sub-tiles per chain of the exact column group: 128 events (the bit budget below)
 constexpr int kChunkSub2 = 16;   // sub-tiles per chain of the remainder column group (no exactness to protect: drained 4x less often)
@@ -87,54 +87,40 @@ constexpr int kPhiBits = 11;     // |ph| <= 2^11 quanta
 constexpr float kGammaScale = 1024.0f;               // responsibilities are scaled by 2^10 in the operand
 constexpr float kGammaMagic = 1.5f * 134217728.0f;   // 1.5 * 2^27: ulp = 16 = 2^-6 in the scaled units
 
-// Row layout of the feature operand.  The four warps of a builder warpgroup run ONE instruction stream (round 1 / early
-// round 2 unrolled a different quarter of the feature list per warp: 50 KB of SASS against a 32 KB L1.5 instruction cache,
-// a third of the builders' stall samples were instruction fetch): warp p loads the event's coordinates ROTATED by p*D/4
-// dimensions (a run-time shared-memory address) and evaluates the same canonical list of RPP rows on them —
-//     r = 0                      1
-//     r = 1 + a          (a < S) z'_a
-//     r = 1 + S + a      (a < S) z'_a^2
-//     r = 1 + 2S + a*D/2 + (d-1) (a < S, 1 <= d <= D/2)   z'_a * z'_{(a+d) mod D}
-// with z'_t = z_{(t + pS) mod D}, S = D/4.  The rotations of the canonical pairs cover every unordered pair of
-// dimensions once, except the D/2 antipodal pairs (d = D/2), which two warps produce (one copy is ignored), and the
-// constant row (kept from warp 0).  Warp p writes operand rows [p*CPP*8, p*CPP*8 + RPP); tc_row_map() gives the packed
-// statistic each row feeds.
+// Row layout of the feature operand: mstep_rows.h.  Every operand row is a product z_a * z_b of two factors (a dimension
+// or the ones pseudo-dimension); consumer thread (warp w, lane group gid) of tile mt owns the 4 rows
+// mt * 128 + h * 64 + 16 w + gid + 8 s, which share the factor a.  The thread builds the wgmma A fragments of its rows
+// from the raw z tile itself (register operand), so the feature operand never goes through shared memory.
 template <int D> struct MCfg {
     static_assert(D % 4 == 0, "tensor M-step: D must be a multiple of 4");
     static constexpr int F = 1 + D + D * (D + 1) / 2;
-    static constexpr int S = D / 4;                       // rotation step between the four builder warps
-    static constexpr int RPP = 1 + 2 * S + S * (D / 2);   // canonical rows per warp
-    static constexpr int CPP = (RPP + 7) / 8;             // 16-byte chunks per warp
-    static constexpr int NCHUNK = 4 * CPP;                // chunks written per event
-    static constexpr int MT = (NCHUNK * 8 + 127) / 128;   // M tiles of 128 feature rows
-    // Bytes of one part (leading or remainder): only the NCHUNK * 8 rows the builders write.  The MMAs of the last tile
-    // read up to MT * 128 rows, i.e. past the end of the part into the next part or the gamma stages: FP16 values that
-    // land only in accumulator rows tc_row_info() marks as unused.
-    static constexpr int PHI_PART = NCHUNK * 8 * kTE * 2;
-    static constexpr int PHI_STAGE = 2 * PHI_PART;
+    static constexpr int S = D / 4;
+    static constexpr int MT = (4 * ((1 + 2 * S + S * (D / 2) + 7) / 8) * 8 + 127) / 128;   // feature tiles (mstep_tiles)
     static constexpr int G_PART = kNCL * kTE * 2;
     static constexpr int G_STAGE = 3 * G_PART;            // gh, gl, gs: three K-major N = 32 images
-    static constexpr int RAWX = D * kTE * 4;              // [D][32 events] from the SoA copy
+    // raw z stage: the [D][32 events] tile (SWIZZLE_128B), padded to 1 KB, then 1 KB of ones (8 rows of the same swizzle:
+    // the ones pseudo-dimension at a stage-relative address like every dimension)
+    static constexpr int RAWZ = (D * kTE * 4 + 1023) / 1024 * 1024;
+    static constexpr int RAWX = RAWZ + 1024;
     static constexpr int RAWG = kNCL * kTE * 4;
-    static constexpr int OFF_PHI = 0;
-    static constexpr int OFF_G = OFF_PHI + kNST * PHI_STAGE;
+    static constexpr int OFF_G = 0;
     static constexpr int OFF_RAWX = OFF_G + kNST * G_STAGE;
     static constexpr int OFF_RAWG = OFF_RAWX + kNRAW * RAWX;
     static constexpr int NCT = MT * 128;                  // consumer threads (one warpgroup per 128-row feature tile)
     static constexpr int OFF_RACC = OFF_RAWG + kNRAW * RAWG;   // [32][NCT] FP32 partial sums, one private column per thread
     static constexpr int OFF_BAR = OFF_RACC + 32 * NCT * 4;
     static constexpr int SMEM_BYTES = OFF_BAR + 512;
-    static constexpr int THREADS = 384 + NCT;             // producer warpgroup, two builder warpgroups, consumers
-    // register pools: producer / builders / consumers.  The kernel is launched with REG_LAUNCH registers per thread
+    static constexpr int THREADS = 128 + NCT;             // producer warpgroup, consumers
+    // register pools: producer warpgroup / consumers.  The kernel is launched with REG_LAUNCH registers per thread
     // (the __launch_bounds__ maximum, which ptxas uses when setmaxnreg is present); setmaxnreg only redistributes that
     // allocation, so a warpgroup's increase waits until the others' decreases have freed enough — the sum must fit.
+    // With one feature tile (256 threads) every thread may have 255 registers: no redistribution.
     static constexpr int REG_LAUNCH = (65536 / THREADS) / 8 * 8 > 255 ? 255 : (65536 / THREADS) / 8 * 8;
-    static constexpr int REG_P = MT == 1 ? 40 : 24;
-    static constexpr int REG_B = MT == 3 ? 80 : 112;
-    static constexpr int REG_C = MT == 3 ? 96 : (MT == 2 ? 112 : 240);
-    static_assert(128 * REG_P + 256 * REG_B + NCT * REG_C <= THREADS * REG_LAUNCH, "register pools");
+    static constexpr int REG_P = MT == 1 ? REG_LAUNCH : 56;
+    static constexpr int REG_C = MT == 3 ? 152 : (MT == 2 ? 224 : REG_LAUNCH);
+    static_assert(128 * REG_P + NCT * REG_C <= THREADS * REG_LAUNCH, "register pools");
+    static_assert(OFF_RAWX % 1024 == 0 && RAWX % 1024 == 0 && RAWZ % 1024 == 0, "SWIZZLE_128B TMA destinations need 1024-byte alignment");
     static_assert(OFF_RAWG % 1024 == 0 && RAWG % 1024 == 0, "SWIZZLE_128B TMA destinations need 1024-byte alignment");
-    static_assert((MT * 128 - NCHUNK * 8) * kTE * 2 <= kNST * G_STAGE, "the last part's over-read stays inside the operand stages");
     static_assert(MT <= 3, "feature tiles");
 };
 
@@ -149,75 +135,85 @@ __device__ __forceinline__ void set_regs() {
 // to a power of two: after the standardisation the dimensions have the same scale).
 struct MMagic { float lin, prod; };
 
-__host__ __device__ constexpr int tri_row(int t) {        // t = i(i+1)/2 + j, j <= i  ->  i
-    int i = 0;
-    while ((i + 1) * (i + 2) / 2 <= t) i++;
-    return i;
-}
-
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tmap, int c0, int c1, uint64_t* bar) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(c0), "r"(c1), "r"(smem_u32(bar)) : "memory");
 }
 
-// Leading part / remainder of canonical row r for the (rotated) event z (r is a compile-time constant after
-// unrolling).  Products: both parts come from the EXACT product (fused multiply-adds), rounded once each.
-template <int D>
-__device__ __forceinline__ void feature_split(const float (&z)[D], int r, const MMagic& mg, float& h, float& l) {
-    using C = MCfg<D>;
-    if (r == 0) { h = 1.0f; l = 0.0f; }
-    else if (r <= C::S) {
-        const float v = z[r - 1];
-        h = __fsub_rn(__fadd_rn(v, mg.lin), mg.lin);
-        l = __fsub_rn(v, h);
-    } else if (r < C::RPP) {
-        int a, b;
-        if (r <= 2 * C::S) { a = r - 1 - C::S; b = a; }
-        else { const int t = r - 1 - 2 * C::S; a = t / (D / 2); b = (a + 1 + t % (D / 2)) % D; }
-        h = __fsub_rn(__fmaf_rn(z[a], z[b], mg.prod), mg.prod);
-        l = __fmaf_rn(z[a], z[b], -h);
-    } else { h = 0.0f; l = 0.0f; }
+__device__ __forceinline__ float2 lds_f2(uint32_t addr) {
+    float2 v;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(addr) : "memory");
+    return v;
 }
 
-// Builds the CPP 16-byte chunks of one event for builder warp `part` and stores both parts into the MN-major operand image:
-//   byte(row, e) = (row/8)*512 + (e/8)*128 + (e%8)*16 + (row%8)*2        (LBO = 128, SBO = 512)
-template <int D>
-__device__ __forceinline__ void build_phi_chunks(const float (&z)[D], const MMagic& mg, uint8_t* hi_base, uint8_t* lo_base, int e, int part) {
-    using C = MCfg<D>;
-    const int eoff = part * (C::CPP * 512) + (e >> 3) * 128 + (e & 7) * 16;
+// Leading part / remainder of the feature a * b with rounding constant m: the product rows' operations of the staged
+// layout for every row — a linear row is z_a * 1 (fma(z, 1, m) - m and fma(z, 1, -h) round as (z + m) - m and z - h),
+// the constant row is 1 * 1 with m = 0.  Both parts come from the EXACT product, rounded once each.
+__device__ __forceinline__ void feature_split(float a, float b, float m, float& h, float& l) {
+    h = __fsub_rn(__fmaf_rn(a, b, m), m);
+    l = __fmaf_rn(a, b, -h);
+}
+
+// Timing variants for scripts/prof_mstep.py (`make variant DEFS=-DGMM_MSTEP_CUT=n`); the default build is 0.
+//   1  no MMAs: loads and operand build only (the fragments are kept alive, the stages released at the same points; with
+//      no wgmma to wait on, the raw stage may be released before its loads land)
+//   2  no feature build: the MMAs read the raw z words as their A fragments
+//   3  no drains: the accumulators are added to the partial sums once, after the last sub-tile
+// The results of a variant are wrong.
+#ifndef GMM_MSTEP_CUT
+#define GMM_MSTEP_CUT 0
+#endif
+
+// A fragments of one 64-row half: rows s = 0, 1 of the thread (slot 2h + s), events 16 ks + 2 qd + {0, 1, 8, 9}.
+// za / zb*: the 8 events of the thread ([pair p] = events 8p + 2qd, +1); hi / lo [ks][4]: a0..a3 of k-step ks.
+__device__ __forceinline__ void build_half(const float2 (&za)[4], const float2 (&zb0)[4], const float2 (&zb1)[4], float m0, float m1,
+                                           uint32_t (&hi)[2][4], uint32_t (&lo)[2][4]) {
 #pragma unroll
-    for (int c = 0; c < C::CPP; c++) {
-        float hi[8], lo[8];
-#pragma unroll
-        for (int u = 0; u < 8; u++) feature_split<D>(z, c * 8 + u, mg, hi[u], lo[u]);
-        uint4 h, l;
-        h.x = pack_half2(hi[0], hi[1]); h.y = pack_half2(hi[2], hi[3]); h.z = pack_half2(hi[4], hi[5]); h.w = pack_half2(hi[6], hi[7]);   // exact: <= 2048 quanta
-        l.x = pack_half2(lo[0], lo[1]); l.y = pack_half2(lo[2], lo[3]); l.z = pack_half2(lo[4], lo[5]); l.w = pack_half2(lo[6], lo[7]);
-        *reinterpret_cast<uint4*>(hi_base + c * 512 + eoff) = h;
-        *reinterpret_cast<uint4*>(lo_base + c * 512 + eoff) = l;
+    for (int p = 0; p < 4; p++) {
+        const int ks = p >> 1, u = p & 1;                      // a0 / a1: pair 2ks (rows s = 0, 1); a2 / a3: pair 2ks + 1
+#if GMM_MSTEP_CUT == 2
+        hi[ks][2 * u] = __float_as_uint(zb0[p].x); hi[ks][2 * u + 1] = __float_as_uint(zb1[p].x);
+        lo[ks][2 * u] = __float_as_uint(zb0[p].y); lo[ks][2 * u + 1] = __float_as_uint(zb1[p].y);
+        (void)za; (void)m0; (void)m1;
+#else
+        float h0, l0, h1, l1, h2, l2, h3, l3;
+        feature_split(za[p].x, zb0[p].x, m0, h0, l0);
+        feature_split(za[p].y, zb0[p].y, m0, h1, l1);
+        feature_split(za[p].x, zb1[p].x, m1, h2, l2);
+        feature_split(za[p].y, zb1[p].y, m1, h3, l3);
+        hi[ks][2 * u] = pack_half2(h0, h1);                    // exact: <= 2048 quanta
+        hi[ks][2 * u + 1] = pack_half2(h2, h3);
+        lo[ks][2 * u] = pack_half2(l0, l1);
+        lo[ks][2 * u + 1] = pack_half2(l2, l3);
+#endif
     }
 }
 
-// Packed statistic (index into a cluster's F values, -1 = ignored copy) and the two dimensions (-1 = none) behind
-// operand row `row`; host side of the layout above.
-struct RowInfo { int f, i, j; };
-static RowInfo tc_row_info(int D, int row) {
-    const int S = D / 4, RPP = 1 + 2 * S + S * (D / 2), CPP = (RPP + 7) / 8;
-    const int p = row / (CPP * 8), r = row % (CPP * 8);
-    RowInfo o{-1, -1, -1};
-    if (p >= 4 || r >= RPP) return o;
-    if (r == 0) { if (p == 0) o.f = 0; return o; }
-    if (r <= S) { o.i = (r - 1 + p * S) % D; o.f = 1 + o.i; return o; }
-    int a, b;
-    if (r <= 2 * S) { a = r - 1 - S; b = a; }
-    else { const int t = r - 1 - 2 * S; a = t / (D / 2); b = (a + 1 + t % (D / 2)) % D; }
-    const int ta = (a + p * S) % D, tb = (b + p * S) % D;
-    if (a != b && (b - a + D) % D == D / 2 && ta >= D / 2) return o;       // antipodal pair: the copy with the smaller first index counts
-    o.i = ta > tb ? ta : tb;
-    o.j = ta > tb ? tb : ta;
-    o.f = feat2(D, o.i, o.j);
-    return o;
+// The 8 events of one z-tile row (stage-relative swizzled address: chunk c of row r at c ^ (r & 7), see mstep_rows.h)
+__device__ __forceinline__ void load_row(uint32_t addr, float2 (&z)[4]) {
+#pragma unroll
+    for (int p = 0; p < 4; p++) z[p] = lds_f2(addr ^ (uint32_t)(p << 5));
+}
+
+// The MMAs of one half (both k-steps): ph gh into the exact group, ph gl + pl gs into the remainder group.
+__device__ __forceinline__ void issue_half(float (&ex)[16], float (&rm)[16], const uint32_t (&hi)[2][4], const uint32_t (&lo)[2][4],
+                                           uint32_t gam, bool new1, bool new2) {
+#pragma unroll
+    for (int ks = 0; ks < kTE / 16; ks++) {
+        const uint64_t hdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // gh
+        const uint64_t ldesc = make_smem_desc(gam + kNCL * kTE * 2 + ks * 256, 128, 512);    // gl
+        const uint64_t sdesc = make_smem_desc(gam + 2 * kNCL * kTE * 2 + ks * 256, 128, 512); // gs
+#if GMM_MSTEP_CUT == 1
+        asm volatile("" ::"r"(hi[ks][0]), "r"(hi[ks][1]), "r"(hi[ks][2]), "r"(hi[ks][3]), "r"(lo[ks][0]), "r"(lo[ks][1]), "r"(lo[ks][2]),
+                     "r"(lo[ks][3]), "l"(hdesc), "l"(ldesc), "l"(sdesc));
+        (void)ex; (void)rm; (void)new1; (void)new2;
+#else
+        wgmma_m64n32k16_rs(ex, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], hdesc, ks > 0 || !new1);   // ph gh
+        wgmma_m64n32k16_rs(rm, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], ldesc, ks > 0 || !new2);   // ph gl
+        wgmma_m64n32k16_rs(rm, lo[ks][0], lo[ks][1], lo[ks][2], lo[ks][3], sdesc, true);              // + pl gs
+#endif
+    }
 }
 
 // Feature tile `mt` is drained after sub-tile i when its 128-event chain ends there: the chains of the tiles are
@@ -228,10 +224,11 @@ __device__ __forceinline__ bool chain_starts(int i, int mt) { return i == 0 || (
 __device__ __forceinline__ bool chain2_ends(int i, int mt, int nsub) { return ((i + mt) % kChunkSub2) == kChunkSub2 - 1 || i == nsub - 1; }
 __device__ __forceinline__ bool chain2_starts(int i, int mt) { return i == 0 || ((i + mt) % kChunkSub2) == 0; }
 
+// opmap[row] = a | b << 8: the operand factors of row `row` (mstep_row_layout; codes >= kRowOne: rows of the ones block).
 template <int D>
 __global__ void __launch_bounds__(MCfg<D>::THREADS, 1)
 mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_g, int n,
-                float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic) {
+                float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic, const int* __restrict__ opmap) {
     using C = MCfg<D>;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
@@ -246,14 +243,15 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     const int nsub = (e_end - e_begin + kTE - 1) / kTE;
     const int k0 = blockIdx.y * kNCL;
 
-    // ---- one-time setup ----
-    for (int i = threadIdx.x * 16; i < C::OFF_RAWX; i += C::THREADS * 16) *reinterpret_cast<uint4*>(smem + i) = make_uint4(0, 0, 0, 0);
+    // ---- one-time setup: the ones block of every raw stage, barriers ----
+    for (int i = threadIdx.x; i < kNRAW * 256; i += C::THREADS)
+        reinterpret_cast<float*>(smem + C::OFF_RAWX + (i >> 8) * C::RAWX + C::RAWZ)[i & 255] = 1.0f;
     if (threadIdx.x == 0) {
-        for (int s = 0; s < kNRAW; s++) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 4); }
-        for (int s = 0; s < kNST; s++) { mbar_init(&op_full[s], 4); mbar_init(&op_empty[s], 4 * C::MT); }
+        // raw stage: 3 responsibility-splitting warps and every consumer warp load from it
+        for (int s = 0; s < kNRAW; s++) { mbar_init(&raw_full[s], 1); mbar_init(&raw_empty[s], 3 + 4 * C::MT); }
+        for (int s = 0; s < kNST; s++) { mbar_init(&op_full[s], 3); mbar_init(&op_empty[s], 4 * C::MT); }
         fence_mbar_init();
     }
-    fence_proxy_async_smem();
     __syncthreads();
 
     if (warp < 4) {
@@ -270,125 +268,142 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                     tma_load_2d(smem + C::OFF_RAWG + st * C::RAWG, &tm_g, e0, k0, &raw_full[st]);
                 }
             }
-        }
-    } else if (warp < 12) {
-        set_regs<C::REG_B, C::REG_LAUNCH>();
-        // ===================== operand builders =====================
-        // two builder warpgroups work on alternate sub-tiles (two sub-tiles in flight), the four warps
-        // of a group split the 16-byte feature chunks (c = part mod 4)
-        const int bwg = (warp - 4) >> 2;           // sub-tiles i = bwg (mod 2)
-        const int part = (warp - 4) & 3;
-        const int bt = threadIdx.x - 128 - bwg * 128;   // 0..127 inside the group
-        for (int i = bwg; i < nsub; i += 2) {
-            const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
-            const int os = i % kNST, oph = (i / kNST) & 1;
-            mbar_wait_parked(&raw_full[rs], rph, 200);
-            // --- features of event `lane` ---
-            float z[D];                                // already centred and scaled (tc_set_shift_scale writes the z copy), rotated by part * S
-            {
-                const float* xr = reinterpret_cast<const float*>(smem + C::OFF_RAWX + rs * C::RAWX) + lane;   // [d][32]: conflict-free
-                int dd = part * C::S;
+        } else {
+            // ===================== responsibility operand: warps 1-3 =====================
+            // item (cluster row k, 8-event chunk ce): 128 per sub-tile, thread bt takes bt and (warp 1) bt + 96.
+            // The raw tile is written by TMA with SWIZZLE_128B (16-byte chunk c of row r sits at chunk c ^ (r & 7)), so
+            // 8 lanes reading the same chunk of 8 consecutive rows hit 8 different bank groups; the operand image puts
+            // the 4 K-chunks of an 8-row group next to each other (LBO = 128, SBO = 512), so a warp stores 512
+            // contiguous bytes: no bank conflicts either way.
+            const int bt = threadIdx.x - 32;
+            constexpr int NIT = 2;
+            for (int i = 0; i < nsub; i++) {
+                const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
+                const int os = i % kNST, oph = (i / kNST) & 1;
+                mbar_wait_parked(&raw_full[rs], rph, 200);
+                uint4 gh[NIT], gl[NIT], gs[NIT];
+                float dep = 0.0f;
 #pragma unroll
-                for (int d = 0; d < D; d++) { z[d] = xr[dd * kTE]; dd = dd + 1 == D ? 0 : dd + 1; }
-            }
-            // --- responsibilities: thread -> (cluster row k, 8-event chunk ce), one item per thread.
-            // The raw tile is written by TMA with SWIZZLE_128B (16-byte chunk c of row r sits at chunk
-            // c ^ (r & 7)), so 8 lanes reading the same chunk of 8 consecutive rows hit 8 different
-            // bank groups; the operand image puts the 4 K-chunks of an 8-row group next to each other
-            // (LBO = 128, SBO = 512), so a warp stores 512 contiguous bytes: no bank conflicts either way.
-            uint4 gh, gl, gs;
-            float gdep;
-            {
-                const int kg = bt >> 5, l = bt & 31;
-                const int k = kg * 8 + (l & 7), ce = l >> 3;
-                const uint8_t* grow = smem + C::OFF_RAWG + rs * C::RAWG + k * (kTE * 4);
-                const float4 a = *reinterpret_cast<const float4*>(grow + (((2 * ce) ^ (k & 7)) << 4));
-                const float4 b = *reinterpret_cast<const float4*>(grow + (((2 * ce + 1) ^ (k & 7)) << 4));
-                const float g[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
-                gdep = a.x + b.x;
-                float hi[8], lo[8];
+                for (int u = 0; u < NIT; u++) {
+                    const int it = bt + 96 * u;
+                    if (it >= 128) break;
+                    const int kg = it >> 5, l = it & 31;
+                    const int k = kg * 8 + (l & 7), ce = l >> 3;
+                    const uint8_t* grow = smem + C::OFF_RAWG + rs * C::RAWG + k * (kTE * 4);
+                    const float4 a = *reinterpret_cast<const float4*>(grow + (((2 * ce) ^ (k & 7)) << 4));
+                    const float4 b = *reinterpret_cast<const float4*>(grow + (((2 * ce + 1) ^ (k & 7)) << 4));
+                    const float g[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                    dep += a.x + b.x;
+                    float hi[8], lo[8];
 #pragma unroll
-                for (int u = 0; u < 8; u++) {                  // gh = 16 * round(64 g) (0 .. 1024), gl = 1024 g - gh, both from the exact product
-                    hi[u] = __fsub_rn(__fmaf_rn(g[u], kGammaScale, kGammaMagic), kGammaMagic);
-                    lo[u] = __fmaf_rn(g[u], kGammaScale, -hi[u]);
+                    for (int v = 0; v < 8; v++) {              // gh = 16 * round(64 g) (0 .. 1024), gl = 1024 g - gh, both from the exact product
+                        hi[v] = __fsub_rn(__fmaf_rn(g[v], kGammaScale, kGammaMagic), kGammaMagic);
+                        lo[v] = __fmaf_rn(g[v], kGammaScale, -hi[v]);
+                    }
+                    gh[u] = make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
+                    gl[u] = make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
+                    gs[u] = make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
+                                       pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
                 }
-                gh = make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
-                gl = make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
-                gs = make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
-                                pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
-            }
-            // The raw tiles must BE in registers before the stage goes back to the TMA producer: an mbarrier arrive does
-            // not wait for the warp's outstanding shared-memory loads.  The arrive is therefore made data-dependent on
-            // every load of this thread: a sum over z and one component of the responsibility vector, folded into the
-            // arrive's own operand list below (the asm statement consumes the value, so neither the compiler nor the
-            // hardware can retire it before the loads have landed).
-            float dep = gdep;
-#pragma unroll
-            for (int d = 0; d < D; d++) dep += z[d];
-            __syncwarp();
-            if (lane == 0) mbar_arrive_after(&raw_empty[rs], dep);
-            else asm volatile("" ::"f"(dep));
-            mbar_wait_parked(&op_empty[os], oph ^ 1, 200);
-            uint8_t* phi_hi = smem + C::OFF_PHI + os * C::PHI_STAGE;
-            uint8_t* phi_lo = phi_hi + C::PHI_PART;
-            build_phi_chunks<D>(z, magic, phi_hi, phi_lo, lane, part);
-            {
-                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512); gl = rows 32..63
+                // The raw tile must BE in registers before the stage goes back to the TMA producer: an mbarrier arrive does
+                // not wait for the warp's outstanding shared-memory loads.  The arrive is therefore made data-dependent on
+                // every load of this thread (the asm statement consumes the value, so neither the compiler nor the hardware
+                // can retire it before the loads have landed).
+                __syncwarp();
+                if (lane == 0) mbar_arrive_after(&raw_empty[rs], dep);
+                else asm volatile("" ::"f"(dep));
+                mbar_wait_parked(&op_empty[os], oph ^ 1, 200);
+                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512)
                 uint8_t* g_hi = smem + C::OFF_G + os * C::G_STAGE;
-                const int kg = bt >> 5, l = bt & 31;
-                *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) = gh;
-                *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) = gl;
-                *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) = gs;
+#pragma unroll
+                for (int u = 0; u < NIT; u++) {
+                    const int it = bt + 96 * u;
+                    if (it >= 128) break;
+                    const int kg = it >> 5, l = it & 31;
+                    *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) = gh[u];
+                    *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) = gl[u];
+                    *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) = gs[u];
+                }
+                fence_proxy_async_smem();
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&op_full[os]);
             }
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&op_full[os]);
         }
     } else {
         set_regs<C::REG_C, C::REG_LAUNCH>();
-        // ===================== consumers: wgmma, accumulators in registers =====================
+        // ===================== consumers: operand build and wgmma, accumulators in registers =====================
         // feature tile of this warpgroup (rows 128 mt ..); the shuffle shows ptxas that it is warp-uniform, so the
         // branches on it do not make ptxas serialise the wgmma
-        const int mt = __shfl_sync(0xffffffffu, (warp - 12) >> 2, 0);
-        const int ct = threadIdx.x - 384;                          // consumer thread 0 .. NCT-1
+        const int mt = __shfl_sync(0xffffffffu, (warp - 4) >> 2, 0);
+        const int ct = threadIdx.x - 128;                          // consumer thread 0 .. NCT-1
         const int wq = warp & 3, gid = lane >> 2, qd = lane & 3;
         float* racc = reinterpret_cast<float*>(smem + C::OFF_RACC) + ct;     // [32][NCT]: racc[j * NCT]
 #pragma unroll
         for (int j = 0; j < 32; j++) racc[j * C::NCT] = 0.0f;
+        // this thread's rows: shared factor a, factors b[slot] and rounding constants; stage-relative z-tile addresses of
+        // its 8 events (pair p at addr ^ (p << 5)): row r at r * 128 (ones block rows at RAWZ + rho * 128), chunk
+        // (qd >> 1) ^ (r & 7), byte 8 (qd & 1)
+        uint32_t fa, fb[4];
+        float mg[4];
+        {
+            const int* om = opmap + mt * 128 + wq * 16 + gid;
+            auto addr = [&](int code) {
+                const uint32_t row = code >= kRowOne ? (uint32_t)(C::RAWZ / 128 + code - kRowOne) : (uint32_t)code;
+                return row * 128 + ((((uint32_t)qd >> 1) ^ (row & 7)) << 4) + ((uint32_t)qd & 1) * 8;
+            };
+#pragma unroll
+            for (int s = 0; s < 4; s++) {
+                const int c = om[(s >> 1) * 64 + (s & 1) * 8];
+                const int a = c & 255, b = c >> 8;
+                if (s == 0) fa = addr(a);
+                fb[s] = addr(b);
+                mg[s] = a >= kRowOne && b >= kRowOne ? 0.0f : (a >= kRowOne || b >= kRowOne ? magic.lin : magic.prod);
+            }
+        }
+        const uint32_t zs0 = smem_u32(smem + C::OFF_RAWX);
         float ex[2][16], rm[2][16];                                // per 64-row half: exact group, remainder group
 #pragma unroll
         for (int h = 0; h < 2; h++)
 #pragma unroll
             for (int j = 0; j < 16; j++) { ex[h][j] = 0.0f; rm[h][j] = 0.0f; }
-        int held = -1;                                             // stage of the previous sub-tile while its MMAs may run
+        uint32_t fh[2][2][4], fl[2][2][4];                          // A fragments per half (one set in flight, one built)
+        int held = -1;                                             // responsibility stage of the previous sub-tile while its MMAs may run
+        // Software pipeline per half: the group of half 0 of sub-tile i is issued while half 1 of sub-tile i - 1 runs,
+        // half 1 of sub-tile i while half 0 runs; a half's fragments are rebuilt only after its previous group retired.
         for (int i = 0; i < nsub; i++) {
+            const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
             const int os = i % kNST, oph = (i / kNST) & 1;
-            mbar_wait_parked(&op_full[os], oph, 100);
-            const uint32_t phi = smem_u32(smem + C::OFF_PHI + os * C::PHI_STAGE);
+            const uint32_t zst = zs0 + rs * C::RAWX;
             const uint32_t gam = smem_u32(smem + C::OFF_G + os * C::G_STAGE);
             // a chain starts with its first MMA overwriting the accumulators (the drain leaves them as they are)
             const bool new1 = chain_starts(i, mt), new2 = chain2_starts(i, mt);
+            mbar_wait_parked(&raw_full[rs], rph, 100);
+            float2 za[4], zb0[4], zb1[4];
+            load_row(zst + fa, za);
+            load_row(zst + fb[0], zb0);
+            load_row(zst + fb[1], zb1);
+            build_half(za, zb0, zb1, mg[0], mg[1], fh[0], fl[0]);
+            mbar_wait_parked(&op_full[os], oph, 100);
             wgmma_fence();
-#pragma unroll
-            for (int h = 0; h < 2; h++) {
-#pragma unroll
-                for (int ks = 0; ks < kTE / 16; ks++) {
-                    const uint64_t hdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // gh
-                    const uint64_t ldesc = make_smem_desc(gam + C::G_PART + ks * 256, 128, 512);         // gl
-                    const uint64_t sdesc = make_smem_desc(gam + 2 * C::G_PART + ks * 256, 128, 512);     // gs
-                    const uint32_t arow = mt * 8192 + h * 4096 + ks * 256;
-                    const uint64_t ah = make_smem_desc(phi + arow, /*LBO*/ 128, /*SBO*/ 512);
-                    const uint64_t al = make_smem_desc(phi + C::PHI_PART + arow, 128, 512);
-                    wgmma_m64n32k16_ss_tn(ex[h], ah, hdesc, ks > 0 || !new1);     // ph gh
-                    wgmma_m64n32k16_ss_tn(rm[h], ah, ldesc, ks > 0 || !new2);     // ph gl
-                    wgmma_m64n32k16_ss_tn(rm[h], al, sdesc);                      // + pl gs
-                }
-            }
+            issue_half(ex[0], rm[0], fh[0], fl[0], gam, new1, new2);
             wgmma_commit();
-            // the previous sub-tile's MMAs have read their stage once at most this sub-tile's group is in flight
+            // half 1 of the previous sub-tile has retired: its responsibility stage is free, and so are the fragments of half 1
             wgmma_wait<1>();
             __syncwarp();
             if (lane == 0 && held >= 0) mbar_arrive(&op_empty[held]);
+            load_row(zst + fb[2], zb0);
+            load_row(zst + fb[3], zb1);
+            build_half(za, zb0, zb1, mg[2], mg[3], fh[1], fl[1]);
+            wgmma_fence();
+            issue_half(ex[1], rm[1], fh[1], fl[1], gam, new1, new2);
+            wgmma_commit();
+            // The raw stage goes back to the TMA producer only after this warp's loads from it have landed (an mbarrier
+            // arrive alone does not wait for them, see the responsibility warps).  The wgmma just issued reads the A
+            // fragments of half 1 and the one before those of half 0, which are computed from every z this thread loaded:
+            // the warpgroup-wide wgmma cannot issue before all of them are in registers, and the arrive follows it.
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&raw_empty[rs]);
+            wgmma_wait<1>();                                       // half 0 of this sub-tile has retired
             held = os;
             // drain: exact group at the end of its 128-event chain, remainder group at the end of its longer chain
             // (the second ends only where the first does)
@@ -397,6 +412,7 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&op_empty[os]);
                 held = -1;
+#if GMM_MSTEP_CUT != 3
                 // one half at a time (the empty asm keeps ptxas from hoisting all 32 loads): with every accumulator
                 // live, 32 loads in flight would not fit the consumers' registers at D = 24
 #pragma unroll
@@ -413,9 +429,16 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                         asm volatile("" ::: "memory");
                     }
                 }
+#endif
             }
         }
         wgmma_wait<0>();            // (the last sub-tile drained: nothing in flight; without it ptxas waits in every iteration)
+#if GMM_MSTEP_CUT == 3
+#pragma unroll
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+            for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += ex[h][j] + rm[h][j];
+#endif
         // one plain store of this thread's partial sums: [cta][tile][row][32 clusters]
         float* my = scratch + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * C::MT * 128 * kNCL + (size_t)mt * 128 * kNCL;
 #pragma unroll
@@ -988,6 +1011,7 @@ struct TcState {
     float zmax[GMM_MAX_DIMENSIONS] = {0};    // power-of-two bound of |z_d| over the whole data set
     MMagic magic{0.f, 0.f};          // rounding constants of the coordinate / product rows
     int3* d_rowmap = nullptr;        // [MT * 128] operand row -> (packed statistic, dimension i, dimension j)
+    int* d_opmap = nullptr;          // [MT * 128] operand row -> its factors a | b << 8 (mstep_row_layout)
     CUtensorMap tm_cx{}, tm_cg{};    // tc_launch_mstep_on: maps over the caller's chunk buffers, for cmap_n events
     const void* cmap_z = nullptr;
     const void* cmap_g = nullptr;
@@ -1064,10 +1088,10 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
     TC_CUDA_TRY(cudaMalloc(&t->d_shift_f, sizeof(float) * GMM_MAX_DIMENSIONS));
     TC_CUDA_TRY(cudaMalloc(&t->d_inv_scale_f, sizeof(float) * GMM_MAX_DIMENSIONS));
     TC_CUDA_TRY(cudaMalloc(&t->d_scale, sizeof(double) * GMM_MAX_DIMENSIONS));
-    // tensor maps: SoA events [D][pitch] viewed as (events, dims) -> smem tile [D][32 events];
+    // tensor maps: SoA events [D][pitch] viewed as (events, dims) -> smem tile [D][32 events] (SWIZZLE_128B);
     // responsibilities [Kmax][pitch] viewed as (events, clusters)
     TC_CUDA_TRY(cudaMalloc(&t->d_z_soa, sizeof(float) * memb_pitch * D));
-    if (int rc = make_map_2d(&t->tm_x, t->d_z_soa, (uint64_t)n, (uint64_t)D, (uint64_t)memb_pitch * 4, kTE, (uint32_t)D)) return rc;
+    if (int rc = make_map_2d(&t->tm_x, t->d_z_soa, (uint64_t)n, (uint64_t)D, (uint64_t)memb_pitch * 4, kTE, (uint32_t)D, /*swizzle128=*/true)) return rc;
     if (int rc = make_map_2d(&t->tm_g, d_memb, (uint64_t)n, (uint64_t)Kmax, (uint64_t)memb_pitch * 4, kTE, kNCL, /*swizzle128=*/true)) return rc;
     t->maps_ok = true;
     if (D == 8 || D == 16 || D == 24) {
@@ -1086,22 +1110,28 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
         if (passes > 1) TC_CUDA_TRY(cudaMalloc(&t->d_den, sizeof(float) * memb_pitch));
         t->emap_ok = true;
     }
-    const int rpp = 1 + 2 * (D / 4) + (D / 4) * (D / 2), nrows = 4 * ((rpp + 7) / 8) * 8;
-    const int mt = (nrows + 127) / 128;
+    const int mt = mstep_tiles(D);
     {
-        std::vector<int3> rm((size_t)mt * 128);
+        // operand row -> (packed statistic, dimension i, dimension j) for the finalisation, and its two factors for the kernel
+        const std::vector<MRow> rows = mstep_row_layout(D);
+        if (rows.size() != (size_t)mt * 128) return fail(GMM_ERR_STATE, "tensor M-step row map: the statistics do not fit the feature tiles");
+        std::vector<int3> rm(rows.size());
+        std::vector<int> om(rows.size());
         std::vector<char> seen((size_t)num_features(D), 0);
-        for (int row = 0; row < mt * 128; row++) {
-            const RowInfo ri = tc_row_info(D, row);
-            rm[row] = make_int3(ri.f, ri.i, ri.j);
-            if (ri.f >= 0) {
-                if (seen[ri.f]) return fail(GMM_ERR_STATE, "tensor M-step row map: a statistic is produced twice");
-                seen[ri.f] = 1;
+        for (size_t row = 0; row < rows.size(); row++) {
+            const MRow& r = rows[row];
+            rm[row] = make_int3(r.f, r.i, r.j);
+            om[row] = r.a | r.b << 8;
+            if (r.f >= 0) {
+                if (seen[r.f]) return fail(GMM_ERR_STATE, "tensor M-step row map: a statistic is produced twice");
+                seen[r.f] = 1;
             }
         }
         for (char c : seen) if (!c) return fail(GMM_ERR_STATE, "tensor M-step row map: a statistic is not produced");
         TC_CUDA_TRY(cudaMalloc(&t->d_rowmap, sizeof(int3) * rm.size()));
         TC_CUDA_TRY(cudaMemcpy(t->d_rowmap, rm.data(), sizeof(int3) * rm.size(), cudaMemcpyHostToDevice));
+        TC_CUDA_TRY(cudaMalloc(&t->d_opmap, sizeof(int) * om.size()));
+        TC_CUDA_TRY(cudaMemcpy(t->d_opmap, om.data(), sizeof(int) * om.size(), cudaMemcpyHostToDevice));
     }
     const int ytiles = (Kmax + kNCL - 1) / kNCL;
     t->scratch_floats = (size_t)num_sms * ytiles * mt * 128 * kNCL;
@@ -1121,7 +1151,7 @@ bool tc_estep_range_ok(const TcState* t) {
 void tc_destroy(TcState* t) {
     if (!t) return;
     cudaFree(t->d_shift_f); cudaFree(t->d_inv_scale_f); cudaFree(t->d_scale); cudaFree(t->d_scratch);
-    cudaFree(t->d_opnd); cudaFree(t->d_den); cudaFree(t->d_z_soa); cudaFree(t->d_rowmap);
+    cudaFree(t->d_opnd); cudaFree(t->d_den); cudaFree(t->d_z_soa); cudaFree(t->d_rowmap); cudaFree(t->d_opmap);
     if (t->h_opnd) cudaFreeHost(t->h_opnd);
     if (t->ev_h2d) cudaEventDestroy(t->ev_h2d);
     delete t;
@@ -1747,9 +1777,9 @@ static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUte
     const int gy = (K + kNCL - 1) / kNCL;
     if ((size_t)gx * gy * C::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
     dim3 grid(gx, gy);
-    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tm_x, tm_g, n, t->d_scratch, per, t->magic);
+    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tm_x, tm_g, n, t->d_scratch, per, t->magic, t->d_opmap);
     TC_CUDA_TRY(cudaGetLastError());
-    mstep_tc_finalize_kernel<<<C::NCHUNK * 8, 256, 0, stream>>>(t->d_scratch, gx, C::MT, K, C::F, t->d_rowmap, t->d_scale, d_stats);
+    mstep_tc_finalize_kernel<<<C::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C::MT, K, C::F, t->d_rowmap, t->d_scale, d_stats);
     TC_CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
@@ -1779,7 +1809,7 @@ int tc_launch_mstep_on(TcState* t, int K, const float* d_z, const float* d_memb,
     if (!t || !t->maps_ok) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
     if (t->cmap_z != d_z || t->cmap_g != d_memb || t->cmap_pitch != pitch || t->cmap_n != n) {
         t->cmap_n = -1;
-        if (int rc = make_map_2d(&t->tm_cx, d_z, (uint64_t)n, (uint64_t)t->D, (uint64_t)pitch * 4, kTE, (uint32_t)t->D)) return rc;
+        if (int rc = make_map_2d(&t->tm_cx, d_z, (uint64_t)n, (uint64_t)t->D, (uint64_t)pitch * 4, kTE, (uint32_t)t->D, /*swizzle128=*/true)) return rc;
         if (int rc = make_map_2d(&t->tm_cg, d_memb, (uint64_t)n, (uint64_t)t->Kmax, (uint64_t)pitch * 4, kTE, kNCL, /*swizzle128=*/true)) return rc;
         t->cmap_z = d_z; t->cmap_g = d_memb; t->cmap_pitch = pitch; t->cmap_n = n;
     }

@@ -127,6 +127,19 @@ __device__ __forceinline__ void wgmma_m64n64k16_rs(float (&d)[32], uint32_t a0, 
         : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"((uint32_t)accumulate));
 }
 
+// D[64 x 32] (+)= A[64 x 16] (registers, K-major fragments) * B[16 x 32] (shared memory, K-major); one warpgroup.
+// accumulate = false overwrites D (scale-d = 0).
+__device__ __forceinline__ void wgmma_m64n32k16_rs(float (&d)[16], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint64_t b_desc, bool accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %21, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+        "{%16, %17, %18, %19}, %20, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "l"(b_desc), "r"((uint32_t)accumulate));
+}
+
 // D[64 x 32] (+)= A[64 x 16] * B[16 x 32], both from shared memory: A MN-major (transposed), B K-major; one warpgroup.
 // accumulate = false overwrites D (scale-d = 0): a new accumulation chain starts without writing the registers first.
 __device__ __forceinline__ void wgmma_m64n32k16_ss_tn(float (&d)[16], uint64_t a_desc, uint64_t b_desc, bool accumulate = true) {
