@@ -310,14 +310,24 @@ struct ScoreBuffers {
     }
 };
 
+// Time and kernel counts of the calls that stream E- and M-steps over chunks (gmm_get_score_stats_profile,
+// gmm_get_condition_stats_profile).
+struct StatsProfile {
+    double kernel_ms = 0, wall_ms = 0, wait_ms = 0;
+    long long e_tensor = 0, e_simt = 0, m_tensor = 0, m_simt = 0;
+};
+
 // gmm_score_stats' own buffers (its input stage is gmm_score's two pinned slots and device chunks): ONE compute-side chunk
 // (the kernels of consecutive chunks are serialised on the compute stream), the statistics it adds up, the range flag and,
-// on the first call that asks for memberships, their pinned mirror.
+// on the first call that asks for memberships, their pinned mirror.  gmm_condition_stats uses the same buffers, plus its
+// observed copy (allocated on its first call) and the float centre.
 struct ScoreStatsBuffers {
     long long cap = 0;                          // events per chunk
     size_t pitch = 0;                           // row pitch in floats of the SoA copies and the responsibilities (multiple of 32)
     float* d_z = nullptr;                       // [D][pitch] standardised SoA copy (tensor M-step)
     float* d_xs = nullptr;                      // [D][pitch] raw SoA copy (SIMT kernels)
+    float* d_xo = nullptr;                      // [D][pitch] observed SoA copy of gmm_condition_stats (its n_obs rows)
+    float* d_shift_f = nullptr;                 // [GMM_MAX_DIMENSIONS] the centre in float (gmm_condition_stats' missing rows)
     float* d_memb = nullptr;                    // [8 ceil(Kmax / 8)][pitch] responsibilities of the chunk
     float* h_memb = nullptr;                    // pinned [Kmax][cap]
     double* d_stats = nullptr;                  // [Kmax F + 1]
@@ -326,17 +336,18 @@ struct ScoreStatsBuffers {
     int* h_flag = nullptr;                      // pinned
     cudaEvent_t ev_flag = nullptr;
     cudaEvent_t p0[2] = {nullptr, nullptr}, p1[2] = {nullptr, nullptr}, k0[2] = {nullptr, nullptr}, k1[2] = {nullptr, nullptr};
-    double kernel_ms = 0, wall_ms = 0, wait_ms = 0;   // gmm_get_score_stats_profile
-    long long e_tensor = 0, e_simt = 0, m_tensor = 0, m_simt = 0;
+    StatsProfile prof;                          // gmm_get_score_stats_profile
+    StatsProfile cond_prof;                     // gmm_get_condition_stats_profile
     void release_chunk() {
-        cudaFree(d_z); cudaFree(d_xs); cudaFree(d_memb);
+        cudaFree(d_z); cudaFree(d_xs); cudaFree(d_xo); cudaFree(d_memb);
         if (h_memb) cudaFreeHost(h_memb);
-        d_z = d_xs = d_memb = h_memb = nullptr;
+        d_z = d_xs = d_xo = d_memb = h_memb = nullptr;
         cap = 0; pitch = 0;
     }
     void destroy() {
         release_chunk();
-        cudaFree(d_stats); cudaFree(d_flag);
+        cudaFree(d_stats); cudaFree(d_flag); cudaFree(d_shift_f);
+        d_shift_f = nullptr;
         if (h_stats) cudaFreeHost(h_stats);
         if (h_flag) cudaFreeHost(h_flag);
         d_stats = h_stats = nullptr; d_flag = h_flag = nullptr;
@@ -633,16 +644,19 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
 }
 
 // ---- kernel dispatch -------------------------------------------------------
-// SIMT E-step over n events of the SoA copy xs [D][pitch] into memb [K][pitch] (the shard's, or a gmm_score_stats chunk's)
+// SIMT E-step over n events of the SoA copy xs [D][pitch] into memb [K][pitch] against the epack records `epack` (the
+// shard's or a gmm_score_stats chunk's with the context's D and d_epack; a gmm_condition_stats chunk's with the observed
+// dimensions and its marginal block)
 template <int D>
-static void launch_estep_simt_d(gmm_ctx* c, int K, const float* xs, int n, float* memb, size_t pitch, double* ll) {
+static void launch_estep_simt_d(gmm_ctx* c, int K, const float* epack, const float* xs, int n, float* memb, size_t pitch, double* ll) {
     const int blocks = (n + kEstepThreads - 1) / kEstepThreads;
-    estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, c->d_epack, memb, pitch, ll);
+    estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, epack, memb, pitch, ll);
 }
-static int launch_estep_simt_on(gmm_ctx* c, int K, const float* xs, int n, float* memb, size_t pitch, double* ll) {
+static int launch_estep_simt_on(gmm_ctx* c, int D, int K, const float* epack, const float* xs, int n, float* memb, size_t pitch,
+                                double* ll) {
     if (n == 0) return GMM_OK;
-    switch (c->D) {
-#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K, xs, n, memb, pitch, ll); break;
+    switch (D) {
+#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K, epack, xs, n, memb, pitch, ll); break;
         GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
         GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
         GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
@@ -654,7 +668,7 @@ static int launch_estep_simt_on(gmm_ctx* c, int K, const float* xs, int n, float
     return GMM_OK;
 }
 static int launch_estep_simt(gmm_ctx* c, int K) {
-    return launch_estep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F);
+    return launch_estep_simt_on(c, c->D, K, c->d_epack, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F);
 }
 
 // SIMT scoring of io.n rows of D coordinates against the epack records `epack` (gmm_score: the context's D and d_epack;
@@ -1646,7 +1660,7 @@ int gmm_get_score_profile(gmm_ctx* c, double out[4], int reset) {
 }
 
 // ---- E-step + M-step statistics of new events ---------------------------------------------------------------------------
-static int score_stats_buffers(gmm_ctx* c, bool with_memberships) {
+static int score_stats_buffers(gmm_ctx* c, bool with_memberships, bool with_observed = false) {
     ScoreStatsBuffers& t = c->sstats;
     if (!t.ev_flag) {
         CUDA_TRY(cudaEventCreateWithFlags(&t.ev_flag, cudaEventDisableTiming));
@@ -1656,6 +1670,7 @@ static int score_stats_buffers(gmm_ctx* c, bool with_memberships) {
         CUDA_TRY(cudaMallocHost(&t.h_stats, sizeof(double) * ((size_t)c->Kmax * c->F + 1)));
         CUDA_TRY(cudaMalloc(&t.d_flag, sizeof(int)));
         CUDA_TRY(cudaMallocHost(&t.h_flag, sizeof(int)));
+        CUDA_TRY(cudaMalloc(&t.d_shift_f, sizeof(float) * GMM_MAX_DIMENSIONS));
     }
     const long long want = c->score_chunk;
     if (t.cap < want) {
@@ -1671,13 +1686,14 @@ static int score_stats_buffers(gmm_ctx* c, bool with_memberships) {
         t.pitch = pitch;
     }
     if (with_memberships && !t.h_memb) CUDA_TRY(cudaMallocHost(&t.h_memb, sizeof(float) * (size_t)c->Kmax * t.cap));
+    if (with_observed && !t.d_xo) CUDA_TRY(cudaMalloc(&t.d_xo, sizeof(float) * t.pitch * c->D));
     return GMM_OK;
 }
 
 // Per chunk i (slot b = i & 1 of gmm_score's input stage), in order on the compute stream: prep kernel (SoA copies + range
 // flag) -> flag to the host, while chunk i + 1 is staged and its H2D issued -> the kernels the flag allows -> E-step into the
 // chunk's responsibilities -> M-step adding into the call's statistics -> (memberships) pitched D2H and rows to the caller.
-static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bool with_stats, float* memberships) {
+static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bool with_stats, float* memberships, StatsProfile& pr) {
     ScoreBuffers& s = c->score;
     ScoreStatsBuffers& t = c->sstats;
     const int D = c->D;
@@ -1704,8 +1720,8 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
     auto collect = [&](int b) {                                   // timings of a chunk whose kernels have finished
         float a = 0, k = 0, w = 0;
         if (cudaEventElapsedTime(&a, t.p0[b], t.p1[b]) == cudaSuccess && cudaEventElapsedTime(&k, t.k0[b], t.k1[b]) == cudaSuccess)
-            t.kernel_ms += (double)a + (double)k;
-        if (cudaEventElapsedTime(&w, t.p1[b], t.k0[b]) == cudaSuccess) t.wait_ms += w;
+            pr.kernel_ms += (double)a + (double)k;
+        if (cudaEventElapsedTime(&w, t.p1[b], t.k0[b]) == cudaSuccess) pr.wait_ms += w;
     };
     if (nchunks > 0)
         if (int rc = stage(0)) return rc;
@@ -1747,15 +1763,15 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
             CUDA_TRY(cudaGetLastError());
         }
         int rc = ce ? tc_launch_estep_on(c->tc, K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
-                    : launch_estep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
+                    : launch_estep_simt_on(c, D, K, c->d_epack, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
         if (rc) return rc;
-        (ce ? t.e_tensor : t.e_simt)++;
+        (ce ? pr.e_tensor : pr.e_simt)++;
         CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
         if (with_stats) {
             rc = cm ? tc_launch_mstep_on(c->tc, K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
                     : launch_mstep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats);
             if (rc) return rc;
-            (cm ? t.m_tensor : t.m_simt)++;
+            (cm ? pr.m_tensor : pr.m_simt)++;
         }
         CUDA_TRY(cudaEventRecord(t.k1[b], c->stream));
         if (memberships) {
@@ -1792,7 +1808,7 @@ int gmm_score_stats(gmm_ctx* c, int K, const float* events_aos, long long n, dou
     if (n > 0) {
         rc = score_buffers(c);
         if (rc == GMM_OK) rc = score_stats_buffers(c, memberships != nullptr);
-        if (rc == GMM_OK) rc = score_stats_batch(c, K, events_aos, n, stats_out != nullptr, memberships);
+        if (rc == GMM_OK) rc = score_stats_batch(c, K, events_aos, n, stats_out != nullptr, memberships, c->sstats.prof);
         // nothing of this call may still be in flight when it returns (also after a failure)
         const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
         if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
@@ -1805,17 +1821,17 @@ int gmm_score_stats(gmm_ctx* c, int K, const float* events_aos, long long n, dou
         }
         if (shift_out) std::memcpy(shift_out, c->shift, sizeof(double) * (size_t)c->D);
     }
-    c->sstats.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    c->sstats.prof.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return rc;
 }
 
 int gmm_get_score_stats_profile(gmm_ctx* c, double out[7], int reset) {
     if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_score_stats_profile: bad argument");
-    ScoreStatsBuffers& t = c->sstats;
+    StatsProfile& t = c->sstats.prof;
     out[0] = t.kernel_ms; out[1] = t.wall_ms;
     out[2] = (double)t.e_tensor; out[3] = (double)t.e_simt; out[4] = (double)t.m_tensor; out[5] = (double)t.m_simt;
     out[6] = t.wait_ms;
-    if (reset) { t.kernel_ms = t.wall_ms = t.wait_ms = 0; t.e_tensor = t.e_simt = t.m_tensor = t.m_simt = 0; }
+    if (reset) t = StatsProfile();
     return GMM_OK;
 }
 
@@ -2241,8 +2257,10 @@ static size_t condition_block_floats(int Kmax, int D) {
 
 // The parameter block of the current K clusters in the pinned mirror (gmm.h): the marginal set (mu_O, P_O, constant_O,
 // pi) goes through build_epack, at n_obs dimensions for score_simt_kernel, or zero-padded to a multiple of 4 and followed
-// by mu_M, G and c for condition_simt_kernel.  With nm = 0 the marginal set is the context's own arrays.
-static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const int* mis, int nm, bool impute) {
+// by mu_M, G and c for condition_simt_kernel.  With nm = 0 the marginal set is the context's own arrays.  g_d [K][nm][n_obs]
+// and c_d [K][nm][nm], when not NULL, receive G and S_MM^-1 in double (gmm_condition_stats); `who` names the caller in errors.
+static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const int* mis, int nm, bool impute,
+                            const char* who = "gmm_condition", double* g_d = nullptr, double* c_d = nullptr) {
     const int D = c->D;
     float* block = c->cond.h_block;
     if (nm == 0) {
@@ -2254,7 +2272,8 @@ static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const 
     std::atomic<int> first_bad{K};
     const std::function<void(int)> per_cluster = [&](int k) {
         std::vector<float> p((size_t)n_obs * n_obs);
-        if (!condition_cluster(&c->host, k, D, obs, n_obs, mis, nm, p.data(), &co[k], &g[(size_t)k * nm * n_obs], &cv[(size_t)k * nm])) {
+        if (!condition_cluster(&c->host, k, D, obs, n_obs, mis, nm, p.data(), &co[k], &g[(size_t)k * nm * n_obs], &cv[(size_t)k * nm],
+                               g_d ? g_d + (size_t)k * nm * n_obs : nullptr, c_d ? c_d + (size_t)k * nm * nm : nullptr)) {
             int cur = first_bad.load();
             while (k < cur && !first_bad.compare_exchange_weak(cur, k)) {}
             return;
@@ -2272,7 +2291,7 @@ static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const 
         for (int k = 0; k < K; k++) per_cluster(k);
     }
     if (first_bad.load() < K)
-        return fail(GMM_ERR_STATE, "gmm_condition: the block P_MM of cluster " + std::to_string(first_bad.load()) +
+        return fail(GMM_ERR_STATE, std::string(who) + ": the block P_MM of cluster " + std::to_string(first_bad.load()) +
                                        " (inverse covariance on the missing dimensions) is not positive definite");
     clusters_t marg{};
     marg.means = mo.data(); marg.Rinv = po.data(); marg.constant = co.data(); marg.pi = c->host.pi;
@@ -2445,6 +2464,185 @@ int gmm_get_condition_profile(gmm_ctx* c, double out[2], int reset) {
     if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_condition_profile: bad argument");
     out[0] = c->cond.kernel_ms; out[1] = c->cond.wall_ms;
     if (reset) c->cond.kernel_ms = c->cond.wall_ms = 0;
+    return GMM_OK;
+}
+
+// ---- M-step statistics of events measured on a subset of the dimensions ----------------------------------------------------
+// Per chunk i (slot b = i & 1 of gmm_score's input stage), in order on the compute stream: prep kernel (observed SoA copy, the
+// D-row image of the M-step that will run, range flag) -> flag to the host, while chunk i + 1 is staged and its H2D issued ->
+// marginal SIMT E-step of the observed copy into the chunk's responsibilities -> the context's M-step on the D-row image,
+// adding into the call's statistics -> (memberships) pitched D2H and rows to the caller.  The statistics hold T0, T1 and T2 in
+// the entries of the observed dimensions; the caller expands the others on the host (condition_stats_cluster).
+static int condition_stats_batch(gmm_ctx* c, int K, int n_obs, unsigned obs_mask, const float* ev, long long n, bool with_stats,
+                                 float* memberships) {
+    ScoreBuffers& s = c->score;
+    ScoreStatsBuffers& t = c->sstats;
+    StatsProfile& pr = t.cond_prof;
+    const int D = c->D;
+    const size_t KF = (size_t)K * c->F;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
+    const bool m_tensor = with_stats && use_tensor_mstep(c, K);
+    const float* inv_scale_f = m_tensor ? tc_inv_scale_f(c->tc) : nullptr;
+    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
+    if (m_tensor && !inv_scale_f) return fail(GMM_ERR_STATE, "gmm_condition_stats: the tensor M-step has no centre");
+    float shift_f[GMM_MAX_DIMENSIONS] = {0};               // the float centre the M-steps use (c->shift is rounded to it
+    for (int d = 0; d < D; d++) shift_f[d] = (float)c->shift[d];   // whenever the wgmma M-step can run)
+    CUDA_TRY(cudaMemcpyAsync(t.d_shift_f, shift_f, sizeof(shift_f), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(c->cond.d_block, c->cond.h_block, sizeof(float) * (size_t)K * epack_stride(n_obs), cudaMemcpyHostToDevice,
+                             c->stream));
+    CUDA_TRY(cudaMemsetAsync(t.d_stats, 0, sizeof(double) * (KF + 1), c->stream));
+    auto rows_of = [&](long long i) { return (int)std::min(chunk, n - i * chunk); };
+    auto stage = [&](long long i) -> int {
+        const int b = (int)(i & 1), m = rows_of(i);
+        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
+        std::memcpy(s.h_in[b], ev + (size_t)(i * chunk) * n_obs, sizeof(float) * (size_t)m * n_obs);
+        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the device chunk's previous readers are done with it
+        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * n_obs, cudaMemcpyHostToDevice, s.copy));
+        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
+        return GMM_OK;
+    };
+    auto prep = [&](int b, int m, float* xo, float* z, float* x) -> int {
+        condition_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], m, n_obs, D, obs_mask, t.d_shift_f, inv_scale_f,
+                                                                                   zb, xo, z, x, t.pitch, t.d_flag);
+        CUDA_TRY(cudaGetLastError());
+        return GMM_OK;
+    };
+    auto collect = [&](int b) {                                   // timings of a chunk whose kernels have finished
+        float a = 0, k = 0, w = 0;
+        if (cudaEventElapsedTime(&a, t.p0[b], t.p1[b]) == cudaSuccess && cudaEventElapsedTime(&k, t.k0[b], t.k1[b]) == cudaSuccess)
+            pr.kernel_ms += (double)a + (double)k;
+        if (cudaEventElapsedTime(&w, t.p1[b], t.k0[b]) == cudaSuccess) pr.wait_ms += w;
+    };
+    if (nchunks > 0)
+        if (int rc = stage(0)) return rc;
+    for (long long i = 0; i < nchunks; i++) {
+        const int b = (int)(i & 1), m = rows_of(i);
+        const long long e0 = i * chunk;
+        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
+        CUDA_TRY(cudaMemsetAsync(t.d_flag, 0, sizeof(int), c->stream));
+        CUDA_TRY(cudaEventRecord(t.p0[b], c->stream));
+        if (int rc = prep(b, m, t.d_xo, m_tensor ? t.d_z : nullptr, with_stats && !m_tensor ? t.d_xs : nullptr)) return rc;
+        CUDA_TRY(cudaEventRecord(t.p1[b], c->stream));
+        CUDA_TRY(cudaMemcpyAsync(t.h_flag, t.d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaEventRecord(t.ev_flag, c->stream));
+        if (i + 1 < nchunks)
+            if (int rc = stage(i + 1)) return rc;
+        CUDA_TRY(cudaEventSynchronize(t.ev_flag));
+        if (i > 0) collect(b ^ 1);                                // (the prep of chunk i ran after chunk i - 1's kernels)
+        const int flag = *t.h_flag;
+        if (flag & kScoreStatsNotFinite) return fail(GMM_ERR_ARG, "gmm_condition_stats: an event has a coordinate that is not finite");
+        const bool cm = m_tensor && !(flag & kScoreStatsBeyondZb);
+        if (m_tensor && !cm && mstep_path_of(c) == GMM_PATH_TENSOR)
+            return fail(GMM_ERR_STATE, "gmm_condition_stats: an event lies beyond the tensor M-step's fixed-point range (|z| >= the "
+                                       "training data's bound) and mstep_path is GMM_PATH_TENSOR");
+        CUDA_TRY(cudaEventRecord(t.k0[b], c->stream));
+        if (m_tensor && !cm)                                      // a fallback of this chunk only: its raw image now
+            if (int rc = prep(b, m, nullptr, nullptr, t.d_xs)) return rc;
+        int rc = launch_estep_simt_on(c, n_obs, K, c->cond.d_block, t.d_xo, m, t.d_memb, t.pitch, t.d_stats + KF);
+        if (rc) return rc;
+        pr.e_simt++;
+        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
+        if (with_stats) {
+            rc = cm ? tc_launch_mstep_on(c->tc, K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
+                    : launch_mstep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats);
+            if (rc) return rc;
+            (cm ? pr.m_tensor : pr.m_simt)++;
+        }
+        CUDA_TRY(cudaEventRecord(t.k1[b], c->stream));
+        if (memberships) {
+            CUDA_TRY(cudaMemcpy2DAsync(t.h_memb, sizeof(float) * (size_t)m, t.d_memb, sizeof(float) * t.pitch, sizeof(float) * (size_t)m, K,
+                                       cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(cudaStreamSynchronize(c->stream));
+            for (int k = 0; k < K; k++)
+                std::memcpy(memberships + (size_t)k * n + e0, t.h_memb + (size_t)k * m, sizeof(float) * (size_t)m);
+        }
+    }
+    if (with_stats) CUDA_TRY(cudaMemcpyAsync(t.h_stats, t.d_stats, sizeof(double) * (KF + 1), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    if (nchunks > 0) collect((int)((nchunks - 1) & 1));
+    return GMM_OK;
+}
+
+int gmm_condition_stats(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n, double* stats_out,
+                        double* shift_out, float* memberships) {
+    if (int rc = check_K(c, K, "gmm_condition_stats")) return rc;
+    if (n < 0 || (n > 0 && !events_obs)) return fail(GMM_ERR_ARG, "gmm_condition_stats: bad events (n < 0, or no rows)");
+    if (!obs_dims || n_obs < 1 || n_obs > c->D)
+        return fail(GMM_ERR_ARG, "gmm_condition_stats: obs_dims must hold between 1 and D dimension indices");
+    for (int i = 0; i < n_obs; i++)
+        if (obs_dims[i] < 0 || obs_dims[i] >= c->D || (i > 0 && obs_dims[i] <= obs_dims[i - 1]))
+            return fail(GMM_ERR_ARG, "gmm_condition_stats: obs_dims must be strictly increasing indices in [0, D)");
+    if (!stats_out && !memberships) return fail(GMM_ERR_ARG, "gmm_condition_stats: neither statistics nor memberships requested");
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_condition_stats: parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, "gmm_condition_stats: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    if (!c->have_shift) {
+        // the centre comes from the global column moments, an all-reduce over the ranks: never issued from here
+        if (c->nranks > 1)
+            return fail(GMM_ERR_STATE, "gmm_condition_stats: the context's centre is not fixed yet (run gmm_mstep or gmm_em first on every rank)");
+        if (int rc = ensure_moments(c)) return rc;
+    }
+    const int D = c->D;
+    int mis[GMM_MAX_DIMENSIONS];
+    int nm = 0;
+    unsigned obs_mask = 0;
+    for (int d = 0, i = 0; d < D; d++) {
+        if (i < n_obs && obs_dims[i] == d) { obs_mask |= 1u << d; i++; }
+        else mis[nm++] = d;
+    }
+    const size_t len = (size_t)K * c->F + 1;
+    std::vector<double> g, cm;                              // per cluster G [nm][n_obs] and C = S_MM^-1 [nm][nm], in double
+    int rc = GMM_OK;
+    ConditionBuffers& cb = c->cond;
+    if (nm > 0) {
+        if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, D)));
+        if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, D)));
+        g.resize((size_t)K * nm * n_obs);
+        cm.resize((size_t)K * nm * nm);
+        rc = condition_params(c, K, obs_dims, n_obs, mis, nm, false, "gmm_condition_stats", g.data(), cm.data());
+    }
+    if (rc == GMM_OK && n > 0) {
+        rc = score_buffers(c);
+        if (rc == GMM_OK) rc = score_stats_buffers(c, memberships != nullptr, nm > 0);
+        if (rc == GMM_OK)
+            rc = nm > 0 ? condition_stats_batch(c, K, n_obs, obs_mask, events_obs, n, stats_out != nullptr, memberships)
+                        : score_stats_batch(c, K, events_obs, n, stats_out != nullptr, memberships, c->sstats.cond_prof);
+        // nothing of this call may still be in flight when it returns (also after a failure)
+        const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
+        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+            rc = fail(GMM_ERR_CUDA, std::string("gmm_condition_stats: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    }
+    if (rc == GMM_OK) {
+        if (stats_out) {
+            if (n > 0) std::memcpy(stats_out, c->sstats.h_stats, sizeof(double) * len);
+            else std::fill(stats_out, stats_out + len, 0.0);
+            if (n > 0 && nm > 0) {
+                const std::function<void(int)> per_cluster = [&](int k) {
+                    condition_stats_cluster(stats_out + (size_t)k * c->F, D, obs_dims, n_obs, mis, nm, c->host.means + (size_t)k * D, c->shift,
+                                            &g[(size_t)k * nm * n_obs], &cm[(size_t)k * nm * nm]);
+                };
+                if (K >= 8) {
+                    if (!c->pool) c->pool = new HostPool(c->host_threads);
+                    else c->pool->resize(c->host_threads);
+                    c->pool->run(K, per_cluster);
+                } else {
+                    for (int k = 0; k < K; k++) per_cluster(k);
+                }
+            }
+        }
+        if (shift_out) std::memcpy(shift_out, c->shift, sizeof(double) * (size_t)D);
+    }
+    c->sstats.cond_prof.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_get_condition_stats_profile(gmm_ctx* c, double out[4], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_condition_stats_profile: bad argument");
+    StatsProfile& t = c->sstats.cond_prof;
+    out[0] = t.kernel_ms; out[1] = t.wall_ms; out[2] = (double)t.m_tensor; out[3] = (double)t.m_simt;
+    if (reset) t = StatsProfile();
     return GMM_OK;
 }
 

@@ -341,7 +341,7 @@ void build_epack(int K, int D, const clusters_t* c, float* out) {
 }
 
 bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_obs, const int* mis, int nm, float* p_o,
-                       float* constant_o, float* g, float* cvar) {
+                       float* constant_o, float* g, float* cvar, double* g_d, double* c_d) {
     constexpr int DM = GMM_MAX_DIMENSIONS;
     const float* P = c->Rinv + (size_t)k * D * D;
     auto S = [&](int i, int j) { return 0.5 * ((double)P[i * D + j] + (double)P[j * D + i]); };
@@ -391,8 +391,58 @@ bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_
         cvar[d] = (float)v;
         for (int o = 0; o < n_obs; o++) g[d * n_obs + o] = (float)(-Z[d][o]);
     }
+    if (g_d)
+        for (int d = 0; d < nm; d++)
+            for (int o = 0; o < n_obs; o++) g_d[d * n_obs + o] = -Z[d][o];
+    if (c_d)
+        for (int d = 0; d < nm; d++)
+            for (int e = 0; e <= d; e++) {
+                double v = 0.0;
+                for (int i = d; i < nm; i++) v += Li[i][d] * Li[i][e];
+                c_d[d * nm + e] = c_d[e * nm + d] = v;
+            }
     *constant_o = (float)((double)c->constant[k] + 0.5 * nm * std::log(2.0 * M_PI) - ld);
     return true;
+}
+
+void condition_stats_cluster(double* row, int D, const int* obs, int n_obs, const int* mis, int nm, const float* mu,
+                             const double* shift, const double* g, const double* cm) {
+    constexpr int DM = GMM_MAX_DIMENSIONS;
+    double T1[DM], T2[DM][DM], b[DM], u[DM], GT2[DM][DM];
+    const double T0 = row[0];
+    for (int a = 0; a < n_obs; a++) {
+        T1[a] = row[1 + obs[a]];
+        for (int c = 0; c <= a; c++) T2[a][c] = T2[c][a] = row[feat2(D, obs[a], obs[c])];   // obs increasing: obs[a] >= obs[c]
+    }
+    for (int d = 0; d < nm; d++) {                          // b = (mu_M - s_M) - G (mu_O - s_O),  u = G T1,  G T2
+        const double* gd = g + (size_t)d * n_obs;
+        double v = (double)mu[mis[d]] - shift[mis[d]], w = 0.0;
+        for (int a = 0; a < n_obs; a++) {
+            v -= gd[a] * ((double)mu[obs[a]] - shift[obs[a]]);
+            w += gd[a] * T1[a];
+        }
+        b[d] = v;
+        u[d] = w;
+        for (int a = 0; a < n_obs; a++) {
+            double t = 0.0;
+            for (int c = 0; c < n_obs; c++) t += gd[c] * T2[c][a];
+            GT2[d][a] = t;
+        }
+    }
+    for (int d = 0; d < nm; d++) {
+        const int i = mis[d];
+        row[1 + i] = b[d] * T0 + u[d];
+        for (int a = 0; a < n_obs; a++) {                   // S2_MO = b T1^T + G T2
+            const int j = obs[a];
+            row[i > j ? feat2(D, i, j) : feat2(D, j, i)] = b[d] * T1[a] + GT2[d][a];
+        }
+        for (int e = 0; e <= d; e++) {                      // S2_MM = T0 (b b^T + C) + b u^T + u b^T + G T2 G^T
+            const double* ge = g + (size_t)e * n_obs;
+            double q = 0.0;
+            for (int a = 0; a < n_obs; a++) q += GT2[d][a] * ge[a];
+            row[feat2(D, i, mis[e])] = T0 * (b[d] * b[e] + cm[(size_t)d * nm + e]) + b[d] * u[e] + u[d] * b[e] + q;
+        }
+    }
 }
 
 }  // namespace gmm

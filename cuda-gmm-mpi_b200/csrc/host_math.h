@@ -70,8 +70,17 @@ void build_epack(int K, int D, const clusters_t* c, float* out);
 //   *constant_o        = constant + nm/2 ln 2 pi - 1/2 ln det S_MM
 //   g [nm][n_obs]      = -S_MM^-1 S_MO               (regression of the missing dimensions on dx_O)
 //   cvar [nm]          = diag(S_MM^-1)                (conditional variances)
+//   g_d [nm][n_obs], c_d [nm][nm]: when not NULL, G and the full S_MM^-1 in double (gmm_condition_stats' expansion)
 // S_MM is factorised once (Cholesky).  false = S_MM is not positive definite (a pivot <= 0 or not finite); nothing written.
 bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_obs, const int* mis, int nm, float* p_o,
-                       float* constant_o, float* g, float* cvar);
+                       float* constant_o, float* g, float* cvar, double* g_d = nullptr, double* c_d = nullptr);
+// gmm_condition_stats' expansion of one cluster's packed row (F doubles, about `shift`) in place, in double: on entry the
+// entries of the observed dimensions hold T0 = sum r, T1 = sum r y, T2 = sum r y y^T (y = x_O - s_O, r the marginal
+// posterior); the entries that involve a missing dimension are overwritten with their expectations given x_O,
+//   S1_M = b T0 + G T1,  S2_MO = b T1^T + G T2,  S2_MM = T0 (b b^T + C) + b u^T + u b^T + G T2 G^T,  u = G T1,
+// with b = (mu_M - s_M) - G (mu_O - s_O).  mu: the cluster's float means [D]; g [nm][n_obs] = G and cm [nm][nm] = C = S_MM^-1
+// as condition_cluster returns them in double.
+void condition_stats_cluster(double* row, int D, const int* obs, int n_obs, const int* mis, int nm, const float* mu,
+                             const double* shift, const double* g, const double* cm);
 
 }  // namespace gmm

@@ -112,4 +112,53 @@ condition_simt_kernel(const float* __restrict__ x_obs, int n, int n_obs, int n_m
     }
 }
 
+// Chunk preparation of gmm_condition_stats: ONE pass over a chunk's rows [n][n_obs] (the coordinates of the observed
+// dimensions) that writes
+//   xo_soa[a][e] = x                the observed SoA copy [n_obs][pitch] the marginal E-step reads (when xo_soa != NULL);
+//   the D-row image [D][pitch] the context's M-step reads, so that the missing dimensions add exact zeros (when
+//   shift_f is the float centre the M-step uses) and the observed entries of its output are the marginal moments:
+//     z_img (wgmma M-step)  (x - shift_f) * inv_scale_f on an observed row, with standardise_soa_kernel's operations
+//                           (bit-identical to score_stats_prep_kernel's z), and 0 on a missing row;
+//     x_img (FP64 M-step)   x on an observed row and shift_f on a missing row;
+//   *flag |= kScoreStatsNotFinite for a coordinate that is not finite, kScoreStatsBeyondZb for |z| >= zb on an observed
+//            dimension (tested when z_img != NULL).
+// obs_mask: bit d set when dimension d is observed (its column in the rows is the number of observed dimensions below it).
+// Block (32, 8), as score_stats_prep_kernel.
+__global__ void __launch_bounds__(256)
+condition_stats_prep_kernel(const float* __restrict__ rows_obs, int n, int n_obs, int D, unsigned obs_mask,
+                            const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float zb,
+                            float* __restrict__ xo_soa, float* __restrict__ z_img, float* __restrict__ x_img, size_t pitch,
+                            int* __restrict__ flag) {
+    __shared__ float tile[32][33];
+    const int e0 = blockIdx.x * 32;
+    const int rows = min(32, n - e0);
+    const int tid = threadIdx.y * 32 + threadIdx.x;
+    const float* src = rows_obs + (size_t)e0 * n_obs;
+    for (int i = tid; i < rows * n_obs; i += 256) tile[i / n_obs][i % n_obs] = src[i];
+    __syncthreads();
+    const int e = e0 + threadIdx.x;
+    int bits = 0;
+    if (threadIdx.x < rows) {
+        for (int d = threadIdx.y; d < D; d += 8) {
+            if (!((obs_mask >> d) & 1u)) {
+                if (z_img) z_img[(size_t)d * pitch + e] = 0.0f;
+                if (x_img) x_img[(size_t)d * pitch + e] = shift_f[d];
+                continue;
+            }
+            const int a = __popc(obs_mask & ((1u << d) - 1u));
+            const float x = tile[threadIdx.x][a];
+            if (!isfinite(x)) bits |= kScoreStatsNotFinite;
+            if (xo_soa) xo_soa[(size_t)a * pitch + e] = x;
+            if (x_img) x_img[(size_t)d * pitch + e] = x;
+            if (z_img) {
+                const float z = __fmul_rn(__fsub_rn(x, shift_f[d]), inv_scale_f[d]);
+                if (!(fabsf(z) < zb)) bits |= kScoreStatsBeyondZb;
+                z_img[(size_t)d * pitch + e] = z;
+            }
+        }
+    }
+    bits = __reduce_or_sync(0xffffffffu, bits);
+    if (bits && threadIdx.x == 0) atomicOr(flag, bits);
+}
+
 }  // namespace gmm

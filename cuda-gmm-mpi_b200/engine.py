@@ -87,6 +87,9 @@ def load_library():
     L.gmm_condition.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_void_p, _DP]
     L.gmm_get_condition_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_condition_stats.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p,
+                                      C.c_void_p]
+    L.gmm_get_condition_stats_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
@@ -378,6 +381,30 @@ class Engine:
         out = (C.c_double * 2)()
         _check(self.lib.gmm_get_condition_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], wall_ms=out[1])
+
+    def condition_stats(self, K, obs_dims, events_obs, stats=True, memberships=False):
+        """M-step statistics of events measured on the dimensions obs_dims only (gmm_condition_stats): the expected full-D
+        statistics under the current K-cluster parameters, and the posteriors under the marginal mixture of obs_dims.
+        events_obs is [n][len(obs_dims)].  Returns (stats [K*F+1] float64 or None, shift [D] float64, memberships [K][n]
+        float32 or None).  The statistics add to gmm_score_stats' and to other calls'; host_finalize turns their sum into
+        one EM iteration."""
+        obs = np.ascontiguousarray(obs_dims, np.int32).reshape(-1)
+        ev = np.ascontiguousarray(events_obs, np.float32)
+        if ev.ndim != 2 or ev.shape[1] != obs.size:
+            raise ValueError(f"events_obs must be [n][{obs.size}], got {ev.shape}")
+        n = ev.shape[0]
+        st = np.empty(stats_len(K, self.D), np.float64) if stats else None
+        sh = np.empty(self.D, np.float64)
+        mb = np.empty((K, n), np.float32) if memberships else None
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        _check(self.lib.gmm_condition_stats(self.h, K, obs.ctypes.data if obs.size else None, int(obs.size), ev.ctypes.data if n else None,
+                                            n, ptr(st), ptr(sh), ptr(mb)))
+        return st, sh, mb
+
+    def condition_stats_profile(self, reset=False):
+        out = (C.c_double * 4)()
+        _check(self.lib.gmm_get_condition_stats_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1], mstep_tensor_chunks=int(out[2]), mstep_simt_chunks=int(out[3]))
 
     def fit_profile(self):
         out = (C.c_double * 4)()

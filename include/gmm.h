@@ -355,6 +355,46 @@ int  gmm_condition(gmm_ctx*, int K, const int* obs_dims, int n_obs, const float*
 /* Since the last reset: out[0] kernel ms, out[1] wall ms inside gmm_condition.                                        */
 int  gmm_get_condition_profile(gmm_ctx*, double out[2], int reset);
 
+/* M-step statistics of n events measured on a subset O of the dimensions: the E-step of EM with values missing at
+ * random (Ghahramani and Jordan 1994), so that EM can fit a full-D mixture to tubes of a split panel that share a
+ * backbone.  The statistics are gmm_score_stats' (packed, about the context's centre, summable over calls, ranks and
+ * missing patterns) with every entry that involves a missing dimension replaced by its expectation given x_O under the
+ * parameter set the next gmm_estep(ctx, K) would use.  One EM iteration over tubes t: stats = sum_t
+ * gmm_condition_stats(tube t) (+ gmm_score_stats of complete rows), gmm_host_finalize, gmm_set_clusters.
+ *   obs_dims, n_obs, events_obs   as gmm_condition defines them (rows [n][n_obs] in the order of obs_dims).
+ *   stats_out   [gmm_stats_len(K, D)], full-D layout of gmm_host_finalize about the centre; overwritten, not
+ *               accumulated; the last slot is the sum of the events' marginal log-densities (the observed-data
+ *               log-likelihood).  May be NULL (then no M-step work is done).
+ *   shift_out   [D] the centre s (float-rounded when the wgmma M-step can run); may be NULL.
+ *   memberships [K][n] cluster-major: the posteriors under the MARGINAL mixture of gmm_condition; may be NULL.
+ * At least one of stats_out / memberships must be non-NULL.  No collective; nothing of the EM state or of another
+ * call's profile changes.
+ * Semantics (restated in float64 numpy by tests/_condition_stats_ref.py), with NM = D - n_obs >= 1:
+ *   - the marginal parameters are gmm_condition's (same derivation, same float rounding, same packing); the
+ *     memberships come from the SIMT E-step on them, so their row maximum is gmm_condition's max_resp bit for bit.
+ *   - T0 = sum r, T1 = sum r y, T2 = sum r y y^T (y = x_O - s_O) come from the context's own M-step run over all D
+ *     dimensions on rows whose missing dimensions contribute zeros.
+ *   - per cluster, in double from the float Rinv (P), with S = (P + P^T) / 2: G = -S_MM^-1 S_MO, C = S_MM^-1 (the full
+ *     conditional covariance), b = (mu_M - s_M) - G (mu_O - s_O), u = G T1.  Then E[x_M | x_O, k] - s_M = b + G y and
+ *       S0 = T0, S1_O = T1, S2_OO = T2,  S1_M = b T0 + u,  S2_MO = b T1^T + G T2,
+ *       S2_MM = T0 (b b^T + C) + b u^T + u b^T + G T2 G^T.
+ *   - n_obs = D is gmm_score_stats: the same code path and the same bits.
+ * Kernels: a prep kernel, the SIMT E-step on the observed dimensions, and the M-step gmm_score_stats would choose, per
+ * chunk of option "score_chunk" events (a chunk with an observed coordinate at or beyond the tensor M-step's bound zb
+ * runs the FP64 SIMT M-step, or fails with GMM_ERR_STATE under mstep_path = GMM_PATH_TENSOR).  Rows stream through
+ * gmm_score's slots; the chunk buffers are gmm_score_stats', plus an observed copy of D x score_chunk floats allocated on
+ * the first call with NM >= 1 and freed by gmm_destroy.
+ * Errors: K outside [1, Kmax], n < 0, events_obs == NULL with n > 0, obs_dims == NULL, n_obs outside [1, D], indices
+ * that are not strictly increasing or out of range, both outputs NULL, or a coordinate that is not finite ->
+ * GMM_ERR_ARG; K != the K of the current parameters, a call between gmm_mstep and gmm_constants, a cluster whose block
+ * P_MM is not positive definite (the first one is named in the message), or a multi-rank context whose centre is not
+ * fixed yet -> GMM_ERR_STATE.  n = 0 gives zero statistics and fills shift_out.                                       */
+int  gmm_condition_stats(gmm_ctx*, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n,
+                         double* stats_out, double* shift_out, float* memberships);
+/* Since the last reset: out[0] kernel ms (prep + E + M), out[1] wall ms inside gmm_condition_stats, out[2] / out[3]
+ * chunks whose statistics came from the wgmma / FP64 SIMT M-step.                                                    */
+int  gmm_get_condition_stats_profile(gmm_ctx*, double out[4], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce

@@ -8,7 +8,12 @@ host-to-host rate (host clock around gmm_condition, best of --repeats after one 
 numpy restatement (tests/_condition_ref.py) takes on --numpy-n events, scaled to 10M.  Prints the card's name, power limit
 and maximum SM clock (read-only nvidia-smi query) first.
 
-    python scripts/bench_condition.py [--n 10000000] [--repeats 3] [--em 10] [--numpy-n 200000]
+With --mode stats it measures gmm_condition_stats on the same rows instead: the kernel time (prep + marginal E-step + M-step)
+per 10M events (gmm_get_condition_stats_profile) beside the resident E- and M-step times per 10M events of the same context
+(gmm_get_profile over --em EM iterations on the 10M fitted events), the M-step kernel that served the chunks, and the
+host-to-host rate with and without memberships (host clock around the call, best of --repeats after one warm-up call).
+
+    python scripts/bench_condition.py [--mode condition|stats] [--n 10000000] [--repeats 3] [--em 10] [--numpy-n 200000]
                                       [--shapes 24x64x16,16x32x8,32x512x16]
 """
 import argparse
@@ -36,6 +41,7 @@ def main():
     ap.add_argument("--em", type=int, default=10)
     ap.add_argument("--numpy-n", type=int, default=200_000)
     ap.add_argument("--shapes", default="24x64x16,16x32x8,32x512x16")
+    ap.add_argument("--mode", choices=("condition", "stats"), default="condition")
     a = ap.parse_args()
     pkg = entry.load_package()
     pkg.load_library()
@@ -47,6 +53,9 @@ def main():
         fit = pkg.synth.make_blobs(a.n, D, K, seed=20260921)
         new = np.ascontiguousarray(pkg.synth.make_blobs(a.n, D, K, seed=20261015)[:, :n_obs])
         res = dict(n=a.n, D=D, K=K, n_obs=n_obs)
+        if a.mode == "stats":
+            print(json.dumps(stats_shape(pkg, a, fit, new, D, K, obs)), flush=True)
+            continue
         with pkg.Engine(fit, K) as eng:
             eng.seed(K)
             eng.em(K, a.em, a.em)
@@ -80,6 +89,42 @@ def main():
             cref.condition(cl, K, obs, new[s:min(m, s + 20_000)])
         res["numpy_f64_ms_per_10M"] = round((time.perf_counter() - t0) * 1e3 * 1e7 / m, 0)
         print(json.dumps(res), flush=True)
+
+
+def stats_shape(pkg, a, fit, new, D, K, obs):
+    n_obs = len(obs)
+    res = dict(mode="stats", n=a.n, D=D, K=K, n_obs=n_obs)
+    with pkg.Engine(fit, K) as eng:
+        eng.seed(K)
+        eng.em(K, 2, 2)
+        eng.profile(reset=True)
+        eng.em_iterations(K, a.em)                  # the resident steps on the same context, for comparison
+        p = eng.profile()
+        res.update(resident_estep_ms_per_10M=round(p["estep_ms"] / a.em * 1e7 / a.n, 3),
+                   resident_mstep_ms_per_10M=round(p["mstep_ms"] / a.em * 1e7 / a.n, 3))
+        st = np.empty(pkg.stats_len(K, D), np.float64)
+        sh = np.empty(D, np.float64)
+        mb = np.empty((K, a.n), np.float32)
+        for memberships in (False, True):
+            call = lambda: eng.lib.gmm_condition_stats(eng.h, K, obs.ctypes.data, n_obs, new.ctypes.data, a.n, st.ctypes.data,  # noqa: E731
+                                                       sh.ctypes.data, mb.ctypes.data if memberships else None)
+            assert call() == 0, eng.lib.gmm_last_error()                          # warm-up: buffers
+            eng.condition_stats_profile(reset=True)
+            walls = []
+            for _ in range(a.repeats):
+                t0 = time.perf_counter()
+                rc = call()
+                walls.append(time.perf_counter() - t0)
+                assert rc == 0, eng.lib.gmm_last_error()
+            prof = eng.condition_stats_profile()
+            tag = "with_memberships" if memberships else "stats_only"
+            if not memberships:
+                res.update(kernel_ms_per_10M=round(prof["kernel_ms"] / a.repeats * 1e7 / a.n, 3),
+                           mstep_tensor_chunks=prof["mstep_tensor_chunks"] // a.repeats,
+                           mstep_simt_chunks=prof["mstep_simt_chunks"] // a.repeats)
+            res[f"host_to_host_ms_{tag}"] = round(min(walls) * 1e3, 1)
+            res[f"host_to_host_events_per_s_{tag}"] = float(f"{a.n / min(walls):.3g}")
+    return res
 
 
 if __name__ == "__main__":
