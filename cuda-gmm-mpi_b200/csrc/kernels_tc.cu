@@ -24,19 +24,19 @@
 //                                                       g is below the quantum; ~1 % of the magnitude, its truncation
 //                                                       bias is 1e-8 of the statistic
 // The raw-moment cancellation |mu - shift|^2 / sigma^2 ~ 100 multiplies unbiased rounding noise only.
-// Each column group is its own N = 32 accumulator: ph x gh into the exact one, then ph x gl and pl x gs into the
-// remainder one.  All MMAs of a consumer have the same shape and no two accumulators overlap, so ptxas keeps the
-// wgmma of a sub-tile in flight together (an N = 64 MMA filling both groups plus an N = 32 MMA into its upper half
-// made it wait for every MMA before issuing the next, C7511).
+// Each column group is its own N = NCL accumulator (NCL = 32 or 64 clusters per CTA): ph x gh into the exact one, then
+// ph x gl and pl x gs into the remainder one.  All MMAs of a consumer have the same shape and no two accumulators overlap,
+// so ptxas keeps the wgmma of a sub-tile in flight together (an N = 64 MMA filling both groups plus an N = 32 MMA into
+// its upper half made it wait for every MMA before issuing the next, C7511).
 //
-// Dataflow per CTA (persistent over a contiguous range of events, 32 clusters per CTA row of the grid):
-//   warp 0      TMA producer: tile [D][32 events] of the pre-standardised SoA copy z and raw
-//               responsibility tile [32 clusters][32 events] (2-D tensor maps, both SWIZZLE_128B, zero fill out of bounds)
+// Dataflow per CTA (persistent over a contiguous range of events; NCL clusters and, at NCL = 64, half of the feature rows):
+//   warp 0      TMA producer: tile [D][32 events] of the pre-standardised SoA copy z and raw responsibility boxes
+//               [32 clusters][32 events] (2-D tensor maps, both SWIZZLE_128B, zero fill out of bounds)
 //   warps 1-3   split the responsibilities and write the wgmma B images gh / gl / gs (no-swizzle core-matrix layout)
-//   warpgroups 1 .. MT  consumers, one per 128-row feature tile: each thread builds the A fragments of its 4 feature rows
-//               (mstep_rows.h) from the raw z tile in registers — the feature operand never goes through shared memory —
-//               and per 32 events the warpgroup issues 2 x 2 x 3 m64n32k16 wgmma (A from registers), one group per
-//               64-row half, the group of one half running while the other half is built.  The exact group is drained
+//   warpgroups 1 .. MT  consumers: each thread builds the A fragments of its feature rows (mstep_rows.h) from the raw z
+//               tile in registers — the feature operand never goes through shared memory — and per 32 events the
+//               warpgroup issues 2 x 3 wgmma per 64-row half it owns (A from registers: m64n32k16 for both halves of a
+//               tile, or m64n64k16 for one half), each group running while the next is built.  The exact group is drained
 //               every 128 events and the remainder group every 512 into FP32 round-to-nearest partial sums held in shared
 //               memory (one private slot per thread), written ONCE per CTA (no scratch zeroing, no atomics).
 // A second tiny kernel reduces the per-CTA partials in double and un-scales.
@@ -53,6 +53,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "host_math.h"
@@ -75,7 +76,7 @@ using namespace ptx;
 // M-step kernel configuration
 // ---------------------------------------------------------------------------
 constexpr int kTE = 32;          // events per sub-tile (MMA K extent per operand part)
-constexpr int kNCL = 32;         // clusters per CTA pass (N of the exact / remainder groups: register budget of the consumers)
+constexpr int kNCL = 32;         // clusters per responsibility TMA box and per column block of the partial sums
 constexpr int kNST = 3;          // responsibility operand stages
 constexpr int kNRAW = 4;         // raw (TMA) stages
 constexpr int kChunkSub = 4;     // sub-tiles per chain of the exact column group: 128 events (the bit budget below)
@@ -91,18 +92,27 @@ constexpr float kGammaMagic = 1.5f * 134217728.0f;   // 1.5 * 2^27: ulp = 16 = 2
 // or the ones pseudo-dimension); consumer thread (warp w, lane group gid) of tile mt owns the 4 rows
 // mt * 128 + h * 64 + 16 w + gid + 8 s, which share the factor a.  The thread builds the wgmma A fragments of its rows
 // from the raw z tile itself (register operand), so the feature operand never goes through shared memory.
-template <int D> struct MCfg {
+//
+// Two schedules, chosen by K (launch_mstep_d), with the same MT consumer warpgroups and 64 accumulators per thread:
+//   NCL = 32  (K <= 32)  a CTA covers all 2 MT feature halves for 32 clusters: each consumer owns both halves of its tile
+//   NCL = 64  (K > 32)   the two CTAs of an event range split the 2 MT halves, each for 64 clusters: each consumer owns one
+//                        half (part p, consumer c: half p MT + c).  The feature operand of an event is built once per 64
+//                        clusters instead of once per 32, and the pair shares its z / gamma tiles through L2.
+template <int D, int NCL_> struct MCfg {
     static_assert(D % 4 == 0, "tensor M-step: D must be a multiple of 4");
+    static_assert(NCL_ == 32 || NCL_ == 64, "tensor M-step: 32 or 64 clusters per CTA");
+    static constexpr int NCL = NCL_;
+    static constexpr int HPC = 64 / NCL;                  // 64-row feature halves per consumer warpgroup
     static constexpr int F = 1 + D + D * (D + 1) / 2;
     static constexpr int S = D / 4;
     static constexpr int MT = (4 * ((1 + 2 * S + S * (D / 2) + 7) / 8) * 8 + 127) / 128;   // feature tiles (mstep_tiles)
-    static constexpr int G_PART = kNCL * kTE * 2;
-    static constexpr int G_STAGE = 3 * G_PART;            // gh, gl, gs: three K-major N = 32 images
+    static constexpr int G_PART = NCL * kTE * 2;
+    static constexpr int G_STAGE = 3 * G_PART;            // gh, gl, gs: three K-major N = NCL images
     // raw z stage: the [D][32 events] tile (SWIZZLE_128B), padded to 1 KB, then 1 KB of ones (8 rows of the same swizzle:
     // the ones pseudo-dimension at a stage-relative address like every dimension)
     static constexpr int RAWZ = (D * kTE * 4 + 1023) / 1024 * 1024;
     static constexpr int RAWX = RAWZ + 1024;
-    static constexpr int RAWG = kNCL * kTE * 4;
+    static constexpr int RAWG = NCL * kTE * 4;            // NCL / 32 boxes of [32 clusters][32 events]
     static constexpr int OFF_G = 0;
     static constexpr int OFF_RAWX = OFF_G + kNST * G_STAGE;
     static constexpr int OFF_RAWG = OFF_RAWX + kNRAW * RAWX;
@@ -196,22 +206,29 @@ __device__ __forceinline__ void load_row(uint32_t addr, float2 (&z)[4]) {
     for (int p = 0; p < 4; p++) z[p] = lds_f2(addr ^ (uint32_t)(p << 5));
 }
 
-// The MMAs of one half (both k-steps): ph gh into the exact group, ph gl + pl gs into the remainder group.
-__device__ __forceinline__ void issue_half(float (&ex)[16], float (&rm)[16], const uint32_t (&hi)[2][4], const uint32_t (&lo)[2][4],
+// The MMAs of one half (both k-steps) for NCL clusters: ph gh into the exact group, ph gl + pl gs into the remainder group.
+template <int NCL>
+__device__ __forceinline__ void issue_half(float (&ex)[NCL / 2], float (&rm)[NCL / 2], const uint32_t (&hi)[2][4], const uint32_t (&lo)[2][4],
                                            uint32_t gam, bool new1, bool new2) {
 #pragma unroll
     for (int ks = 0; ks < kTE / 16; ks++) {
         const uint64_t hdesc = make_smem_desc(gam + ks * 256, /*LBO*/ 128, /*SBO*/ 512);     // gh
-        const uint64_t ldesc = make_smem_desc(gam + kNCL * kTE * 2 + ks * 256, 128, 512);    // gl
-        const uint64_t sdesc = make_smem_desc(gam + 2 * kNCL * kTE * 2 + ks * 256, 128, 512); // gs
+        const uint64_t ldesc = make_smem_desc(gam + NCL * kTE * 2 + ks * 256, 128, 512);     // gl
+        const uint64_t sdesc = make_smem_desc(gam + 2 * NCL * kTE * 2 + ks * 256, 128, 512); // gs
 #if GMM_MSTEP_CUT == 1
         asm volatile("" ::"r"(hi[ks][0]), "r"(hi[ks][1]), "r"(hi[ks][2]), "r"(hi[ks][3]), "r"(lo[ks][0]), "r"(lo[ks][1]), "r"(lo[ks][2]),
                      "r"(lo[ks][3]), "l"(hdesc), "l"(ldesc), "l"(sdesc));
         (void)ex; (void)rm; (void)new1; (void)new2;
 #else
-        wgmma_m64n32k16_rs(ex, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], hdesc, ks > 0 || !new1);   // ph gh
-        wgmma_m64n32k16_rs(rm, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], ldesc, ks > 0 || !new2);   // ph gl
-        wgmma_m64n32k16_rs(rm, lo[ks][0], lo[ks][1], lo[ks][2], lo[ks][3], sdesc, true);              // + pl gs
+        if constexpr (NCL == 32) {
+            wgmma_m64n32k16_rs(ex, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], hdesc, ks > 0 || !new1);   // ph gh
+            wgmma_m64n32k16_rs(rm, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], ldesc, ks > 0 || !new2);   // ph gl
+            wgmma_m64n32k16_rs(rm, lo[ks][0], lo[ks][1], lo[ks][2], lo[ks][3], sdesc, true);              // + pl gs
+        } else {
+            wgmma_m64n64k16_rs(ex, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], hdesc, ks > 0 || !new1);
+            wgmma_m64n64k16_rs(rm, hi[ks][0], hi[ks][1], hi[ks][2], hi[ks][3], ldesc, ks > 0 || !new2);
+            wgmma_m64n64k16_rs(rm, lo[ks][0], lo[ks][1], lo[ks][2], lo[ks][3], sdesc, true);
+        }
 #endif
     }
 }
@@ -225,11 +242,14 @@ __device__ __forceinline__ bool chain2_ends(int i, int mt, int nsub) { return ((
 __device__ __forceinline__ bool chain2_starts(int i, int mt) { return i == 0 || ((i + mt) % kChunkSub2) == 0; }
 
 // opmap[row] = a | b << 8: the operand factors of row `row` (mstep_row_layout; codes >= kRowOne: rows of the ones block).
-template <int D>
-__global__ void __launch_bounds__(MCfg<D>::THREADS, 1)
-mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_g, int n,
+// Grid (ranges * 64 / NCL, ceil(K / NCL)): CTA x = range * 64 / NCL + part, so with NCL = 64 the two CTAs of a range run in
+// the same wave and the second reader of every z / gamma tile finds it in L2.
+template <int D, int NCL>
+__global__ void __launch_bounds__(MCfg<D, NCL>::THREADS, 1)
+mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_g, int n, int K,
                 float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic, const int* __restrict__ opmap) {
-    using C = MCfg<D>;
+    using C = MCfg<D, NCL>;
+    constexpr int HPC = C::HPC;
     extern __shared__ __align__(1024) uint8_t smem[];
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::OFF_BAR);
     uint64_t* raw_full = bars;                 // [kNRAW]
@@ -238,10 +258,11 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     uint64_t* op_empty = op_full + kNST;       // [kNST]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int e_begin = blockIdx.x * events_per_cta;
+    const int range = blockIdx.x / (2 / HPC), part = blockIdx.x % (2 / HPC);
+    const int e_begin = range * events_per_cta;
     const int e_end = min(n, e_begin + events_per_cta);
     const int nsub = (e_end - e_begin + kTE - 1) / kTE;
-    const int k0 = blockIdx.y * kNCL;
+    const int k0 = blockIdx.y * NCL;
 
     // ---- one-time setup: the ones block of every raw stage, barriers ----
     for (int i = threadIdx.x; i < kNRAW * 256; i += C::THREADS)
@@ -258,35 +279,42 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
         set_regs<C::REG_P, C::REG_LAUNCH>();
         if (warp == 0) {
             // ===================== TMA producer =====================
+            // one responsibility box per 32 clusters that holds a live one (a box wholly above K is not loaded: the
+            // columns it would fill are not read back)
+            const int nbox = min(NCL, K - k0 + kNCL - 1) / kNCL;
             if (elect_one()) {
                 for (int i = 0; i < nsub; i++) {
                     const int st = i % kNRAW, ph = (i / kNRAW) & 1;
                     mbar_wait_parked(&raw_empty[st], ph ^ 1, 500);
-                    mbar_arrive_expect_tx(&raw_full[st], kTE * D * 4 + C::RAWG);
+                    mbar_arrive_expect_tx(&raw_full[st], kTE * D * 4 + nbox * kNCL * kTE * 4);
                     const int e0 = e_begin + i * kTE;
                     tma_load_2d(smem + C::OFF_RAWX + st * C::RAWX, &tm_x, e0, 0, &raw_full[st]);
-                    tma_load_2d(smem + C::OFF_RAWG + st * C::RAWG, &tm_g, e0, k0, &raw_full[st]);
+                    for (int b = 0; b < nbox; b++)
+                        tma_load_2d(smem + C::OFF_RAWG + st * C::RAWG + b * kNCL * kTE * 4, &tm_g, e0, k0 + b * kNCL, &raw_full[st]);
                 }
             }
         } else {
             // ===================== responsibility operand: warps 1-3 =====================
-            // item (cluster row k, 8-event chunk ce): 128 per sub-tile, thread bt takes bt and (warp 1) bt + 96.
+            // item (cluster row k, 8-event chunk ce): 4 NCL per sub-tile, thread bt takes bt, bt + 96, ...
             // The raw tile is written by TMA with SWIZZLE_128B (16-byte chunk c of row r sits at chunk c ^ (r & 7)), so
             // 8 lanes reading the same chunk of 8 consecutive rows hit 8 different bank groups; the operand image puts
             // the 4 K-chunks of an 8-row group next to each other (LBO = 128, SBO = 512), so a warp stores 512
-            // contiguous bytes: no bank conflicts either way.
+            // contiguous bytes: no bank conflicts either way.  Each item's images are stored before the next is split,
+            // so the 56-register pool holds one item at a time.
             const int bt = threadIdx.x - 32;
-            constexpr int NIT = 2;
+            constexpr int NITEM = 4 * NCL, NIT = (NITEM + 95) / 96;
             for (int i = 0; i < nsub; i++) {
                 const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
                 const int os = i % kNST, oph = (i / kNST) & 1;
                 mbar_wait_parked(&raw_full[rs], rph, 200);
-                uint4 gh[NIT], gl[NIT], gs[NIT];
+                mbar_wait_parked(&op_empty[os], oph ^ 1, 200);
+                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512)
+                uint8_t* g_hi = smem + C::OFF_G + os * C::G_STAGE;
                 float dep = 0.0f;
 #pragma unroll
                 for (int u = 0; u < NIT; u++) {
                     const int it = bt + 96 * u;
-                    if (it >= 128) break;
+                    if (it >= NITEM) break;
                     const int kg = it >> 5, l = it & 31;
                     const int k = kg * 8 + (l & 7), ce = l >> 3;
                     const uint8_t* grow = smem + C::OFF_RAWG + rs * C::RAWG + k * (kTE * 4);
@@ -300,10 +328,13 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                         hi[v] = __fsub_rn(__fmaf_rn(g[v], kGammaScale, kGammaMagic), kGammaMagic);
                         lo[v] = __fmaf_rn(g[v], kGammaScale, -hi[v]);
                     }
-                    gh[u] = make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
-                    gl[u] = make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
-                    gs[u] = make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
-                                       pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
+                    *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) =
+                        make_uint4(pack_half2(hi[0], hi[1]), pack_half2(hi[2], hi[3]), pack_half2(hi[4], hi[5]), pack_half2(hi[6], hi[7]));
+                    *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) =
+                        make_uint4(pack_half2(lo[0], lo[1]), pack_half2(lo[2], lo[3]), pack_half2(lo[4], lo[5]), pack_half2(lo[6], lo[7]));
+                    *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) =
+                        make_uint4(pack_half2(g[0] * kGammaScale, g[1] * kGammaScale), pack_half2(g[2] * kGammaScale, g[3] * kGammaScale),
+                                   pack_half2(g[4] * kGammaScale, g[5] * kGammaScale), pack_half2(g[6] * kGammaScale, g[7] * kGammaScale));
                 }
                 // The raw tile must BE in registers before the stage goes back to the TMA producer: an mbarrier arrive does
                 // not wait for the warp's outstanding shared-memory loads.  The arrive is therefore made data-dependent on
@@ -312,18 +343,6 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                 __syncwarp();
                 if (lane == 0) mbar_arrive_after(&raw_empty[rs], dep);
                 else asm volatile("" ::"f"(dep));
-                mbar_wait_parked(&op_empty[os], oph ^ 1, 200);
-                // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512)
-                uint8_t* g_hi = smem + C::OFF_G + os * C::G_STAGE;
-#pragma unroll
-                for (int u = 0; u < NIT; u++) {
-                    const int it = bt + 96 * u;
-                    if (it >= 128) break;
-                    const int kg = it >> 5, l = it & 31;
-                    *reinterpret_cast<uint4*>(g_hi + kg * 512 + l * 16) = gh[u];
-                    *reinterpret_cast<uint4*>(g_hi + C::G_PART + kg * 512 + l * 16) = gl[u];
-                    *reinterpret_cast<uint4*>(g_hi + 2 * C::G_PART + kg * 512 + l * 16) = gs[u];
-                }
                 fence_proxy_async_smem();
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&op_full[os]);
@@ -332,27 +351,30 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
     } else {
         set_regs<C::REG_C, C::REG_LAUNCH>();
         // ===================== consumers: operand build and wgmma, accumulators in registers =====================
-        // feature tile of this warpgroup (rows 128 mt ..); the shuffle shows ptxas that it is warp-uniform, so the
-        // branches on it do not make ptxas serialise the wgmma
-        const int mt = __shfl_sync(0xffffffffu, (warp - 4) >> 2, 0);
+        // consumer warpgroup cw (the shuffle shows ptxas that it is warp-uniform, so the branches on the tile index do not
+        // make ptxas serialise the wgmma), its first 64-row half hx (of the 2 MT halves) and that half's feature tile mt
+        const int cw = __shfl_sync(0xffffffffu, (warp - 4) >> 2, 0);
+        const int hx = HPC == 2 ? 2 * cw : part * C::MT + cw;
+        const int mt = hx >> 1;
         const int ct = threadIdx.x - 128;                          // consumer thread 0 .. NCT-1
         const int wq = warp & 3, gid = lane >> 2, qd = lane & 3;
         float* racc = reinterpret_cast<float*>(smem + C::OFF_RACC) + ct;     // [32][NCT]: racc[j * NCT]
 #pragma unroll
         for (int j = 0; j < 32; j++) racc[j * C::NCT] = 0.0f;
-        // this thread's rows: shared factor a, factors b[slot] and rounding constants; stage-relative z-tile addresses of
-        // its 8 events (pair p at addr ^ (p << 5)): row r at r * 128 (ones block rows at RAWZ + rho * 128), chunk
-        // (qd >> 1) ^ (r & 7), byte 8 (qd & 1)
-        uint32_t fa, fb[4];
-        float mg[4];
+        // this thread's rows hx * 64 + h * 64 + 16 wq + gid + 8 s (slot 2 h + s): shared factor a, factors b[slot] and
+        // rounding constants; stage-relative z-tile addresses of its 8 events (pair p at addr ^ (p << 5)): row r at
+        // r * 128 (ones block rows at RAWZ + rho * 128), chunk (qd >> 1) ^ (r & 7), byte 8 (qd & 1)
+        constexpr int NSLOT = 2 * HPC;
+        uint32_t fa, fb[NSLOT];
+        float mg[NSLOT];
         {
-            const int* om = opmap + mt * 128 + wq * 16 + gid;
+            const int* om = opmap + hx * 64 + wq * 16 + gid;
             auto addr = [&](int code) {
                 const uint32_t row = code >= kRowOne ? (uint32_t)(C::RAWZ / 128 + code - kRowOne) : (uint32_t)code;
                 return row * 128 + ((((uint32_t)qd >> 1) ^ (row & 7)) << 4) + ((uint32_t)qd & 1) * 8;
             };
 #pragma unroll
-            for (int s = 0; s < 4; s++) {
+            for (int s = 0; s < NSLOT; s++) {
                 const int c = om[(s >> 1) * 64 + (s & 1) * 8];
                 const int a = c & 255, b = c >> 8;
                 if (s == 0) fa = addr(a);
@@ -361,94 +383,120 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
             }
         }
         const uint32_t zs0 = smem_u32(smem + C::OFF_RAWX);
-        float ex[2][16], rm[2][16];                                // per 64-row half: exact group, remainder group
+        float ex[HPC][NCL / 2], rm[HPC][NCL / 2];                  // per half of this consumer: exact group, remainder group
 #pragma unroll
-        for (int h = 0; h < 2; h++)
+        for (int h = 0; h < HPC; h++)
 #pragma unroll
-            for (int j = 0; j < 16; j++) { ex[h][j] = 0.0f; rm[h][j] = 0.0f; }
-        uint32_t fh[2][2][4], fl[2][2][4];                          // A fragments per half (one set in flight, one built)
+            for (int j = 0; j < NCL / 2; j++) { ex[h][j] = 0.0f; rm[h][j] = 0.0f; }
+        // Accumulator slot q (0 .. 31) of this thread: half q / (NCL / 2), value q % (NCL / 2).  16 at a time (the empty asm
+        // keeps ptxas from hoisting all 32 loads): with every accumulator live, 32 loads in flight would not fit the
+        // consumers' registers at D = 24.
+        auto add_to_racc = [&](float (&acc)[HPC][NCL / 2]) {
+#pragma unroll
+            for (int c = 0; c < 2; c++) {
+#pragma unroll
+                for (int j = 0; j < 16; j++) {
+                    const int q = 16 * c + j;
+                    racc[q * C::NCT] += acc[q / (NCL / 2)][q % (NCL / 2)];
+                }
+                asm volatile("" ::: "memory");
+            }
+        };
+        uint32_t fh[2][2][4], fl[2][2][4];                          // two A fragment sets: one in flight, one built
+        float2 za[4];
         int held = -1;                                             // responsibility stage of the previous sub-tile while its MMAs may run
-        // Software pipeline per half: the group of half 0 of sub-tile i is issued while half 1 of sub-tile i - 1 runs,
-        // half 1 of sub-tile i while half 0 runs; a half's fragments are rebuilt only after its previous group retired.
-        for (int i = 0; i < nsub; i++) {
+        // One MMA group: half h of this consumer for sub-tile i, A fragments in (gh, gl).  Two halves per consumer: the
+        // group of half 0 of sub-tile i is issued while half 1 of sub-tile i - 1 runs, half 1 of sub-tile i while half 0 runs.
+        // One half: the group of sub-tile i runs while sub-tile i + 1 is built.  Either way each group waits (wait_group 1)
+        // for the one before it, whose fragment set the next build overwrites.
+        auto group = [&](int i, auto hc, uint32_t (&gh)[2][4], uint32_t (&gl)[2][4]) {
+            constexpr int h = decltype(hc)::value;
             const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
             const int os = i % kNST, oph = (i / kNST) & 1;
             const uint32_t zst = zs0 + rs * C::RAWX;
             const uint32_t gam = smem_u32(smem + C::OFF_G + os * C::G_STAGE);
             // a chain starts with its first MMA overwriting the accumulators (the drain leaves them as they are)
             const bool new1 = chain_starts(i, mt), new2 = chain2_starts(i, mt);
-            mbar_wait_parked(&raw_full[rs], rph, 100);
-            float2 za[4], zb0[4], zb1[4];
-            load_row(zst + fa, za);
-            load_row(zst + fb[0], zb0);
-            load_row(zst + fb[1], zb1);
-            build_half(za, zb0, zb1, mg[0], mg[1], fh[0], fl[0]);
-            mbar_wait_parked(&op_full[os], oph, 100);
-            wgmma_fence();
-            issue_half(ex[0], rm[0], fh[0], fl[0], gam, new1, new2);
-            wgmma_commit();
-            // half 1 of the previous sub-tile has retired: its responsibility stage is free, and so are the fragments of half 1
-            wgmma_wait<1>();
-            __syncwarp();
-            if (lane == 0 && held >= 0) mbar_arrive(&op_empty[held]);
-            load_row(zst + fb[2], zb0);
-            load_row(zst + fb[3], zb1);
-            build_half(za, zb0, zb1, mg[2], mg[3], fh[1], fl[1]);
-            wgmma_fence();
-            issue_half(ex[1], rm[1], fh[1], fl[1], gam, new1, new2);
-            wgmma_commit();
-            // The raw stage goes back to the TMA producer only after this warp's loads from it have landed (an mbarrier
-            // arrive alone does not wait for them, see the responsibility warps).  The wgmma just issued reads the A
-            // fragments of half 1 and the one before those of half 0, which are computed from every z this thread loaded:
-            // the warpgroup-wide wgmma cannot issue before all of them are in registers, and the arrive follows it.
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&raw_empty[rs]);
-            wgmma_wait<1>();                                       // half 0 of this sub-tile has retired
-            held = os;
-            // drain: exact group at the end of its 128-event chain, remainder group at the end of its longer chain
-            // (the second ends only where the first does)
-            if (chain_ends(i, mt, nsub)) {
-                wgmma_wait<0>();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&op_empty[os]);
-                held = -1;
-#if GMM_MSTEP_CUT != 3
-                // one half at a time (the empty asm keeps ptxas from hoisting all 32 loads): with every accumulator
-                // live, 32 loads in flight would not fit the consumers' registers at D = 24
-#pragma unroll
-                for (int h = 0; h < 2; h++) {
-#pragma unroll
-                    for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += ex[h][j];
-                    asm volatile("" ::: "memory");
-                }
-                if (chain2_ends(i, mt, nsub)) {
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-#pragma unroll
-                        for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += rm[h][j];
-                        asm volatile("" ::: "memory");
-                    }
-                }
-#endif
+            if constexpr (h == 0) {
+                mbar_wait_parked(&raw_full[rs], rph, 100);
+                load_row(zst + fa, za);
             }
+            float2 zb0[4], zb1[4];
+            load_row(zst + fb[2 * h], zb0);
+            load_row(zst + fb[2 * h + 1], zb1);
+            build_half(za, zb0, zb1, mg[2 * h], mg[2 * h + 1], gh, gl);
+            if constexpr (h == 0) mbar_wait_parked(&op_full[os], oph, 100);
+            wgmma_fence();
+            issue_half<NCL>(ex[h], rm[h], gh, gl, gam, new1, new2);
+            wgmma_commit();
+            if constexpr (h == HPC - 1) {
+                // The raw stage goes back to the TMA producer only after this warp's loads from it have landed (an mbarrier
+                // arrive alone does not wait for them, see the responsibility warps).  The groups of this sub-tile read A
+                // fragments computed from every z this thread loaded: the warpgroup-wide wgmma cannot issue before all of
+                // them are in registers, and the arrive follows it.
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&raw_empty[rs]);
+            }
+            wgmma_wait<1>();
+            if constexpr (h == 0) {
+                // the previous sub-tile's last group has retired: its responsibility stage is free
+                __syncwarp();
+                if (lane == 0 && held >= 0) mbar_arrive(&op_empty[held]);
+            }
+            if constexpr (h == HPC - 1) {
+                held = os;
+                // drain: exact group at the end of its 128-event chain, remainder group at the end of its longer chain
+                // (the second ends only where the first does)
+                if (chain_ends(i, mt, nsub)) {
+                    wgmma_wait<0>();
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&op_empty[os]);
+                    held = -1;
+#if GMM_MSTEP_CUT != 3
+                    add_to_racc(ex);
+                    if (chain2_ends(i, mt, nsub)) add_to_racc(rm);
+#endif
+                }
+            }
+        };
+        using H0 = std::integral_constant<int, 0>;
+        using H1 = std::integral_constant<int, 1>;
+        if constexpr (HPC == 2) {
+            for (int i = 0; i < nsub; i++) {
+                group(i, H0{}, fh[0], fl[0]);
+                group(i, H1{}, fh[1], fl[1]);
+            }
+        } else {
+            // whole pairs, then an odd last sub-tile: a skipped second group inside the loop would give ptxas a path on
+            // which set 0 is rebuilt while its group runs, and it would serialise the wgmma (C7513)
+            int i = 0;
+            for (; i + 1 < nsub; i += 2) {
+                group(i, H0{}, fh[0], fl[0]);
+                group(i + 1, H0{}, fh[1], fl[1]);
+            }
+            if (i < nsub) group(i, H0{}, fh[0], fl[0]);
         }
         wgmma_wait<0>();            // (the last sub-tile drained: nothing in flight; without it ptxas waits in every iteration)
 #if GMM_MSTEP_CUT == 3
 #pragma unroll
-        for (int h = 0; h < 2; h++)
+        for (int h = 0; h < HPC; h++)
 #pragma unroll
-            for (int j = 0; j < 16; j++) racc[(h * 16 + j) * C::NCT] += ex[h][j] + rm[h][j];
+            for (int j = 0; j < NCL / 2; j++) ex[h][j] += rm[h][j];
+        add_to_racc(ex);
 #endif
-        // one plain store of this thread's partial sums: [cta][tile][row][32 clusters]
-        float* my = scratch + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * C::MT * 128 * kNCL + (size_t)mt * 128 * kNCL;
+        // one plain store of this thread's partial sums: [32-cluster block][range][tile][row][32 clusters], the layout
+        // mstep_tc_finalize_kernel reduces (the same for both schedules)
+        const int nranges = gridDim.x * HPC / 2;
 #pragma unroll
-        for (int h = 0; h < 2; h++)
+        for (int h = 0; h < HPC; h++)
 #pragma unroll
-            for (int j = 0; j < 16; j += 2) {
-                const int row = h * 64 + wq * 16 + gid + 8 * ((j >> 1) & 1);
+            for (int j = 0; j < NCL / 2; j += 2) {
+                const int q = h * (NCL / 2) + j;
+                const int row = ((hx & 1) + h) * 64 + wq * 16 + gid + 8 * ((j >> 1) & 1);
                 const int col = (j >> 2) * 8 + 2 * qd;
-                *reinterpret_cast<float2*>(my + (size_t)row * kNCL + col) =
-                    make_float2(racc[(h * 16 + j) * C::NCT], racc[(h * 16 + j + 1) * C::NCT]);
+                const int ty = blockIdx.y * (NCL / kNCL) + col / kNCL;
+                float* dst = scratch + ((((size_t)ty * nranges + range) * C::MT + mt) * 128 + row) * kNCL + col % kNCL;
+                *reinterpret_cast<float2*>(dst) = make_float2(racc[q * C::NCT], racc[(q + 1) * C::NCT]);
             }
     }
 }
@@ -1004,7 +1052,7 @@ struct TcState {
     float* d_shift_f = nullptr;      // [32]
     float* d_inv_scale_f = nullptr;  // [32]
     double* d_scale = nullptr;       // [32] = 1 / inv_scale_f (double)
-    float* d_scratch = nullptr;      // [CTAs][MT][128][64] per-CTA partial sums, written once per launch
+    float* d_scratch = nullptr;      // [32-cluster blocks][ranges][MT][128][32] per-range partial sums, written once per launch
     size_t scratch_floats = 0;
     bool have_shift = false;
     bool mstep_ready = false;        // the fixed-point quanta of the feature rows are set and inside the supported range
@@ -1133,7 +1181,7 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
         TC_CUDA_TRY(cudaMalloc(&t->d_opmap, sizeof(int) * om.size()));
         TC_CUDA_TRY(cudaMemcpy(t->d_opmap, om.data(), sizeof(int) * om.size(), cudaMemcpyHostToDevice));
     }
-    const int ytiles = (Kmax + kNCL - 1) / kNCL;
+    const int ytiles = (Kmax + 63) / 64 * (64 / kNCL);         // 32-cluster column blocks of whole 64-cluster CTAs
     t->scratch_floats = (size_t)num_sms * ytiles * mt * 128 * kNCL;
     TC_CUDA_TRY(cudaMalloc(&t->d_scratch, sizeof(float) * t->scratch_floats));
     return GMM_OK;
@@ -1762,24 +1810,32 @@ int tc_launch_score(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream)
     }
 }
 
+// K <= 32: one CTA per event range and 32 clusters.  K > 32: two CTAs per range and 64 clusters, each building half of the
+// feature rows (MCfg): the feature operand is built once per 64 clusters, and both CTAs read the range's tiles in one wave.
 template <int D>
 static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, cudaStream_t stream) {
-    using C = MCfg<D>;
-    static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
+    using C32 = MCfg<D, 32>;
+    using C64 = MCfg<D, 64>;
+    static_assert(C32::SMEM_BYTES <= 232448 && C64::SMEM_BYTES <= 232448, "shared memory budget");
     if (!t->attr_mstep) {
-        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
+        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
         t->attr_mstep = true;
     }
     int gx = t->num_sms;
     int per = (n + gx - 1) / gx;
     per = (per + kTE - 1) / kTE * kTE;
     gx = (n + per - 1) / per;
-    const int gy = (K + kNCL - 1) / kNCL;
-    if ((size_t)gx * gy * C::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
-    dim3 grid(gx, gy);
-    mstep_tc_kernel<D><<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(tm_x, tm_g, n, t->d_scratch, per, t->magic, t->d_opmap);
+    const bool pair = K > 32;
+    const int ncl = pair ? 64 : 32;
+    const int gy = (K + ncl - 1) / ncl;
+    if ((size_t)gx * gy * (ncl / kNCL) * C32::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
+    if (pair)
+        mstep_tc_kernel<D, 64><<<dim3(2 * gx, gy), C64::THREADS, C64::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap);
+    else
+        mstep_tc_kernel<D, 32><<<dim3(gx, gy), C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap);
     TC_CUDA_TRY(cudaGetLastError());
-    mstep_tc_finalize_kernel<<<C::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C::MT, K, C::F, t->d_rowmap, t->d_scale, d_stats);
+    mstep_tc_finalize_kernel<<<C32::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C32::MT, K, C32::F, t->d_rowmap, t->d_scale, d_stats);
     TC_CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }

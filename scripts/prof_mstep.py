@@ -13,9 +13,11 @@ then
 Per library and shape: one E-step for the responsibilities, 3 warm-up M-steps, then the CUDA-event time of `--launches`
 M-steps (the engine's per-phase timer brackets the two kernels); the median of 3 such blocks is printed as ms per launch.
 Beside it, two times computed from the shapes (not measured):
-  - the tensor floor: the executed m64n32k16 MMAs at 4096 FP16 flop per clock and SM, at the card's maximum SM clock;
-  - the shared-memory model of both operand paths (staged feature operand, register feature operand) at 128 bytes per
-    clock and SM: the bytes every 32-event sub-tile of a CTA moves through shared memory, times the sub-tiles an SM runs.
+  - the tensor floor: the executed MMAs at 4096 FP16 flop per clock and SM, at the card's maximum SM clock;
+  - the shared-memory model at 128 bytes per clock and SM: the bytes every 32-event sub-tile of a CTA moves through shared
+    memory, times the sub-tiles an SM runs, for the staged feature operand of earlier builds and for the register feature
+    operand in the schedule launch_mstep_d() picks for K (32 clusters per CTA at K <= 32; at K > 32 two CTAs per event
+    range, each with half of the feature rows and 64 clusters).
 The number of warpgroup MMA instructions (HGMMA) in each library's mstep_tc_kernel is counted with cuobjdump -sass, so
 a variant whose MMAs the compiler dropped is visible.  The card's name, power limit and maximum SM clock are printed
 first.  Needs a GPU; the M-step runs on the tensor path only (no SIMT fall-back).
@@ -35,7 +37,7 @@ sys.path.insert(0, ROOT)
 import __graft_entry__ as entry  # noqa: E402
 
 SHAPES = {"c3": (10_000_000, 24, 64), "c2": (1_000_000, 16, 32)}
-KTE, NCL = 32, 32
+KTE = 32
 
 
 def smi(fields):
@@ -55,25 +57,33 @@ def tiles(D):
     return (rows + 127) // 128, rows
 
 
-def subtiles_per_sm(N, K, sms):
-    """launch_mstep_d(): contiguous event ranges of whole sub-tiles, one CTA per range and 32 clusters; an SM runs
+def ncl(K, register_a=True):
+    """Clusters per CTA of launch_mstep_d() (the staged path always had 32)."""
+    return 64 if register_a and K > 32 else 32
+
+
+def subtiles_per_sm(N, K, sms, register_a=True):
+    """launch_mstep_d(): contiguous event ranges of whole sub-tiles, NCL / 32 CTAs per range and NCL clusters; an SM runs
     ceil(CTAs / SMs) CTAs one after the other."""
     per = -(-N // sms)
     per = -(-per // KTE) * KTE
     gx = -(-N // per)
-    gy = -(-K // NCL)
-    return -(-(gx * gy) // sms) * (per // KTE)
+    c = ncl(K, register_a)
+    gy = -(-K // c)
+    return -(-(gx * (c // 32) * gy) // sms) * (per // KTE)
 
 
-def smem_bytes_per_subtile(D, register_a):
+def smem_bytes_per_subtile(D, K, register_a):
     """Shared-memory bytes one 32-event sub-tile of a CTA moves, per operand path."""
     mt, rows = tiles(D)
     nct = 128 * mt
-    b = mt * 2 * 2 * 3 * NCL * 16 * 2                 # wgmma B reads: per consumer, half and k-step gh, gl, gs (1 KB each)
-    gam = NCL * KTE * 4 + 3 * NCL * KTE * 2 + D * KTE * 4 + NCL * KTE * 4   # raw gamma read, images written, TMA writes
+    c = ncl(K, register_a)
+    hpc = 64 // c                                     # 64-row halves per consumer warpgroup
+    b = mt * hpc * 2 * 3 * c * 16 * 2                 # wgmma B reads: per consumer, half and k-step gh, gl, gs (c * 32 B each)
+    gam = c * KTE * 4 + 3 * c * KTE * 2 + D * KTE * 4 + c * KTE * 4   # raw gamma read, images written, TMA writes
     drains = nct * 32 * 4 * 2 // 4 + nct * 32 * 4 * 2 // 16    # racc read + write: exact group every 4, remainder every 16
     if register_a:
-        a = nct * 5 * 8 * 4                           # each consumer thread: 5 dimensions x 8 events of z
+        a = nct * (1 + 2 * hpc) * 8 * 4               # each consumer thread: 1 + 2 per half dimensions x 8 events of z
     else:
         a = rows * KTE * 2 * 2                        # builders write ph / pl
         a += mt * 2 * 2 * 3 * 64 * 16 * 2             # wgmma A reads: per half and k-step ah twice, al once (2 KB each)
@@ -81,13 +91,15 @@ def smem_bytes_per_subtile(D, register_a):
     return a + b + gam + drains
 
 
-def mma_flops_per_subtile(D):
+def mma_flops_per_subtile(D, K):
     mt, _ = tiles(D)
-    return mt * 2 * 2 * 3 * 64 * NCL * 16 * 2        # per consumer warpgroup 2 halves x 2 k-steps x 3 m64n32k16
+    c = ncl(K)
+    return mt * (64 // c) * 2 * 3 * 64 * c * 16 * 2  # per consumer warpgroup: halves x 2 k-steps x 3 m64n{c}k16
 
 
-def hgmma_count(lib, D):
-    """HGMMA instructions in mstep_tc_kernel<D> of a library (cuobjdump -sass), or None when cuobjdump is missing."""
+def hgmma_count(lib, D, K):
+    """HGMMA instructions in the mstep_tc_kernel<D, NCL> that runs at K (any NCL in a library that has one template argument),
+    from cuobjdump -sass, or None when cuobjdump is missing."""
     tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     if not os.path.exists(tool):
         return None
@@ -96,7 +108,7 @@ def hgmma_count(lib, D):
     for ln in out.splitlines():
         m = re.search(r"Function : (\S+)", ln)
         if m:
-            inside = re.search(rf"mstep_tc_kernelILi{D}E", m.group(1)) is not None
+            inside = re.search(rf"mstep_tc_kernelILi{D}E(Li{ncl(K)}E)?E", m.group(1)) is not None
             continue
         if inside and "HGMMA" in ln and "gdesc[URZ]" not in ln:     # (ptxas's empty HGMMA of a lone commit does no work)
             count += 1
@@ -145,12 +157,14 @@ def main():
     for shape in a.shapes.split(","):
         N, D, K = SHAPES[shape]
         n_sub = subtiles_per_sm(N, K, sms)
+        n_sub_staged = subtiles_per_sm(N, K, sms, register_a=False)
         clk = max_mhz * 1e3                           # clocks per ms
         model = dict(
-            tensor_floor_ms=round(n_sub * mma_flops_per_subtile(D) / 4096 / clk, 4),
-            smem_model_staged_ms=round(n_sub * smem_bytes_per_subtile(D, False) / 128 / clk, 4),
-            smem_model_register_a_ms=round(n_sub * smem_bytes_per_subtile(D, True) / 128 / clk, 4),
-            smem_bytes_per_subtile=dict(staged=smem_bytes_per_subtile(D, False), register_a=smem_bytes_per_subtile(D, True)))
+            clusters_per_cta=ncl(K),
+            tensor_floor_ms=round(n_sub * mma_flops_per_subtile(D, K) / 4096 / clk, 4),
+            smem_model_staged_ms=round(n_sub_staged * smem_bytes_per_subtile(D, K, False) / 128 / clk, 4),
+            smem_model_register_a_ms=round(n_sub * smem_bytes_per_subtile(D, K, True) / 128 / clk, 4),
+            smem_bytes_per_subtile=dict(staged=smem_bytes_per_subtile(D, K, False), register_a=smem_bytes_per_subtile(D, K, True)))
         print(json.dumps(dict(shape=shape, subtiles_per_sm=n_sub, **model)), flush=True)
         for lib in a.libs:
             env = dict(os.environ)
@@ -165,7 +179,7 @@ def main():
                 continue
             res = json.loads(lines[-1])
             res["lib"] = os.path.basename(lib)
-            res["hgmma_in_kernel"] = hgmma_count(path, D)
+            res["hgmma_in_kernel"] = hgmma_count(path, D, K)
             print(json.dumps(res), flush=True)
 
 
