@@ -497,6 +497,8 @@ struct gmm_ctx {
     long long dev_finalize_launches = 0, dev_replays = 0;
     int fin_fault_iter = -1;     // option "finalize_fault_iter" (tests): that iteration of the next batch reports a failure
     bool params_partial = false; // gmm_mstep has updated N, means, R but not yet Rinv / constants / the operand (upload_params clears)
+    bool set_from_finalize = false;  // the host copy came from a finalisation (device or host): Rinv, constant, pi and the
+                                     // E-step operand were derived from R, not given (seed, gmm_set_clusters, order reduction)
     ScoreBuffers score;          // gmm_score: streaming buffers, allocated on first use
     long long score_chunk = 1 << 20;   // option "score_chunk": events per streamed chunk of gmm_score / gmm_score_stats
     ScoreStatsBuffers sstats;    // gmm_score_stats: chunk buffers, allocated on first use
@@ -587,6 +589,7 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
     if (int rc = check_path(c, K)) return rc;
     auto t0 = std::chrono::steady_clock::now();
     const bool from_outside = !with_finalize;          // seed / set_clusters / order reduction: avgvar may have changed
+    const bool from_R = with_constants;                // (with_constants is cleared below once the loop has done that work)
     c->estep_tensor_ready = false;
     if (use_tensor_estep(c, K)) {
         if (int rc = ensure_moments(c)) return rc;
@@ -639,6 +642,7 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
     }
     c->cur_K = K;
     c->params_partial = false;
+    c->set_from_finalize = from_R;
     c->memcpy_ms +=std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return GMM_OK;
 }
@@ -1385,6 +1389,7 @@ static int run_dev_iterations(gmm_ctx* c, int K, int iters, float* ll_prev) {
     const int first_bad = h_bad[2], code = h_bad[3];
     if (first_bad < 0) {
         scatter_param_set(c, K);
+        c->set_from_finalize = true;
         if (ll_prev) *ll_prev = (float)h_ll[(iters - 1) & 1];
         return GMM_OK;
     }
@@ -1399,10 +1404,12 @@ static int run_dev_iterations(gmm_ctx* c, int K, int iters, float* ll_prev) {
         scatter_param_set(c, K);
     }
     c->iterations -= iters - first_bad;
-    // A set left by the device finalisation is rebuilt as the host path builds it after its own finalisation: inverse,
-    // constant, pi and the E-step operand from ONE factorisation of R (the device set is bit-identical to it); refactorising
-    // the stored float Rinv would hand the E-step a slightly different operand.
-    if (int rc = upload_params(c, K, /*with_constants=*/first_bad > 0)) return rc;
+    // A set left by a finalisation (this batch's device set, or at first_bad == 0 the set an earlier device batch or host
+    // iteration finalised) is rebuilt as the host path builds it after its own finalisation: inverse, constant, pi and the
+    // E-step operand from ONE factorisation of R (the device set is bit-identical to it); refactorising the stored float
+    // Rinv would hand the E-step a slightly different operand.  A set that came from outside (seed, gmm_set_clusters, order
+    // reduction) keeps its Rinv, as the host path did when it was uploaded.
+    if (int rc = upload_params(c, K, /*with_constants=*/first_bad > 0 || c->set_from_finalize)) return rc;
     if (int rc = zero_stats(c, K)) return rc;
     if (int rc = run_estep(c, K)) return rc;
     float prev = 0.f;

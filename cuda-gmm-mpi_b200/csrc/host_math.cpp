@@ -173,7 +173,9 @@ void finalize_cluster(const double* stats, const double* shift, int k, int D, cl
         const double inv = 1.0 / (double)Nf;
         for (int i = 0; i < D; i++)
             for (int j = 0; j <= i; j++) {
-                double cov = (Nf >= 1.0f) ? s[feat2(D, i, j)] - m[i] * s[1 + j] : 0.0;   // kernel :658-668
+                // kernel :658-668; the product is fused with the subtraction explicitly, as finalize_params_kernel fuses it
+                // (bit identity of the two finalisations must not hang on whether this compiler contracts the line)
+                double cov = (Nf >= 1.0f) ? std::fma(-m[i], s[1 + j], s[feat2(D, i, j)]) : 0.0;
                 if (i == j) cov += c->avgvar[k];                                      // kernel :673-675
                 const float v = (float)(cov * inv);                                   // gaussian.cu:664-667
                 R[i * D + j] = v;

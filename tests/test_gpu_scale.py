@@ -260,12 +260,18 @@ def _run_iterations(pkg, ev, K, n, finalize, fault=None, em=False):
     return got, ll, fp, got2, ll2, fp2
 
 
+def _assert_bit_identical(a, b, K, la, lb):
+    assert la == lb
+    for f in ("N", "pi", "constant", "means", "R", "Rinv", "memberships"):
+        np.testing.assert_array_equal(getattr(a, f)[:K], getattr(b, f)[:K], err_msg=f)
+
+
 @pytest.mark.parametrize("shape", [(30_000, 8, 6), (20_000, 16, 20), (25_000, 24, 64), (9_000, 24, 100)])
 def test_device_finalisation_equals_host_finalisation(loaded, shape):
     """Option "finalize": the one-kernel device-side step between the reduced statistics and the next E-step (N, means, R,
-    inverse, constants, pi, E-step operand) against the host finalisation of the same library — same arithmetic, so the
-    two runs agree far inside the run-level tolerance — through gmm_em_iterations and through gmm_em (K > 64 included:
-    two operand passes)."""
+    inverse, constants, pi, E-step operand) against the host finalisation of the same library — the same operations in the
+    same order, so the two runs agree bit for bit — through gmm_em_iterations and through gmm_em (K > 64 included: two
+    operand passes)."""
     pkg = loaded
     N, D, K = shape
     n = 6
@@ -277,9 +283,7 @@ def test_device_finalisation_equals_host_finalisation(loaded, shape):
         assert fp_d["device_finalize_launches"] == n and fp_d["host_replays"] == 0
         assert fp2_d["device_finalize_launches"] == n + 2
         for a, b, la, lb in ((dev, host, ll_d, ll_h), (dev2, host2, ll2_d, ll2_h)):
-            assert abs(la - lb) <= 2e-6 * abs(lb)
-            assert_params_close(a, b, K, rtol_N=2e-5)
-            np.testing.assert_allclose(a.memberships, b.memberships, rtol=0, atol=2e-5)
+            _assert_bit_identical(a, b, K, la, lb)
 
 
 @pytest.mark.parametrize("fault", [0, 3, 5])
@@ -296,6 +300,4 @@ def test_device_finalisation_replay_on_the_host(loaded, fault):
         assert fp["host_replays"] == 1 and fp["device_finalize_launches"] == n
         assert fp2["device_finalize_launches"] == n and fp2["host_replays"] == 1     # second batch: host path
         for a, b, la, lb in ((rep, host, ll_r, ll_h), (rep2, host2, ll2_r, ll2_h)):
-            assert abs(la - lb) <= 2e-6 * abs(lb)
-            assert_params_close(a, b, K, rtol_N=2e-5)
-            np.testing.assert_allclose(a.memberships, b.memberships, rtol=0, atol=2e-5)
+            _assert_bit_identical(a, b, K, la, lb)
