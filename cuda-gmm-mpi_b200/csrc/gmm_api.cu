@@ -505,6 +505,13 @@ struct gmm_ctx {
     KmeansBuffers kmeans;        // gmm_seed_kmeans: allocated on first use
     SampleBuffers sample;        // gmm_sample: parameter block, allocated on first use
     ConditionBuffers cond;       // gmm_condition: parameter block and imputation buffers, allocated on first use
+    // gmm_set_weights: per-event weights of the shard, used by the E-step log-likelihood and the M-step statistics
+    float* d_w = nullptr;        // [memb_pitch], zero beyond n (allocated on the first call)
+    bool weighted = false;       // d_w is in effect
+    double w_total = 0;          // global sum of the weights (the N of the default epsilon and of the Rissanen score)
+    double w_scale = 1;          // the global largest weight (the tensor M-step divides the weights by it)
+    bool w_tensor_ok = true;     // the weights' dynamic range fits the tensor M-step (kWeightRangeTc)
+    bool seeding = false;        // gmm_seed_kmeans: its M-steps ignore the weights
 };
 
 namespace gmm {
@@ -563,10 +570,22 @@ static int default_host_threads(int ranks_on_box) {
 static int estep_path_of(const gmm_ctx* c) { return c->estep_path >= 0 ? c->estep_path : c->path; }
 static int mstep_path_of(const gmm_ctx* c) { return c->mstep_path >= 0 ? c->mstep_path : c->path; }
 static bool use_tensor_estep(const gmm_ctx* c, int K) { return estep_path_of(c) != GMM_PATH_SIMT && c->n > 0 && tc_estep_supported(c->D, K); }
+// Weights of the shard for the E- and M-step kernels (NULL: unit weights; seeding ignores them).
+static const float* step_weights(const gmm_ctx* c) { return c->weighted && !c->seeding ? c->d_w : nullptr; }
+// Largest dynamic range max w / min positive w of the weights that the tensor M-step serves.  A weight whose scaled value
+// is not 1 moves a whole group of confident events off the points the operand's fixed-point part holds exactly, and their
+// common FP16 rounding then biases the statistics: the CPU emulation (tests/test_weights_error_model.py, DESIGN §5.11)
+// leaves a quarter of the per-cluster bar with two values 1 and 1.4 at the widest legal data range.  So the tensor M-step
+// serves one positive value (a constant factor, zeros allowed); any other weights are served by the FP64 SIMT M-step.
+// Only the steps of the context's own shard read the weights (run_mstep_accumulate); gmm_score_stats and
+// gmm_condition_stats choose their M-step without them.
+constexpr double kWeightRangeTc = 1.0;
 // (the tensor M-step also needs the data range to fit its fixed-point operand budget: known once the moments are)
 static bool use_tensor_mstep(const gmm_ctx* c, int K) {
     return mstep_path_of(c) != GMM_PATH_SIMT && c->n > 0 && tc_mstep_supported(c->D, K) && (!c->have_shift || tc_mstep_ready(c->tc));
 }
+// N of the default epsilon and of the Rissanen score: the number of events, or the sum of the weights
+static double em_count(const gmm_ctx* c) { return c->weighted ? c->w_total : (double)c->n_global; }
 // GMM_PATH_TENSOR never degrades silently: the M-step (the covariance contraction) must be covered.
 static int check_path(const gmm_ctx* c, int K) {
     if (mstep_path_of(c) == GMM_PATH_TENSOR && !tc_mstep_supported(c->D, K))
@@ -652,15 +671,17 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
 // shard's or a gmm_score_stats chunk's with the context's D and d_epack; a gmm_condition_stats chunk's with the observed
 // dimensions and its marginal block)
 template <int D>
-static void launch_estep_simt_d(gmm_ctx* c, int K, const float* epack, const float* xs, int n, float* memb, size_t pitch, double* ll) {
+static void launch_estep_simt_d(gmm_ctx* c, int K, const float* epack, const float* xs, int n, float* memb, size_t pitch, double* ll,
+                                const float* w) {
     const int blocks = (n + kEstepThreads - 1) / kEstepThreads;
-    estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, epack, memb, pitch, ll);
+    if (w) estep_simt_kernel<D, true><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, epack, memb, pitch, ll, w);
+    else estep_simt_kernel<D><<<blocks, kEstepThreads, 0, c->stream>>>(xs, pitch, n, K, epack, memb, pitch, ll);
 }
 static int launch_estep_simt_on(gmm_ctx* c, int D, int K, const float* epack, const float* xs, int n, float* memb, size_t pitch,
-                                double* ll) {
+                                double* ll, const float* w = nullptr) {
     if (n == 0) return GMM_OK;
     switch (D) {
-#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K, epack, xs, n, memb, pitch, ll); break;
+#define GMM_CASE(d) case d: launch_estep_simt_d<d>(c, K, epack, xs, n, memb, pitch, ll, w); break;
         GMM_CASE(1) GMM_CASE(2) GMM_CASE(3) GMM_CASE(4) GMM_CASE(5) GMM_CASE(6) GMM_CASE(7) GMM_CASE(8)
         GMM_CASE(9) GMM_CASE(10) GMM_CASE(11) GMM_CASE(12) GMM_CASE(13) GMM_CASE(14) GMM_CASE(15) GMM_CASE(16)
         GMM_CASE(17) GMM_CASE(18) GMM_CASE(19) GMM_CASE(20) GMM_CASE(21) GMM_CASE(22) GMM_CASE(23) GMM_CASE(24)
@@ -672,7 +693,8 @@ static int launch_estep_simt_on(gmm_ctx* c, int D, int K, const float* epack, co
     return GMM_OK;
 }
 static int launch_estep_simt(gmm_ctx* c, int K) {
-    return launch_estep_simt_on(c, c->D, K, c->d_epack, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F);
+    return launch_estep_simt_on(c, c->D, K, c->d_epack, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats + (size_t)K * c->F,
+                                step_weights(c));
 }
 
 // SIMT scoring of io.n rows of D coordinates against the epack records `epack` (gmm_score: the context's D and d_epack;
@@ -697,9 +719,11 @@ static int launch_score_simt(gmm_ctx* c, int D, int K, const float* epack, const
     return GMM_OK;
 }
 
-// FP64 SIMT M-step over n events of the SoA copy xs and the responsibilities memb (both [..][pitch]), adding into stats
+// FP64 SIMT M-step over n events of the SoA copy xs and the responsibilities memb (both [..][pitch]), adding into stats;
+// w (optional): per-event weights
 template <int JMAX, int CPT>
-static int launch_mstep_simt_t(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats) {
+static int launch_mstep_simt_t(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats,
+                               const float* w) {
     constexpr int FP = 16 * JMAX, KT = 16 * CPT, GS = KT + 2;
     const size_t smem = sizeof(double) * (size_t)(kMstepTE * FP + kMstepTE * GS + kMstepTE * GMM_MAX_DIMENSIONS) +
                         sizeof(short) * 2 * FP;
@@ -707,6 +731,7 @@ static int launch_mstep_simt_t(gmm_ctx* c, int K, const float* xs, int n, const 
     static bool attr_set[64] = {false};
     if (c->device >= 64 || !attr_set[c->device]) {
         CUDA_TRY(cudaFuncSetAttribute(mstep_simt_kernel<JMAX, CPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        CUDA_TRY(cudaFuncSetAttribute(mstep_simt_kernel<JMAX, CPT, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         if (c->device < 64) attr_set[c->device] = true;
     }
     int gx = c->num_sms;
@@ -715,15 +740,17 @@ static int launch_mstep_simt_t(gmm_ctx* c, int K, const float* xs, int n, const 
     if (per < kMstepTE) per = kMstepTE;
     gx = (n + per - 1) / per;
     dim3 grid(gx, (K + KT - 1) / KT);
-    mstep_simt_kernel<JMAX, CPT><<<grid, kMstepThreads, smem, c->stream>>>(xs, pitch, n, c->D, K, memb, pitch, c->d_shift, stats, per);
+    if (w) mstep_simt_kernel<JMAX, CPT, true><<<grid, kMstepThreads, smem, c->stream>>>(xs, pitch, n, c->D, K, memb, pitch, c->d_shift, stats, per, w);
+    else mstep_simt_kernel<JMAX, CPT><<<grid, kMstepThreads, smem, c->stream>>>(xs, pitch, n, c->D, K, memb, pitch, c->d_shift, stats, per);
     CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
-static int launch_mstep_simt_on(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats) {
+static int launch_mstep_simt_on(gmm_ctx* c, int K, const float* xs, int n, const float* memb, size_t pitch, double* stats,
+                                const float* w = nullptr) {
     if (n == 0) return GMM_OK;
     const int F = c->F;
     const int cpt = K <= 16 ? 1 : (K <= 32 ? 2 : 4);
-#define GMM_MS(j, p) return launch_mstep_simt_t<j, p>(c, K, xs, n, memb, pitch, stats)
+#define GMM_MS(j, p) return launch_mstep_simt_t<j, p>(c, K, xs, n, memb, pitch, stats, w)
     if (F <= 48) {
         if (cpt == 1) GMM_MS(3, 1);
         if (cpt == 2) GMM_MS(3, 2);
@@ -743,7 +770,7 @@ static int launch_mstep_simt_on(gmm_ctx* c, int K, const float* xs, int n, const
 #undef GMM_MS
 }
 static int launch_mstep_simt(gmm_ctx* c, int K) {
-    return launch_mstep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats);
+    return launch_mstep_simt_on(c, K, c->d_x_soa, c->n, c->d_memb, c->memb_pitch, c->d_stats, step_weights(c));
 }
 
 static int zero_stats(gmm_ctx* c, int K) {
@@ -756,7 +783,7 @@ static int zero_stats(gmm_ctx* c, int K) {
 // log-likelihood added to stats[K*F].
 static int run_estep(gmm_ctx* c, int K) {
     timer_begin(c, c->t_estep);
-    int rc = c->estep_tensor_ready ? tc_launch_estep(c->tc, K, c->d_stats + (size_t)K * c->F, c->stream)
+    int rc = c->estep_tensor_ready ? tc_launch_estep(c->tc, K, c->d_stats + (size_t)K * c->F, c->stream, step_weights(c))
                                    : launch_estep_simt(c, K);
     timer_end(c, c->t_estep);
     c->memb_valid = (rc == GMM_OK);
@@ -767,11 +794,18 @@ static int run_estep(gmm_ctx* c, int K) {
 static int run_mstep_accumulate(gmm_ctx* c, int K) {
     // Both M-step kernels ADD into stats[0 .. K*F): whatever an earlier call left there (column moments, seed rows,
     // the reduced statistics of a finished gmm_em / gmm_mstep) has to go; the log-likelihood slot [K*F] stays.
+    const float* w = step_weights(c);
+    if (w && !c->w_tensor_ok && mstep_path_of(c) == GMM_PATH_TENSOR)
+        return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the weights' dynamic range (max / min positive) exceeds what the "
+                                 "tensor M-step's fixed-point operand serves");
     if (c->stats_clean_K != K) CUDA_TRY(cudaMemsetAsync(c->d_stats, 0, sizeof(double) * (size_t)K * c->F, c->stream));
     c->stats_clean_K = 0;
     timer_begin(c, c->t_mstep);
     int rc;
-    if (use_tensor_mstep(c, K)) { rc = tc_launch_mstep(c->tc, K, c->d_stats, c->stream); c->mstep_tensor++; }
+    if (use_tensor_mstep(c, K) && (!w || c->w_tensor_ok)) {
+        rc = tc_launch_mstep(c->tc, K, c->d_stats, c->stream, w, w ? c->w_scale : 1.0);
+        c->mstep_tensor++;
+    }
     else { rc = launch_mstep_simt(c, K); c->mstep_simt++; }
     timer_end(c, c->t_mstep);
     return rc;
@@ -1048,6 +1082,7 @@ void gmm_destroy(gmm_ctx* c) {
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
     cudaFree(c->d_pset[0]); cudaFree(c->d_pset[1]); cudaFree(c->d_avgvar); cudaFree(c->d_bad); cudaFree(c->d_llprev);
+    cudaFree(c->d_w);
     if (c->h_pset) cudaFreeHost(c->h_pset);
     if (c->h_small) cudaFreeHost(c->h_small);
     if (c->h_epack) cudaFreeHost(c->h_epack);
@@ -1256,6 +1291,65 @@ int gmm_set_clusters(gmm_ctx* c, int K, const clusters_t* in) {
     return GMM_OK;
 }
 
+// Per-event weights of the shard.  Validated and agreed before anything changes: every rank learns the global sum, the
+// largest weight and the smallest positive one, whether any rank saw an invalid weight and how many ranks passed weights
+// from two all-reduces, so a rejected call leaves the weights in effect on every rank, and a call that passes NULL on some
+// ranks only is rejected on all of them (the ranks would otherwise disagree on N = sum w, and so on gmm_em's stopping test).
+int gmm_set_weights(gmm_ctx* c, const float* weights, double* total_out) {
+    if (!c) return fail(GMM_ERR_ARG, "gmm_set_weights: null context");
+    CUDA_TRY(cudaSetDevice(c->device));
+    double sum = 0.0, wmax = 0.0, wmin = std::numeric_limits<double>::infinity(), bad = 0.0, has = weights ? 1.0 : 0.0;
+    if (weights) {
+        for (int e = 0; e < c->n; e++) {
+            const float w = weights[e];
+            if (!(w >= 0.0f) || !std::isfinite(w)) { bad = 1.0; continue; }
+            sum += (double)w;
+            wmax = std::max(wmax, (double)w);
+            if (w > 0.0f) wmin = std::min(wmin, (double)w);
+        }
+    }
+    if (c->nranks > 1) {
+        double h[5] = {sum, bad, has, wmax, -wmin};   // summed | maximised
+        double* d_h = nullptr;
+        CUDA_TRY(cudaMalloc(&d_h, sizeof(h)));
+        ncclResult_t r = ncclSuccess;
+        cudaError_t e = cudaMemcpyAsync(d_h, h, sizeof(h), cudaMemcpyHostToDevice, c->stream);
+        if (e == cudaSuccess) {
+            r = nccl().AllReduce(d_h, d_h, 3, ncclDouble, ncclSum, c->comm, c->stream);
+            if (r == ncclSuccess) r = nccl().AllReduce(d_h + 3, d_h + 3, 2, ncclDouble, ncclMax, c->comm, c->stream);
+            if (r == ncclSuccess) e = cudaMemcpyAsync(h, d_h, sizeof(h), cudaMemcpyDeviceToHost, c->stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        }
+        cudaFree(d_h);
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+        if (e != cudaSuccess) return fail(GMM_ERR_CUDA, std::string("gmm_set_weights: ") + cudaGetErrorString(e));
+        sum = h[0]; bad = h[1]; has = h[2]; wmax = h[3]; wmin = -h[4];
+        if (has != 0.0 && has != (double)c->nranks)
+            return fail(GMM_ERR_ARG, "gmm_set_weights: weights on some ranks and NULL on others (pass weights on all ranks, or NULL on all)");
+    }
+    if (!weights) {
+        c->weighted = false;
+        c->memb_valid = false;
+        if (total_out) *total_out = (double)c->n_global;
+        return GMM_OK;
+    }
+    if (bad != 0.0) return fail(GMM_ERR_ARG, "gmm_set_weights: a weight is negative or not finite");
+    if (!(sum > 0.0)) return fail(GMM_ERR_ARG, "gmm_set_weights: the weights sum to zero");
+    if (!c->d_w) {
+        CUDA_TRY(cudaMalloc(&c->d_w, sizeof(float) * c->memb_pitch));
+        CUDA_TRY(cudaMemsetAsync(c->d_w, 0, sizeof(float) * c->memb_pitch, c->stream));   // the M-step reads whole 32-event tiles
+    }
+    if (c->n > 0) CUDA_TRY(cudaMemcpyAsync(c->d_w, weights, sizeof(float) * (size_t)c->n, cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    c->w_scale = wmax;
+    c->w_tensor_ok = wmax <= kWeightRangeTc * wmin;
+    c->w_total = sum;
+    c->weighted = true;
+    c->memb_valid = false;
+    if (total_out) *total_out = sum;
+    return GMM_OK;
+}
+
 int gmm_get_clusters(gmm_ctx* c, int K, clusters_t* out, int with_memberships) {
     if (int rc = check_K(c, K, "gmm_get_clusters")) return rc;
     if (!out) return fail(GMM_ERR_ARG, "gmm_get_clusters: null clusters");
@@ -1459,7 +1553,7 @@ int gmm_em(gmm_ctx* c, int K, int min_iters, int max_iters, float epsilon, float
     if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_em: parameters for this K have not been set (gmm_seed / gmm_set_clusters)");
     CUDA_TRY(cudaSetDevice(c->device));
     if (int rc = ensure_moments(c)) return rc;
-    if (epsilon < 0) epsilon = em_epsilon(c->D, c->n_global);
+    if (epsilon < 0) epsilon = em_epsilon(c->D, em_count(c));
     const size_t ll_idx = (size_t)K * c->F;
     if (int rc = zero_stats(c, K)) return rc;
     if (int rc = run_estep(c, K)) return rc;                 // initial E-step, gaussian.cu:487-523
@@ -2079,6 +2173,11 @@ int gmm_seed_kmeans(gmm_ctx* c, int K, int max_iter, unsigned long long seed, cl
     KmeansBuffers& b = c->kmeans;
     const int D = c->D, F = c->F;
     c->memb_valid = false;
+    struct Unweighted {                                    // seeding ignores the weights (gmm.h), on every return path
+        gmm_ctx* c;
+        explicit Unweighted(gmm_ctx* cc) : c(cc) { c->seeding = true; }
+        ~Unweighted() { c->seeding = false; }
+    } unweighted(c);
     if (int rc = kmeanspp_run(c, K, seed)) return rc;
     std::vector<float> cent((size_t)K * D);
     CUDA_TRY(cudaMemcpyAsync(cent.data(), b.d_centres, sizeof(float) * cent.size(), cudaMemcpyDeviceToHost, c->stream));
@@ -2715,7 +2814,7 @@ int gmm_fit(gmm_ctx* c, int K0, int target_K, int min_iters, int max_iters, clus
         if (int rc = gmm_seed(c, K0, nullptr)) return rc;
         c->fit_seed_ms += ms_since(t0);
     }
-    const float epsilon = em_epsilon(D, c->n_global);
+    const float epsilon = em_epsilon(D, em_count(c));
     float min_rissanen = 0;
     int ideal = K0;
     if (saved->memberships && !c->d_memb_saved && c->n > 0)
@@ -2723,7 +2822,7 @@ int gmm_fit(gmm_ctx* c, int K0, int target_K, int min_iters, int max_iters, clus
     for (int K = K0; K >= stop_number;) {
         float likelihood; int iters;
         if (int rc = gmm_em(c, K, min_iters, max_iters, epsilon, &likelihood, &iters)) return rc;
-        const float r = rissanen(likelihood, K, D, c->n_global);          // :826
+        const float r = rissanen(likelihood, K, D, em_count(c));          // :826
         if (c->verbose && c->rank == 0) std::printf("K=%d loglik=%e Rissanen Score: %e\n", K, likelihood, r);
         if (K == K0 || (r < min_rissanen && target_K == 0) || K == target_K) {   // :839
             const auto t0 = now();

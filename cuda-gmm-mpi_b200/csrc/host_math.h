@@ -51,8 +51,9 @@ void seed_from_moments(const double* sum_x, const double* sum_x2, long long N, i
 // Row index of seed event c (gaussian.cu:110-120: (int)(c*seed), seed in float).
 long long seed_event_index(int c, int K, long long N);
 
-float rissanen(float loglik, int K, int D, long long N);
-float em_epsilon(int D, long long N);
+// N: the number of events, or the sum of the weights (gmm_set_weights); (float)N as the reference forms it.
+float rissanen(float loglik, int K, int D, double N);
+float em_epsilon(int D, double N);
 
 // One order-reduction step (gaussian.cu:860-907).  Returns new K.  The K(K-1)/2 trial merges run on the caller's
 // worker team when `pfor` is given (pfor(n, fn) calls fn(0..n-1) in parallel), else on an OpenMP team of num_threads.

@@ -35,12 +35,13 @@ __device__ __forceinline__ double warp_sum(double v) {
 // go to memb while a running max / sum-exp is kept (online log-sum-exp); the
 // second sweep re-reads them (L2-resident: the block wrote them microseconds
 // ago) and stores exp(l - denom).  The per-event log-likelihood terms are
-// reduced in double and added to *ll_out.
+// reduced in double and added to *ll_out.  WT (gmm_set_weights): the event's term is w[e] * denom; the
+// responsibilities do not depend on the weights.
 // ---------------------------------------------------------------------------
-template <int D>
+template <int D, bool WT = false>
 __global__ void __launch_bounds__(kEstepThreads)
 estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, const float* __restrict__ epack,
-                  float* __restrict__ memb, size_t pitch, double* __restrict__ ll_out) {
+                  float* __restrict__ memb, size_t pitch, double* __restrict__ ll_out, const float* __restrict__ w = nullptr) {
     constexpr int STRIDE = epack_stride_c(D);
     constexpr int COEF = (D + 3) & ~3;
     constexpr int NCOEF = D * (D + 1) / 2;
@@ -91,7 +92,9 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
             *g = expf(*g - denom);                          // estep2 :498-501
         }
     }
-    double ll = valid ? (double)denom : 0.0;
+    double ll;
+    if constexpr (WT) ll = valid ? (double)w[e] * (double)denom : 0.0;
+    else ll = valid ? (double)denom : 0.0;
     ll = warp_sum(ll);
     if ((threadIdx.x & 31) == 0) sred[threadIdx.x >> 5] = ll;
     __syncthreads();
@@ -193,15 +196,16 @@ score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __
 // the statistics are exact up to the final double rounding) — it is the
 // accuracy anchor for the wgmma path, not the fast path.
 // Thread layout: 256 threads = 16 (cluster groups of CPT) x 16 (feature lanes,
-// JMAX features each); TE events per shared-memory tile.
+// JMAX features each); TE events per shared-memory tile.  WT (gmm_set_weights): the responsibility operand is
+// g * w[e], formed in double (exact: a product of two floats).
 // ---------------------------------------------------------------------------
 constexpr int kMstepThreads = 256;
 constexpr int kMstepTE = 32;
 
-template <int JMAX, int CPT>
+template <int JMAX, int CPT, bool WT = false>
 __global__ void __launch_bounds__(kMstepThreads, 1)
 mstep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int D, int K, const float* __restrict__ memb, size_t pitch,
-                  const double* __restrict__ shift, double* __restrict__ stats, int events_per_block) {
+                  const double* __restrict__ shift, double* __restrict__ stats, int events_per_block, const float* __restrict__ w = nullptr) {
     constexpr int FP = 16 * JMAX;          // padded feature count
     constexpr int KT = 16 * CPT;           // clusters per block
     constexpr int GS = KT + 2;             // padded row of the gamma tile (16-byte aligned rows)
@@ -247,7 +251,8 @@ mstep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int D, int
             const int kk = idx / kMstepTE, t = idx % kMstepTE;
             const long long e = e0 + t;
             const int k = k0 + kk;
-            gt[t * GS + kk] = (k < K && e < eend) ? (double)memb[(size_t)k * pitch + e] : 0.0;
+            if constexpr (WT) gt[t * GS + kk] = (k < K && e < eend) ? (double)memb[(size_t)k * pitch + e] * (double)w[e] : 0.0;
+            else gt[t * GS + kk] = (k < K && e < eend) ? (double)memb[(size_t)k * pitch + e] : 0.0;
         }
         __syncthreads();
         for (int idx = tid; idx < kMstepTE * FP; idx += kMstepThreads) {      // features

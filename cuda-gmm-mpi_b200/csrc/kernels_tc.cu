@@ -244,10 +244,16 @@ __device__ __forceinline__ bool chain2_starts(int i, int mt) { return i == 0 || 
 // opmap[row] = a | b << 8: the operand factors of row `row` (mstep_row_layout; codes >= kRowOne: rows of the ones block).
 // Grid (ranges * 64 / NCL, ceil(K / NCL)): CTA x = range * 64 / NCL + part, so with NCL = 64 the two CTAs of a range run in
 // the same wave and the second reader of every z / gamma tile finds it in L2.
-template <int D, int NCL>
+// WT (gmm_set_weights): the responsibility operand is g * w^, w^ = 1 for w = w_max (the largest weight), else w * w_inv
+// (w_inv = 1 / w_max rounded; no division in the 56-register pool), so w^ is at most 1 and the product lies in [0, 1] like g:
+// the split below and its bit budget are unchanged.  The library runs this instance for weights of one positive value only
+// (gmm_api.cu kWeightRangeTc), where w^ is exactly 0 or 1 and the operand is the unweighted one with rows removed.  wts: [>= 32 * ceil(n / 32)] floats, zero beyond n.
+// mstep_tc_finalize_kernel multiplies the sums by w_max.
+template <int D, int NCL, bool WT = false>
 __global__ void __launch_bounds__(MCfg<D, NCL>::THREADS, 1)
 mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_g, int n, int K,
-                float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic, const int* __restrict__ opmap) {
+                float* __restrict__ scratch, int events_per_cta, const __grid_constant__ MMagic magic, const int* __restrict__ opmap,
+                const float* __restrict__ wts, float w_max, float w_inv) {
     using C = MCfg<D, NCL>;
     constexpr int HPC = C::HPC;
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -306,6 +312,16 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
             for (int i = 0; i < nsub; i++) {
                 const int rs = i % kNRAW, rph = (i / kNRAW) & 1;
                 const int os = i % kNST, oph = (i / kNST) & 1;
+                // every item of this thread has the 8-event chunk ce = (bt & 31) >> 3 (items step by 96): its 8 weights are
+                // loaded and scaled once per sub-tile, before the wait
+                [[maybe_unused]] float wv[8];
+                if constexpr (WT) {
+                    const float4* wp = reinterpret_cast<const float4*>(wts + e_begin + i * kTE + 8 * ((bt & 31) >> 3));
+                    const float4 wa = __ldg(wp), wb = __ldg(wp + 1);
+                    wv[0] = wa.x; wv[1] = wa.y; wv[2] = wa.z; wv[3] = wa.w; wv[4] = wb.x; wv[5] = wb.y; wv[6] = wb.z; wv[7] = wb.w;
+#pragma unroll
+                    for (int v = 0; v < 8; v++) wv[v] = wv[v] == w_max ? 1.0f : __fmul_rn(wv[v], w_inv);
+                }
                 mbar_wait_parked(&raw_full[rs], rph, 200);
                 mbar_wait_parked(&op_empty[os], oph ^ 1, 200);
                 // K-major B image: byte(k, e) = (k/8)*512 + (e/8)*128 + (k%8)*16 + (e%8)*2      (LBO = 128, SBO = 512)
@@ -320,8 +336,12 @@ mstep_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant_
                     const uint8_t* grow = smem + C::OFF_RAWG + rs * C::RAWG + k * (kTE * 4);
                     const float4 a = *reinterpret_cast<const float4*>(grow + (((2 * ce) ^ (k & 7)) << 4));
                     const float4 b = *reinterpret_cast<const float4*>(grow + (((2 * ce + 1) ^ (k & 7)) << 4));
-                    const float g[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+                    float g[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
                     dep += a.x + b.x;
+                    if constexpr (WT) {
+#pragma unroll
+                        for (int v = 0; v < 8; v++) g[v] = __fmul_rn(g[v], wv[v]);
+                    }
                     float hi[8], lo[8];
 #pragma unroll
                     for (int v = 0; v < 8; v++) {              // gh = 16 * round(64 g) (0 .. 1024), gl = 1024 g - gh, both from the exact product
@@ -516,9 +536,10 @@ __global__ void standardise_soa_kernel(const float* __restrict__ xs, float* __re
 
 // Reduce the per-CTA FP32 partials in double, undo the operand scaling and write the packed statistics.
 // rowmap[row] = (packed statistic index or -1, dimension i, dimension j) of operand row `row` (tc_row_info).
+// wscale: the largest weight, which the weighted M-step divided the weights by (1 without weights: no bit changes).
 __global__ void __launch_bounds__(256)
 mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, int K, int F, const int3* __restrict__ rowmap,
-                         const double* __restrict__ scale, double* __restrict__ stats) {
+                         const double* __restrict__ scale, double* __restrict__ stats, double wscale) {
     // one block per operand row; thread -> (cluster column, eighth of the CTAs): 128-byte coalesced reads
     constexpr int NQ = 256 / kNCL;
     __shared__ double part[NQ][kNCL];
@@ -526,7 +547,7 @@ mstep_tc_finalize_kernel(const float* __restrict__ scratch, int ncta_x, int MT, 
     if (rm.x < 0) return;
     const int mt = blockIdx.x / 128, row = blockIdx.x % 128;
     const int col = threadIdx.x & (kNCL - 1), q = threadIdx.x / kNCL;
-    double fac = 1.0 / (double)kGammaScale;
+    double fac = wscale / (double)kGammaScale;
     if (rm.y >= 0) fac *= scale[rm.y];
     if (rm.z >= 0) fac *= scale[rm.z];
     for (int ty = 0; ty * kNCL < K; ty++) {
@@ -750,11 +771,12 @@ __device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], c
     }
 }
 
-template <int D, int NSG>
+template <int D, int NSG, bool WT = false>
 __global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
 estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
                 const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float* __restrict__ memb,
-                size_t pitch, int n, int K, double* __restrict__ ll_out, int mode, const float* den_in, float* den_out) {
+                size_t pitch, int n, int K, double* __restrict__ ll_out, int mode, const float* den_in, float* den_out,
+                const float* __restrict__ wts) {
     // K / NSG (= ceil(K / 16)) / b_img / ck / memb describe ONE pass of at most 64 clusters.  More than 64 clusters take 2P - 1 launches
     // for P passes, and every responsibility is written exactly once:
     //   mode 1 (passes 0 .. P-2)  log-denominator only: den_out[e] = ln(sum_k exp(logit)) (+ den_in[e] in log space), no stores
@@ -762,6 +784,7 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
     //                             pass, den_out[e] = the event's total log-denominator, log-likelihood
     //   mode 3 (passes 0 .. P-2)  responsibilities against the known total den_in[e]: no log-sum-exp
     //   mode 0                    single pass (K <= 64)
+    // WT (gmm_set_weights): the log-likelihood adds wts[e] * denominator; the responsibilities do not depend on the weights.
     using C = ECfg<D>;
     constexpr int CP = C::CP;
     extern __shared__ __align__(1024) uint8_t smem[];
@@ -858,7 +881,11 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
                     }
                     if (qd == 0) den_out[er[r]] = denom;
                 }
-                if (qd == 0 && er[r] < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
+                if constexpr (WT) {
+                    if (qd == 0 && er[r] < n && (mode == 0 || mode == 2)) ll_acc += (double)wts[er[r]] * (double)denom;
+                } else {
+                    if (qd == 0 && er[r] < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
+                }
             }
         }
         if (mode != 1 && GMM_ESTEP_CUT != 2) {
@@ -1714,18 +1741,23 @@ int tc_launch_finalize(TcState* t, int K, const double* d_stats, const float* d_
 }
 
 template <int D>
-static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, cudaStream_t stream) {
+static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, const float* w,
+                          cudaStream_t stream) {
     using C = ECfg<D>;
     static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
-    // one instance per number of resident supergroups (1 .. 4) of a pass
-    static void (*const kern[C::MAXSG])(const float*, const uint8_t*, const float*, const float*, const float*, float*, size_t, int, int,
-                                        double*, int, const float*, float*) = {estep_tc_kernel<D, 1>, estep_tc_kernel<D, 2>,
-                                                                              estep_tc_kernel<D, 3>, estep_tc_kernel<D, 4>};
+    // one instance per number of resident supergroups (1 .. 4) of a pass, unweighted and weighted
+    using KernFn = void (*)(const float*, const uint8_t*, const float*, const float*, const float*, float*, size_t, int, int, double*, int,
+                            const float*, float*, const float*);
+    static const KernFn kern0[C::MAXSG] = {estep_tc_kernel<D, 1>, estep_tc_kernel<D, 2>, estep_tc_kernel<D, 3>, estep_tc_kernel<D, 4>};
+    static const KernFn kern1[C::MAXSG] = {estep_tc_kernel<D, 1, true>, estep_tc_kernel<D, 2, true>, estep_tc_kernel<D, 3, true>,
+                                           estep_tc_kernel<D, 4, true>};
     static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_estep) {
-        for (auto* k : kern) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern0) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern1) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_estep = true;
     }
+    const KernFn* kern = w ? kern1 : kern0;
     const int ntiles = (n + 127) / 128;
     int grid = t->num_sms;
     if (grid > ntiles) grid = ntiles;
@@ -1739,7 +1771,7 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
         const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
         kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
             x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f,
-            memb + (size_t)(64 * p) * pitch, pitch, n, Kp, d_ll, mode, den_in, den_out);
+            memb + (size_t)(64 * p) * pitch, pitch, n, Kp, d_ll, mode, den_in, den_out, w);
         return cudaGetLastError();
     };
     if (NP == 1) TC_CUDA_TRY(launch(0, 0, nullptr, nullptr));
@@ -1751,25 +1783,26 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
     return GMM_OK;
 }
 
-static int launch_estep_any(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, cudaStream_t stream) {
+static int launch_estep_any(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, const float* w,
+                            cudaStream_t stream) {
     if (!t || !t->emap_ok) return fail(GMM_ERR_STATE, "tensor E-step not initialised for this shape");
     switch (t->D) {
-        case 8: return launch_estep_d<8>(t, K, x, n, memb, pitch, den, d_ll, stream);
-        case 16: return launch_estep_d<16>(t, K, x, n, memb, pitch, den, d_ll, stream);
-        case 24: return launch_estep_d<24>(t, K, x, n, memb, pitch, den, d_ll, stream);
+        case 8: return launch_estep_d<8>(t, K, x, n, memb, pitch, den, d_ll, w, stream);
+        case 16: return launch_estep_d<16>(t, K, x, n, memb, pitch, den, d_ll, w, stream);
+        case 24: return launch_estep_d<24>(t, K, x, n, memb, pitch, den, d_ll, w, stream);
         default: return fail(GMM_ERR_ARG, "tensor E-step: unsupported D");
     }
 }
 
-int tc_launch_estep(TcState* t, int K, double* d_ll, cudaStream_t stream) {
+int tc_launch_estep(TcState* t, int K, double* d_ll, cudaStream_t stream, const float* d_w) {
     if (!t) return fail(GMM_ERR_STATE, "tensor E-step not initialised for this shape");
-    return launch_estep_any(t, K, t->d_x, t->n, t->d_memb, t->memb_pitch, t->d_den, d_ll, stream);
+    return launch_estep_any(t, K, t->d_x, t->n, t->d_memb, t->memb_pitch, t->d_den, d_ll, d_w, stream);
 }
 
 int tc_launch_estep_on(TcState* t, int K, const float* d_x_aos, int n, float* d_memb, size_t pitch, float* d_den, double* d_ll,
                        cudaStream_t stream) {
     if (n <= 0) return GMM_OK;
-    return launch_estep_any(t, K, d_x_aos, n, d_memb, pitch, d_den, d_ll, stream);
+    return launch_estep_any(t, K, d_x_aos, n, d_memb, pitch, d_den, d_ll, nullptr, stream);
 }
 
 template <int D>
@@ -1813,15 +1846,19 @@ int tc_launch_score(TcState* t, int K, const TcScoreIo& io, cudaStream_t stream)
 // K <= 32: one CTA per event range and 32 clusters.  K > 32: two CTAs per range and 64 clusters, each building half of the
 // feature rows (MCfg): the feature operand is built once per 64 clusters, and both CTAs read the range's tiles in one wave.
 template <int D>
-static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, cudaStream_t stream) {
+static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, const float* w,
+                          double wscale, cudaStream_t stream) {
     using C32 = MCfg<D, 32>;
     using C64 = MCfg<D, 64>;
     static_assert(C32::SMEM_BYTES <= 232448 && C64::SMEM_BYTES <= 232448, "shared memory budget");
     if (!t->attr_mstep) {
         TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
         TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
+        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
+        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
         t->attr_mstep = true;
     }
+    const float w_max = (float)wscale, w_inv = (float)(1.0 / wscale);
     int gx = t->num_sms;
     int per = (n + gx - 1) / gx;
     per = (per + kTE - 1) / kTE * kTE;
@@ -1830,34 +1867,40 @@ static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUte
     const int ncl = pair ? 64 : 32;
     const int gy = (K + ncl - 1) / ncl;
     if ((size_t)gx * gy * (ncl / kNCL) * C32::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
-    if (pair)
-        mstep_tc_kernel<D, 64><<<dim3(2 * gx, gy), C64::THREADS, C64::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap);
-    else
-        mstep_tc_kernel<D, 32><<<dim3(gx, gy), C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap);
+    const dim3 grid(pair ? 2 * gx : gx, gy);
+    if (pair) {
+        if (w) mstep_tc_kernel<D, 64, true><<<grid, C64::THREADS, C64::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, w, w_max, w_inv);
+        else mstep_tc_kernel<D, 64><<<grid, C64::THREADS, C64::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, nullptr, 1.0f, 1.0f);
+    } else {
+        if (w) mstep_tc_kernel<D, 32, true><<<grid, C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, w, w_max, w_inv);
+        else mstep_tc_kernel<D, 32><<<grid, C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, nullptr, 1.0f, 1.0f);
+    }
     TC_CUDA_TRY(cudaGetLastError());
-    mstep_tc_finalize_kernel<<<C32::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C32::MT, K, C32::F, t->d_rowmap, t->d_scale, d_stats);
+    mstep_tc_finalize_kernel<<<C32::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C32::MT, K, C32::F, t->d_rowmap, t->d_scale, d_stats,
+                                                                w ? wscale : 1.0);
     TC_CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
 
-static int launch_mstep_any(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, cudaStream_t stream) {
+static int launch_mstep_any(TcState* t, int K, const CUtensorMap& tm_x, const CUtensorMap& tm_g, int n, double* d_stats, const float* w,
+                            double wscale, cudaStream_t stream) {
     if (!t || !t->maps_ok) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
     if (!t->have_shift) return fail(GMM_ERR_STATE, "tensor-core M-step needs gmm_seed (shift/scale) first");
     if (!t->mstep_ready) return fail(GMM_ERR_STATE, "tensor-core M-step: the data range exceeds the fixed-point operand budget");
     switch (t->D) {
-        case 4: return launch_mstep_d<4>(t, K, tm_x, tm_g, n, d_stats, stream);
-        case 8: return launch_mstep_d<8>(t, K, tm_x, tm_g, n, d_stats, stream);
-        case 12: return launch_mstep_d<12>(t, K, tm_x, tm_g, n, d_stats, stream);
-        case 16: return launch_mstep_d<16>(t, K, tm_x, tm_g, n, d_stats, stream);
-        case 20: return launch_mstep_d<20>(t, K, tm_x, tm_g, n, d_stats, stream);
-        case 24: return launch_mstep_d<24>(t, K, tm_x, tm_g, n, d_stats, stream);
+        case 4: return launch_mstep_d<4>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
+        case 8: return launch_mstep_d<8>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
+        case 12: return launch_mstep_d<12>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
+        case 16: return launch_mstep_d<16>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
+        case 20: return launch_mstep_d<20>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
+        case 24: return launch_mstep_d<24>(t, K, tm_x, tm_g, n, d_stats, w, wscale, stream);
         default: return fail(GMM_ERR_ARG, "tensor-core M-step: unsupported D");
     }
 }
 
-int tc_launch_mstep(TcState* t, int K, double* d_stats, cudaStream_t stream) {
+int tc_launch_mstep(TcState* t, int K, double* d_stats, cudaStream_t stream, const float* d_w, double wscale) {
     if (!t) return fail(GMM_ERR_STATE, "tensor-core M-step not initialised for this shape");
-    return launch_mstep_any(t, K, t->tm_x, t->tm_g, t->n, d_stats, stream);
+    return launch_mstep_any(t, K, t->tm_x, t->tm_g, t->n, d_stats, d_w, wscale, stream);
 }
 
 int tc_launch_mstep_on(TcState* t, int K, const float* d_z, const float* d_memb, size_t pitch, int n, double* d_stats, cudaStream_t stream) {
@@ -1869,7 +1912,7 @@ int tc_launch_mstep_on(TcState* t, int K, const float* d_z, const float* d_memb,
         if (int rc = make_map_2d(&t->tm_cg, d_memb, (uint64_t)n, (uint64_t)t->Kmax, (uint64_t)pitch * 4, kTE, kNCL, /*swizzle128=*/true)) return rc;
         t->cmap_z = d_z; t->cmap_g = d_memb; t->cmap_pitch = pitch; t->cmap_n = n;
     }
-    return launch_mstep_any(t, K, t->tm_cx, t->tm_cg, n, d_stats, stream);
+    return launch_mstep_any(t, K, t->tm_cx, t->tm_cg, n, d_stats, nullptr, 1.0, stream);
 }
 
 const float* tc_shift_f(const TcState* t) { return t && t->have_shift ? t->d_shift_f : nullptr; }

@@ -37,7 +37,8 @@ int  tc_params_cluster(TcState*, const clusters_t* host, int k, int K);
 // (constants_cluster_spd): no second factorisation of the inverse.
 int  tc_params_cluster_w(TcState*, const clusters_t* host, int k, int K, const double* W);
 int  tc_params_commit(TcState*, int K, int bad, cudaStream_t stream);
-int  tc_launch_estep(TcState*, int K, double* d_ll, cudaStream_t stream);
+// d_w (optional): per-event weights of the shard ([n] floats): the log-likelihood adds w * denominator (gmm_set_weights).
+int  tc_launch_estep(TcState*, int K, double* d_ll, cudaStream_t stream, const float* d_w = nullptr);
 // Scoring of a chunk of new events ([n][D] on the device) against the resident operand of the current parameters
 // (score_tc_kernel): labels / max_resp / logp per event, ll += sum of logp, *flag = 1 when an event is outside the FP16
 // operand range.  run_*: per-event running state of the passes, n entries each (needed for K > 64 only).
@@ -66,7 +67,9 @@ size_t tc_param_set_off(int Kmax, int D, int which);
 int  tc_launch_finalize(TcState*, int K, const double* d_stats, const float* d_avgvar, float* d_set, double* d_ll, int* d_bad, int iter,
                         int fault_iter, cudaStream_t stream);
 // Accumulates sum_n g[k][n] * phi_f(x_n - shift) into d_stats[k*F + f] (double, original units).
-int  tc_launch_mstep(TcState*, int K, double* d_stats, cudaStream_t stream);
+// d_w (optional): per-event weights of the shard ([memb_pitch] floats, zero beyond n), wscale = the largest of them: the
+// sums are of w g phi.
+int  tc_launch_mstep(TcState*, int K, double* d_stats, cudaStream_t stream, const float* d_w = nullptr, double wscale = 1.0);
 
 // The same two steps on caller-owned buffers (gmm_score_stats: chunks of new events, nothing of the state's buffers is
 // written except the M-step's per-launch scratch).  pitch: row pitch in floats of memb (and of z), a multiple of 32.

@@ -70,6 +70,7 @@ def load_library():
     L.gmm_seed.argtypes = [C.c_void_p, C.c_int, _CP]
     L.gmm_seed_kmeans.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_ulonglong, _CP, _FP, _IP, _DP]
     L.gmm_set_clusters.argtypes = [C.c_void_p, C.c_int, _CP]
+    L.gmm_set_weights.argtypes = [C.c_void_p, C.c_void_p, _DP]
     L.gmm_get_clusters.argtypes = [C.c_void_p, C.c_int, _CP, C.c_int]
     L.gmm_estep.argtypes = [C.c_void_p, C.c_int, _FP]
     L.gmm_mstep.argtypes = [C.c_void_p, C.c_int]
@@ -264,6 +265,22 @@ class Engine:
     def set_clusters(self, K, cl):
         s = cl.struct()
         _check(self.lib.gmm_set_clusters(self.h, K, C.byref(s)))
+
+    def set_weights(self, w=None):
+        """Per-event weights of this shard (gmm_set_weights): float32 [n_local], finite, >= 0; None clears them.
+        Returns the global sum of the weights."""
+        ptr = None
+        if w is not None:
+            w = np.ascontiguousarray(w, np.float32)
+            if w.shape != (self.n,):
+                raise ValueError(f"weights must be [{self.n}], got {w.shape}")
+            ptr = w.ctypes.data if w.size else None
+            if ptr is None:                                 # an empty shard still sets (zero) weights
+                w = np.zeros(1, np.float32)
+                ptr = w.ctypes.data
+        total = C.c_double()
+        _check(self.lib.gmm_set_weights(self.h, ptr, C.byref(total)))
+        return total.value
 
     def get_clusters(self, K, out=None, with_memberships=False):
         out = out or self.new_clusters(with_memberships)

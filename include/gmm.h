@@ -177,6 +177,33 @@ int  gmm_seed_kmeans(gmm_ctx*, int K, int max_iter, unsigned long long seed,
 /* H2D of N,pi,constant,avgvar,means,R,Rinv (gaussian.cu:446-452, 935-941). */
 int  gmm_set_clusters(gmm_ctx*, int K, const clusters_t* host_in);
 
+/* Per-event weights of THIS shard ([n_local] floats, finite, >= 0), used by every later E-step log-likelihood and
+ * M-step statistic of the context's own shard.  NULL clears them (back to unit weights).  Collective with several
+ * ranks.  *total_out (may be NULL) = the global sum of the weights (n_global after NULL).
+ * Semantics: EM over the multiset in which event n appears w_n times, extended to real w >= 0 (integer weights give
+ * the EM of replicated rows):
+ *   - gmm_estep's log-likelihood is sum w logp; the M-step statistics of gmm_mstep, gmm_em, gmm_em_iterations (host
+ *     and device-side finalisation) and gmm_fit are S0 = sum w g, S1 = sum w g (x - s), S2 = sum w g (x - s)(x - s)^T;
+ *     everything after them (the all-reduce, N, pi = N / sum N, the N thresholds, the order reduction) is unchanged.
+ *   - gmm_em's default epsilon and gmm_fit's Rissanen score use N = sum w in place of n_global (the public
+ *     gmm_host_epsilon / gmm_host_rissanen do not change).
+ *   - ignored: gmm_seed and gmm_seed_kmeans (initialisation only), the memberships (posteriors do not depend on the
+ *     weights), and gmm_score, gmm_score_stats, gmm_sample, gmm_condition, gmm_condition_stats (they do not read the shard;
+ *     their kernels, outputs and profiles are the same with and without weights set).
+ *   - kernels: weighted instances of the context's own E- and M-step kernels.  The wgmma M-step divides the weights by
+ *     the largest one; it serves weights whose positive values are all equal (dynamic range
+ *     max w / min positive w = 1: a constant factor, zeros allowed), the range its fixed-point operand holds to the
+ *     per-cluster accuracy bar (DESIGN.md §5.11).  Other weights run the FP64 SIMT M-step, or fail with GMM_ERR_ARG at the next M-step when "mstep_path" (or "path") is
+ *     GMM_PATH_TENSOR.  The decision uses the global extremes: every rank takes the same path.
+ *   - setting or clearing weights marks the memberships stale, as gmm_set_clusters does: gmm_mstep and
+ *     gmm_em_iterations then need a gmm_estep first.  gmm_upload_events / gmm_upload_events_file keep the weights (they
+ *     belong to event positions).
+ * Device memory: one [n_local rounded up to 32] float buffer, allocated on the first call, freed by gmm_destroy.
+ * Errors: a weight that is NaN, infinite or negative on any rank, a global sum of 0, or weights on some ranks and NULL on
+ * others -> GMM_ERR_ARG on every rank, and the weights in effect before the call stay unchanged; a failed collective ->
+ * GMM_ERR_NCCL.                                      */
+int  gmm_set_weights(gmm_ctx*, const float* weights, double* total_out);
+
 /* D2H of the parameters, optionally the memberships of THIS shard into
  * host_out->memberships laid out [K][n_local] (gaussian.cu:761-774).       */
 int  gmm_get_clusters(gmm_ctx*, int K, clusters_t* host_out, int with_memberships);
