@@ -35,6 +35,7 @@
 #include "kernels_sample.cuh"
 #include "kernels_seed.cuh"
 #include "kernels_tc.cuh"
+#include "kernels_vb.cuh"
 
 namespace gmm {
 
@@ -512,6 +513,12 @@ struct gmm_ctx {
     double w_scale = 1;          // the global largest weight (the tensor M-step divides the weights by it)
     bool w_tensor_ok = true;     // the weights' dynamic range fits the tensor M-step (kWeightRangeTc)
     bool seeding = false;        // gmm_seed_kmeans: its M-steps ignore the weights
+    // gmm_vb_em: block partials of the responsibility entropy (resp_entropy_kernel), allocated on first use
+    double* d_ent = nullptr;     // [ent_blocks + 1]: the partials, then the rank's sum for the all-reduce
+    double* h_ent = nullptr;     // pinned mirror
+    int ent_blocks = 0;
+    PhaseTimer t_entropy;
+    double vb_final_ms = 0, vb_wall_ms = 0;   // gmm_get_vb_profile
 };
 
 namespace gmm {
@@ -536,7 +543,7 @@ static void timer_collect(gmm_ctx* c, PhaseTimer& t) {          // call after a 
 }
 static void collect_all(gmm_ctx* c) {
     timer_collect(c, c->t_estep); timer_collect(c, c->t_mstep); timer_collect(c, c->t_reduce); timer_collect(c, c->t_fused);
-    timer_collect(c, c->t_final);
+    timer_collect(c, c->t_final); timer_collect(c, c->t_entropy);
 }
 
 static void bind_host(gmm_ctx* c) {
@@ -1083,6 +1090,8 @@ void gmm_destroy(gmm_ctx* c) {
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
     cudaFree(c->d_pset[0]); cudaFree(c->d_pset[1]); cudaFree(c->d_avgvar); cudaFree(c->d_bad); cudaFree(c->d_llprev);
     cudaFree(c->d_w);
+    cudaFree(c->d_ent);
+    if (c->h_ent) cudaFreeHost(c->h_ent);
     if (c->h_pset) cudaFreeHost(c->h_pset);
     if (c->h_small) cudaFreeHost(c->h_small);
     if (c->h_epack) cudaFreeHost(c->h_epack);
@@ -2216,6 +2225,169 @@ int gmm_seed_kmeans(gmm_ctx* c, int K, int max_iter, unsigned long long seed, cl
     if (centres_out) std::memcpy(centres_out, cent.data(), sizeof(float) * cent.size());
     if (iters_out) *iters_out = iters;
     if (inertia_out) *inertia_out = inertia;
+    return GMM_OK;
+}
+
+// ---- variational Bayesian mixture (gmm_vb_em) -----------------------------------------------------------------------------
+// The default prior moments from the context's own M-step at K = 1 on unit responsibilities: the Lloyd assignment kernel
+// with one centre writes a row of ones (and zeros in the rows the tensor M-step's cluster boxes read), and the weights
+// enter as in every M-step.  mean = s + S1 / S0, covariance = (S2 - S1 S1^T / S0) / (S0 - 1): np.cov's ddof = 1, with
+// denominator sum w - 1 under weights.  Overwrites the device memberships.
+static int vb_default_moments(gmm_ctx* c, double* mean, double* cov) {
+    if (int rc = kmeans_buffers(c)) return rc;
+    const int D = c->D, Kw = std::min((c->Kmax + 7) / 8 * 8, 32);
+    CUDA_TRY(cudaMemsetAsync(c->kmeans.d_centres, 0, sizeof(float) * D, c->stream));
+    c->memb_valid = false;
+    if (int rc = kmeans_assign_launch(c, 1, Kw)) return rc;
+    if (int rc = run_mstep_accumulate(c, 1)) return rc;
+    if (int rc = reduce_stats_to_host(c, 1)) return rc;
+    const double* s = c->h_stats;
+    const double S0 = s[0];
+    if (!(S0 > 1.0)) return fail(GMM_ERR_ARG, "gmm_vb_em: the default prior covariance needs a total weight above 1");
+    for (int i = 0; i < D; i++) {
+        mean[i] = c->shift[i] + s[1 + i] / S0;
+        for (int j = 0; j <= i; j++) cov[i * D + j] = cov[j * D + i] = (s[feat2(D, i, j)] - s[1 + i] * s[1 + j] / S0) / (S0 - 1.0);
+    }
+    return GMM_OK;
+}
+
+// resp_entropy_kernel over the current memberships, its partials queued to the pinned mirror (read after the next stream
+// synchronisation by vb_entropy_sum).
+static int vb_entropy_launch(gmm_ctx* c, int K, int* grid_out) {
+    if (!c->d_ent) {
+        c->ent_blocks = kEntropyBlocksPerSm * c->num_sms;
+        CUDA_TRY(cudaMalloc(&c->d_ent, sizeof(double) * (size_t)(c->ent_blocks + 1)));
+        CUDA_TRY(cudaMallocHost(&c->h_ent, sizeof(double) * (size_t)(c->ent_blocks + 1)));
+    }
+    const int nq = (c->n + 3) / 4;
+    const int grid = std::max(1, std::min(c->ent_blocks, (nq + kEntropyThreads - 1) / kEntropyThreads));
+    *grid_out = c->n > 0 ? grid : 0;
+    if (c->n == 0) return GMM_OK;
+    const float* w = step_weights(c);
+    timer_begin(c, c->t_entropy);
+    if (w) resp_entropy_kernel<true><<<grid, kEntropyThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, c->n, K, w, c->d_ent);
+    else resp_entropy_kernel<false><<<grid, kEntropyThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, c->n, K, nullptr, c->d_ent);
+    timer_end(c, c->t_entropy);
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(c->h_ent, c->d_ent, sizeof(double) * grid, cudaMemcpyDeviceToHost, c->stream));
+    return GMM_OK;
+}
+
+// sum_n w_n sum_k g ln g over all ranks: this rank's partials in block order, then one ncclAllReduce of one double.
+static int vb_entropy_sum(gmm_ctx* c, int grid, double* out) {
+    double s = 0.0;
+    for (int i = 0; i < grid; i++) s += c->h_ent[i];
+    if (c->nranks > 1) {
+        double* slot = c->d_ent + c->ent_blocks;
+        c->h_ent[c->ent_blocks] = s;
+        CUDA_TRY(cudaMemcpyAsync(slot, c->h_ent + c->ent_blocks, sizeof(double), cudaMemcpyHostToDevice, c->stream));
+        ncclResult_t r = nccl().AllReduce(slot, slot, 1, ncclDouble, ncclSum, c->comm, c->stream);
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+        CUDA_TRY(cudaMemcpyAsync(c->h_ent + c->ent_blocks, slot, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));
+        s = c->h_ent[c->ent_blocks];
+    }
+    *out = s;
+    return GMM_OK;
+}
+
+// VB M-step from the reduced statistics in h_stats: the per-cluster part on the finalisation's worker team (K >= 8), the
+// weights and the bound serially, then the parameter set uploaded as gmm_set_clusters uploads one (Rinv and constant kept).
+static int vb_finalize_upload(gmm_ctx* c, int K, const VbPrior& p, std::vector<VbCluster>& cl, gmm_vb_posterior* post, double* bound) {
+    auto t0 = std::chrono::steady_clock::now();
+    const int D = c->D;
+    const std::function<void(int)> per_cluster = [&](int k) { vb_finalize_cluster(c->h_stats, c->shift, k, D, p, &c->host, &cl[(size_t)k]); };
+    if (K >= 8) {
+        if (!c->pool) c->pool = new HostPool(c->host_threads);
+        else c->pool->resize(c->host_threads);
+        c->pool->run(K, per_cluster);
+    } else {
+        for (int k = 0; k < K; k++) per_cluster(k);
+    }
+    int bad = -1;
+    const int rc = vb_finalize_weights(K, D, p, cl.data(), &c->host, post, bound, &bad);
+    c->vb_final_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (rc) {
+        c->memb_valid = false;
+        return fail(GMM_ERR_STATE, "gmm_vb_em: the covariance of component " + std::to_string(bad) + " is not positive definite in float");
+    }
+    return upload_params(c, K);
+}
+
+int gmm_vb_em(gmm_ctx* c, int K, const gmm_vb_prior* prior, int min_iters, int max_iters, double tol, clusters_t* host_out,
+              gmm_vb_posterior* post_out, double* lower_bound_out, double* lower_bounds_out, int* iters_out, int* converged_out) {
+    if (int rc = check_K(c, K, "gmm_vb_em")) return rc;
+    if (!prior) return fail(GMM_ERR_ARG, "gmm_vb_em: NULL prior");
+    if (min_iters < 0 || max_iters < min_iters) return fail(GMM_ERR_ARG, "gmm_vb_em: need 0 <= min_iters <= max_iters");
+    if (!(tol >= 0.0)) return fail(GMM_ERR_ARG, "gmm_vb_em: tol must be >= 0");
+    const int D = c->D;
+    VbPrior p;
+    if (int rc = vb_resolve_prior(prior, K, D, &p)) return rc;
+    std::vector<double> mean((size_t)D, 0.0), cov((size_t)D * D, 0.0);
+    for (int d = 0; d < D; d++) cov[(size_t)d * D + d] = 1.0;
+    // the caller's moments are checked before anything runs (a NULL one stands in as 0 / I until the default is known)
+    if (int rc = vb_set_prior_moments(prior->mean ? prior->mean : mean.data(), prior->covariance ? prior->covariance : cov.data(), D, &p))
+        return rc;
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_vb_em: parameters for this K have not been set (gmm_seed / gmm_set_clusters)");
+    if (c->params_partial) return fail(GMM_ERR_STATE, "gmm_vb_em: called between gmm_mstep and gmm_constants");
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    if (int rc = ensure_moments(c)) return rc;
+    if (!prior->mean || !prior->covariance) {
+        if (int rc = vb_default_moments(c, mean.data(), cov.data())) return rc;
+        if (int rc = vb_set_prior_moments(prior->mean ? prior->mean : mean.data(), prior->covariance ? prior->covariance : cov.data(), D, &p))
+            return rc;
+    }
+    std::vector<VbCluster> cl((size_t)K);
+    double bound_par = 0.0, lb = -std::numeric_limits<double>::infinity(), lb_prev = lb;
+    // g0 under the starting set, posterior 0 from it (sklearn's _initialize)
+    if (int rc = zero_stats(c, K)) return rc;
+    if (int rc = run_estep(c, K)) return rc;
+    if (int rc = run_mstep_accumulate(c, K)) return rc;
+    if (int rc = reduce_stats_to_host(c, K)) return rc;
+    if (int rc = vb_finalize_upload(c, K, p, cl, post_out, &bound_par)) return rc;
+    int iters = 0, converged = 0;
+    for (int i = 1; i <= max_iters; i++) {
+        if (int rc = zero_stats(c, K)) return rc;
+        if (int rc = run_estep(c, K)) return rc;
+        if (int rc = run_mstep_accumulate(c, K)) return rc;
+        // the bound of iteration i is used by the tol test of iterations i and i + 1
+        const bool need_bound = lower_bounds_out != nullptr || i >= min_iters - 1;
+        int grid = 0;
+        if (need_bound)
+            if (int rc = vb_entropy_launch(c, K, &grid)) return rc;
+        if (int rc = reduce_stats_to_host(c, K)) return rc;
+        if (int rc = vb_finalize_upload(c, K, p, cl, post_out, &bound_par)) return rc;
+        iters = i;
+        c->iterations++;
+        if (need_bound) {
+            double ent = 0.0;
+            if (int rc = vb_entropy_sum(c, grid, &ent)) return rc;
+            lb = -ent + bound_par;
+            if (lower_bounds_out) lower_bounds_out[i - 1] = lb;
+        }
+        if (i >= min_iters && std::fabs(lb - lb_prev) < tol) { converged = 1; break; }
+        lb_prev = lb;
+    }
+    // the memberships of the final posterior (sklearn's last _e_step)
+    if (int rc = zero_stats(c, K)) return rc;
+    if (int rc = run_estep(c, K)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    collect_all(c);
+    c->vb_wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    if (host_out) copy_params(host_out, &c->host, K, D);
+    if (lower_bound_out) *lower_bound_out = lb;
+    if (iters_out) *iters_out = iters;
+    if (converged_out) *converged_out = converged;
+    return GMM_OK;
+}
+
+int gmm_get_vb_profile(gmm_ctx* c, double out[3], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_vb_profile: bad argument");
+    cudaStreamSynchronize(c->stream);
+    collect_all(c);
+    out[0] = c->t_entropy.total_ms; out[1] = c->vb_final_ms; out[2] = c->vb_wall_ms;
+    if (reset) { c->t_entropy.total_ms = 0; c->vb_final_ms = c->vb_wall_ms = 0; }
     return GMM_OK;
 }
 

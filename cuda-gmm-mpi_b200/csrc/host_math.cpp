@@ -4,6 +4,7 @@
 // (file:line cited per function); the code is written from scratch.
 #include "host_math.h"
 
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -106,10 +107,11 @@ bool reverse_cholesky(const float* R, int D, double (*U)[GMM_MAX_DIMENSIONS], do
     return true;
 }
 
-bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out */) {
+bool constants_cluster_spd(int k, int D, clusters_t* c, double* W /* [D][D] out */, double* half_ln_det) {
     double U[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS];
     double ld;
     if (!reverse_cholesky(c->R + (size_t)k * D * D, D, U, &ld)) return false;
+    if (half_ln_det) *half_ln_det = ld;
     // W = U^-1 (upper triangular), column by column: W[i][j] = -(sum_{m=i+1..j} U[i][m] W[m][j]) / U[i][i]
     for (int j = 0; j < D; j++) {
         for (int i = D - 1; i > j; i--) W[i * D + j] = 0.0;
@@ -447,6 +449,187 @@ void condition_stats_cluster(double* row, int D, const int* obs, int n_obs, cons
     }
 }
 
+// ---------------------------------------------------------------------------
+// Variational Bayesian mixture (gmm_vb_em; sklearn's BayesianGaussianMixture with covariance_type='full', restated in
+// float64 numpy by tests/_vb_ref.py).
+// ---------------------------------------------------------------------------
+double digamma(double x) {
+    // psi(x) = psi(x + m) - sum_{j<m} 1/(x + j) until x + m >= 10, then the asymptotic series in 1/x^2 (Abramowitz and
+    // Stegun 6.3.18) to the x^-14 term, whose truncation error at x >= 10 is about 2e-17 relative.
+    if (!(x > 0.0)) return std::numeric_limits<double>::quiet_NaN();
+    double acc = 0.0;
+    while (x < 10.0) { acc -= 1.0 / x; x += 1.0; }
+    const double r = 1.0 / x, r2 = r * r;
+    const double series =
+        r2 * (1.0 / 12 - r2 * (1.0 / 120 - r2 * (1.0 / 252 - r2 * (1.0 / 240 - r2 * (1.0 / 132 - r2 * (691.0 / 32760 - r2 / 12))))));
+    return acc + std::log(x) - 0.5 * r - series;
+}
+
+int vb_resolve_prior(const gmm_vb_prior* p, int K, int D, VbPrior* out) {
+    if (!p) return fail(GMM_ERR_ARG, "VB prior: NULL prior");
+    if (p->weight_prior_type != GMM_VB_DIRICHLET_PROCESS && p->weight_prior_type != GMM_VB_DIRICHLET_DISTRIBUTION)
+        return fail(GMM_ERR_ARG, "VB prior: unknown weight_prior_type");
+    if (!std::isfinite(p->weight_concentration)) return fail(GMM_ERR_ARG, "VB prior: weight_concentration is not finite");
+    if (!std::isfinite(p->mean_precision)) return fail(GMM_ERR_ARG, "VB prior: mean_precision is not finite");
+    if (std::isnan(p->dof) || std::isinf(p->dof) || (p->dof > 0.0 && p->dof <= D - 1.0))
+        return fail(GMM_ERR_ARG, "VB prior: dof must be > D - 1 (or <= 0 for the default D)");
+    if (std::isnan(p->reg_covar) || std::isinf(p->reg_covar)) return fail(GMM_ERR_ARG, "VB prior: reg_covar is not finite");
+    out->type = p->weight_prior_type;
+    out->gamma0 = p->weight_concentration > 0.0 ? p->weight_concentration : 1.0 / K;
+    out->beta0 = p->mean_precision > 0.0 ? p->mean_precision : 1.0;
+    out->nu0 = p->dof > 0.0 ? p->dof : (double)D;
+    out->reg = p->reg_covar >= 0.0 ? p->reg_covar : 1e-6;
+    return GMM_OK;
+}
+
+// Cholesky A = L L^T of a symmetric [D][D] double matrix (lower triangle read); *half_ld = sum ln L_jj.  false = not
+// positive definite.
+static bool cholesky_half_ld(const double* A, int D, double* half_ld) {
+    double L[GMM_MAX_DIMENSIONS][GMM_MAX_DIMENSIONS];
+    double ld = 0.0;
+    for (int j = 0; j < D; j++) {
+        double s = A[j * D + j];
+        for (int t = 0; t < j; t++) s -= L[j][t] * L[j][t];
+        if (!(s > 0.0) || !std::isfinite(s)) return false;
+        L[j][j] = std::sqrt(s);
+        ld += std::log(L[j][j]);
+        for (int i = j + 1; i < D; i++) {
+            double v = A[i * D + j];
+            for (int t = 0; t < j; t++) v -= L[i][t] * L[j][t];
+            L[i][j] = v / L[j][j];
+        }
+    }
+    *half_ld = ld;
+    return true;
+}
+
+int vb_set_prior_moments(const double* mean, const double* cov, int D, VbPrior* out) {
+    for (int d = 0; d < D; d++)
+        if (!std::isfinite(mean[d])) return fail(GMM_ERR_ARG, "VB prior: mean is not finite");
+    double amax = 0.0;
+    for (int i = 0; i < D * D; i++) {
+        if (!std::isfinite(cov[i])) return fail(GMM_ERR_ARG, "VB prior: covariance is not finite");
+        amax = std::max(amax, std::fabs(cov[i]));
+    }
+    for (int i = 0; i < D; i++)
+        for (int j = 0; j < i; j++)
+            if (std::fabs(cov[i * D + j] - cov[j * D + i]) > 1e-12 * amax)
+                return fail(GMM_ERR_ARG, "VB prior: covariance is not symmetric");
+    double hl;
+    if (!cholesky_half_ld(cov, D, &hl)) return fail(GMM_ERR_ARG, "VB prior: covariance is not positive definite");
+    std::memcpy(out->m0, mean, sizeof(double) * D);
+    std::memcpy(out->psi0, cov, sizeof(double) * D * D);
+    return GMM_OK;
+}
+
+void vb_finalize_cluster(const double* stats, const double* shift, int k, int D, const VbPrior& p, clusters_t* c, VbCluster* out) {
+    const int F = num_features(D);
+    const double* s = stats + (size_t)k * F;
+    const double S0 = s[0];
+    const double nk = S0 + 10.0 * std::numeric_limits<double>::epsilon();      // sklearn: resp.sum(0) + 10 eps
+    double xk[GMM_MAX_DIMENSIONS], dd[GMM_MAX_DIMENSIONS], m[GMM_MAX_DIMENSIONS], df[GMM_MAX_DIMENSIONS];
+    for (int d = 0; d < D; d++) {
+        xk[d] = (S0 * shift[d] + s[1 + d]) / nk;                                 // an empty component gets xk = 0
+        dd[d] = xk[d] - shift[d];
+    }
+    const double beta = p.beta0 + nk, nu = p.nu0 + nk, wmix = nk * p.beta0 / beta;
+    for (int d = 0; d < D; d++) {
+        m[d] = (p.beta0 * p.m0[d] + nk * xk[d]) / beta;
+        df[d] = xk[d] - p.m0[d];
+    }
+    double C[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS];
+    for (int i = 0; i < D; i++)
+        for (int j = 0; j <= i; j++) {
+            // nk sk = sum g (x - xk)(x - xk)^T + nk reg I, with sum g (x - xk)(x - xk)^T = S2 - S1 dd^T - dd S1^T + S0 dd dd^T
+            double q = s[feat2(D, i, j)] - s[1 + i] * dd[j] - dd[i] * s[1 + j] + S0 * dd[i] * dd[j];
+            if (i == j) q += nk * p.reg;
+            const double v = (p.psi0[i * D + j] + q + wmix * df[i] * df[j]) / nu;
+            C[i * D + j] = C[j * D + i] = v;
+        }
+    c->N[k] = (float)nk;
+    float* mu = c->means + (size_t)k * D;
+    float* R = c->R + (size_t)k * D * D;
+    for (int d = 0; d < D; d++) mu[d] = (float)m[d];
+    for (int i = 0; i < D * D; i++) R[i] = (float)C[i];
+    out->nk = nk; out->beta = beta; out->nu = nu;
+    double W[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS], hl_f = 0.0, hl_d = 0.0;
+    out->ok = constants_cluster_spd(k, D, c, W, &hl_f) && cholesky_half_ld(C, D, &hl_d);
+    if (!out->ok) { out->offset = out->log_wishart = 0.0; return; }
+    double sum_psi = 0.0, sum_lg = 0.0;
+    for (int i = 0; i < D; i++) {
+        sum_psi += digamma(0.5 * (nu - i));
+        sum_lg += std::lgamma(0.5 * (nu - i));
+    }
+    out->offset = -0.5 * D * std::log(2.0 * kPi) - hl_f - 0.5 * D * std::log(nu) + 0.5 * (D * std::log(2.0) + sum_psi) - 0.5 * D / beta;
+    const double ldpc = -hl_d - 0.5 * D * std::log(nu);                         // ln det of sklearn's precisions_cholesky_
+    out->log_wishart = -(nu * ldpc + nu * D * 0.5 * std::log(2.0) + sum_lg);
+}
+
+int vb_finalize_weights(int K, int D, const VbPrior& p, const VbCluster* cl, clusters_t* c, gmm_vb_posterior* post, double* bound,
+                        int* bad_k) {
+    for (int k = 0; k < K; k++)
+        if (!cl[k].ok) { if (bad_k) *bad_k = k; return -1; }
+    std::vector<double> a(K), b(K), elog(K), w(K);
+    double log_norm_weight = 0.0, wsum = 0.0;
+    if (p.type == GMM_VB_DIRICHLET_PROCESS) {
+        double tail = 0.0;                                  // sum_{j > k} nk_j, accumulated from the last component down
+        for (int k = K - 1; k >= 0; k--) {
+            a[k] = 1.0 + cl[k].nk;
+            b[k] = p.gamma0 + tail;
+            tail += cl[k].nk;
+        }
+        double run = 0.0, prod = 1.0;
+        for (int k = 0; k < K; k++) {
+            const double ds = digamma(a[k] + b[k]);
+            elog[k] = digamma(a[k]) - ds + run;
+            run += digamma(b[k]) - ds;
+            w[k] = a[k] / (a[k] + b[k]) * prod;
+            prod *= b[k] / (a[k] + b[k]);
+            log_norm_weight -= std::lgamma(a[k]) + std::lgamma(b[k]) - std::lgamma(a[k] + b[k]);   // -sum betaln(a, b)
+        }
+    } else {
+        double sa = 0.0, slg = 0.0;
+        for (int k = 0; k < K; k++) {
+            a[k] = p.gamma0 + cl[k].nk;
+            sa += a[k];
+            slg += std::lgamma(a[k]);
+        }
+        const double ds = digamma(sa);
+        for (int k = 0; k < K; k++) {
+            elog[k] = digamma(a[k]) - ds;
+            w[k] = a[k];
+        }
+        log_norm_weight = std::lgamma(sa) - slg;
+    }
+    for (int k = 0; k < K; k++) wsum += w[k];
+    double log_wishart = 0.0, sum_lb = 0.0;
+    for (int k = 0; k < K; k++) {
+        w[k] /= wsum;
+        const float pf = std::max((float)w[k], std::numeric_limits<float>::min());
+        c->pi[k] = pf;
+        // constant + ln pi = offset + E[ln pi]: ln pi in double of the float pi (the tensor E-step packs constant + ln pi
+        // with ln pi in double, the SIMT E-step with logf; both round to float)
+        c->constant[k] = (float)(cl[k].offset + elog[k] - std::log((double)pf));
+        log_wishart += cl[k].log_wishart;
+        sum_lb += std::log(cl[k].beta);
+    }
+    if (bound) *bound = -log_wishart - log_norm_weight - 0.5 * D * sum_lb;
+    if (post) {
+        for (int k = 0; k < K; k++) {
+            if (post->weights) post->weights[k] = w[k];
+            if (post->weight_concentration) {
+                post->weight_concentration[k] = a[k];
+                if (p.type == GMM_VB_DIRICHLET_PROCESS) post->weight_concentration[K + k] = b[k];
+            }
+            if (post->mean_precision) post->mean_precision[k] = cl[k].beta;
+            if (post->dof) post->dof[k] = cl[k].nu;
+        }
+        if (post->mean_prior) std::memcpy(post->mean_prior, p.m0, sizeof(double) * D);
+        if (post->covariance_prior) std::memcpy(post->covariance_prior, p.psi0, sizeof(double) * D * D);
+    }
+    return 0;
+}
+
 }  // namespace gmm
 
 // ---------------------------------------------------------------------------
@@ -473,6 +656,28 @@ int gmm_host_finalize(const double* stats, const double* shift, int K, int D, cl
     if (!stats || !shift || !inout || K < 1 || K > GMM_MAX_CLUSTERS || D < 1 || D > GMM_MAX_DIMENSIONS)
         return gmm::fail(GMM_ERR_ARG, "gmm_host_finalize: bad argument");
     gmm::finalize_from_stats(stats, shift, K, D, inout, 1);
+    return GMM_OK;
+}
+
+int gmm_host_vb_finalize(const double* stats, const double* shift, int K, int D, const gmm_vb_prior* prior,
+                         clusters_t* out, gmm_vb_posterior* post_out, double* bound_out) {
+    if (!stats || !shift || !out || K < 1 || K > GMM_MAX_CLUSTERS || D < 1 || D > GMM_MAX_DIMENSIONS)
+        return gmm::fail(GMM_ERR_ARG, "gmm_host_vb_finalize: bad argument");
+    gmm::VbPrior p;
+    if (int rc = gmm::vb_resolve_prior(prior, K, D, &p)) return rc;
+    if (!prior->mean || !prior->covariance) return gmm::fail(GMM_ERR_ARG, "gmm_host_vb_finalize: the prior's mean and covariance are required");
+    if (int rc = gmm::vb_set_prior_moments(prior->mean, prior->covariance, D, &p)) return rc;
+    std::vector<gmm::VbCluster> cl((size_t)K);
+    for (int k = 0; k < K; k++) gmm::vb_finalize_cluster(stats, shift, k, D, p, out, &cl[(size_t)k]);
+    int bad = -1;
+    if (gmm::vb_finalize_weights(K, D, p, cl.data(), out, post_out, bound_out, &bad))
+        return gmm::fail(GMM_ERR_STATE, "gmm_host_vb_finalize: the covariance of component " + std::to_string(bad) + " is not positive definite");
+    return GMM_OK;
+}
+
+int gmm_host_digamma(const double* x, double* out, long long n) {
+    if ((!x || !out) && n > 0) return gmm::fail(GMM_ERR_ARG, "gmm_host_digamma: bad argument");
+    for (long long i = 0; i < n; i++) out[i] = gmm::digamma(x[i]);
     return GMM_OK;
 }
 

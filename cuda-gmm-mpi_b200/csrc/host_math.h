@@ -34,7 +34,7 @@ void constants_from_R(int K, int D, clusters_t* c, int num_threads);
 void constants_cluster(int k, int D, clusters_t* c);
 // Same results for a symmetric positive definite R from one (reverse) Cholesky factorisation; also returns the
 // upper-triangular W with Rinv = W^T W.  false = not positive definite, nothing written (use constants_cluster).
-bool constants_cluster_spd(int k, int D, clusters_t* c, double* W);
+bool constants_cluster_spd(int k, int D, clusters_t* c, double* W, double* half_ln_det = nullptr);
 // The factorisation behind it: R = U U^T with U upper triangular, in double from the float R [D][D] (row-major, the
 // off-diagonal pairs averaged), pivots from the last one up; *ld = sum ln U_jj.  Only U's upper triangle is written.
 // false = not positive definite (a pivot <= 0 or not finite).
@@ -83,5 +83,35 @@ bool condition_cluster(const clusters_t* c, int k, int D, const int* obs, int n_
 // as condition_cluster returns them in double.
 void condition_stats_cluster(double* row, int D, const int* obs, int n_obs, const int* mis, int nm, const float* mu,
                              const double* shift, const double* g, const double* cm);
+
+// ---- variational Bayesian mixture (gmm_vb_em, gmm_host_vb_finalize; gmm.h) ----
+double digamma(double x);
+// The prior with its defaults applied (m0 / Psi0 by the caller: the events' moments when the user passes NULL).
+struct VbPrior {
+    int type;                                   // GMM_VB_*
+    double gamma0, beta0, nu0, reg;
+    double m0[GMM_MAX_DIMENSIONS];
+    double psi0[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS];
+};
+// Checks the scalars of `p` and applies their defaults (m0 / Psi0 are copied by vb_set_prior_moments).  GMM_OK or
+// GMM_ERR_ARG with the message set.
+int vb_resolve_prior(const gmm_vb_prior* p, int K, int D, VbPrior* out);
+// m0 and Psi0 (row-major [D][D]): finite, Psi0 symmetric and positive definite; GMM_OK or GMM_ERR_ARG.
+int vb_set_prior_moments(const double* mean, const double* cov, int D, VbPrior* out);
+// What the per-cluster part of the VB M-step leaves for the serial part.
+struct VbCluster {
+    double nk, beta, nu;
+    double offset;          // -D/2 ln 2 pi - 1/2 ln det R(float) - D/2 ln nu + 1/2 (D ln 2 + sum psi) - D / (2 beta)
+    double log_wishart;     // sklearn's _log_wishart_norm of the cluster (ln det C of the double C)
+    bool ok;                // the float R (and the double C) are positive definite
+};
+// The per-cluster part of the VB M-step of cluster k from the packed statistics about `shift`: N, means, R, Rinv of c
+// (Rinv from the reverse Cholesky factorisation of the float R, as the host finalisation forms it) and `out`.
+void vb_finalize_cluster(const double* stats, const double* shift, int k, int D, const VbPrior& p, clusters_t* c, VbCluster* out);
+// The serial part: weight posterior, E[ln pi], weights_, pi (float, floored at FLT_MIN), constant, and the parameter part of
+// the bound.  post (may be NULL) and its arrays receive the posterior.  Returns -1 if a cluster is not positive definite
+// (its index in *bad_k), else 0.
+int vb_finalize_weights(int K, int D, const VbPrior& p, const VbCluster* cl, clusters_t* c, gmm_vb_posterior* post, double* bound,
+                        int* bad_k);
 
 }  // namespace gmm

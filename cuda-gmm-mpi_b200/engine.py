@@ -21,6 +21,43 @@ _IP = C.POINTER(C.c_int)
 _CP = C.POINTER(clusters_t)
 
 PATH_AUTO, PATH_SIMT, PATH_TENSOR = 0, 1, 2
+VB_DIRICHLET_PROCESS, VB_DIRICHLET_DISTRIBUTION = 0, 1
+
+
+class gmm_vb_prior(C.Structure):
+    _fields_ = [("weight_prior_type", C.c_int), ("weight_concentration", C.c_double), ("mean_precision", C.c_double),
+                ("dof", C.c_double), ("mean", _DP), ("covariance", _DP), ("reg_covar", C.c_double)]
+
+
+class gmm_vb_posterior(C.Structure):
+    _fields_ = [("weights", _DP), ("weight_concentration", _DP), ("mean_precision", _DP), ("dof", _DP), ("mean_prior", _DP),
+                ("covariance_prior", _DP)]
+
+
+def _vb_prior(D, prior_type, weight_concentration, mean_precision, dof, mean, covariance, reg_covar):
+    """gmm_vb_prior and the arrays it points to (keep both alive for the call).  None selects the library's default."""
+    keep = []
+
+    def arr(a, shape):
+        if a is None:
+            return None
+        a = np.ascontiguousarray(a, np.float64)
+        if a.shape != shape:
+            raise ValueError(f"prior array must be {shape}, got {a.shape}")
+        keep.append(a)
+        return a.ctypes.data_as(_DP)
+
+    p = gmm_vb_prior(int(prior_type), -1.0 if weight_concentration is None else float(weight_concentration),
+                     -1.0 if mean_precision is None else float(mean_precision), -1.0 if dof is None else float(dof),
+                     arr(mean, (D,)), arr(covariance, (D, D)), -1.0 if reg_covar is None else float(reg_covar))
+    return p, keep
+
+
+def _vb_posterior(K, D, prior_type):
+    post = dict(weights=np.zeros(K), weight_concentration=np.zeros((2, K) if prior_type == VB_DIRICHLET_PROCESS else K),
+                mean_precision=np.zeros(K), dof=np.zeros(K), mean_prior=np.zeros(D), covariance_prior=np.zeros((D, D)))
+    s = gmm_vb_posterior(*(post[f[0]].ctypes.data_as(_DP) for f in gmm_vb_posterior._fields_))
+    return post, s
 
 _lib = None
 
@@ -92,6 +129,11 @@ def load_library():
                                       C.c_void_p]
     L.gmm_get_condition_stats_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_fit.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _CP, _IP, _FP]
+    L.gmm_vb_em.argtypes = [C.c_void_p, C.c_int, C.POINTER(gmm_vb_prior), C.c_int, C.c_int, C.c_double, _CP,
+                            C.POINTER(gmm_vb_posterior), _DP, _DP, _IP, _IP]
+    L.gmm_host_vb_finalize.argtypes = [_DP, _DP, C.c_int, C.c_int, C.POINTER(gmm_vb_prior), _CP, C.POINTER(gmm_vb_posterior), _DP]
+    L.gmm_host_digamma.argtypes = [_DP, _DP, C.c_longlong]
+    L.gmm_get_vb_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
     L.gmm_stats_len.argtypes = [C.c_int, C.c_int]
@@ -137,6 +179,32 @@ def host_finalize(stats, shift, cl, K):
     assert stats.size >= stats_len(K, cl.D) and shift.size >= cl.D
     s = cl.struct()
     _check(load_library().gmm_host_finalize(stats.ctypes.data_as(_DP), shift.ctypes.data_as(_DP), K, cl.D, C.byref(s)))
+
+
+def host_vb_finalize(stats, shift, cl, K, mean, covariance, prior_type=VB_DIRICHLET_PROCESS, weight_concentration=None,
+                     mean_precision=None, dof=None, reg_covar=None):
+    """VB M-step on the host (gmm_host_vb_finalize): packed statistics about `shift` -> the VB parameter set in cl (N, pi,
+    constant, means, R, Rinv) and the posterior.  The prior's mean and covariance are required here.
+    Returns (posterior dict, bound without its entropy term)."""
+    stats = np.ascontiguousarray(stats, np.float64)
+    shift = np.ascontiguousarray(shift, np.float64)
+    assert stats.size >= stats_len(K, cl.D) and shift.size >= cl.D
+    p, keep = _vb_prior(cl.D, prior_type, weight_concentration, mean_precision, dof, mean, covariance, reg_covar)
+    post, ps = _vb_posterior(K, cl.D, prior_type)
+    bound = C.c_double()
+    s = cl.struct()
+    _check(load_library().gmm_host_vb_finalize(stats.ctypes.data_as(_DP), shift.ctypes.data_as(_DP), K, cl.D, C.byref(p), C.byref(s),
+                                               C.byref(ps), C.byref(bound)))
+    del keep
+    return post, bound.value
+
+
+def host_digamma(x):
+    """The library's double digamma (the psi of gmm_vb_em's bound and E-step offsets)."""
+    x = np.ascontiguousarray(x, np.float64).reshape(-1)
+    out = np.empty_like(x)
+    _check(load_library().gmm_host_digamma(x.ctypes.data_as(_DP), out.ctypes.data_as(_DP), x.size))
+    return out
 
 
 def host_rissanen(ll, K, D, N):
@@ -428,6 +496,27 @@ class Engine:
         _check(self.lib.gmm_get_fit_profile(self.h, out))
         return dict(reduce_order_ms=out[0], seed_ms=out[1], save_ms=out[2], device_finalize_launches=int(out[3]),
                     host_replays=int(round((out[3] - int(out[3])) * 1000)))
+
+    def vb_em(self, K, min_iters=0, max_iters=100, tol=1e-3, prior_type=VB_DIRICHLET_PROCESS, weight_concentration=None,
+              mean_precision=None, dof=None, mean=None, covariance=None, reg_covar=None, lower_bounds=False, out=None):
+        """Variational Bayesian EM at K components from the current K-cluster parameters (gmm_vb_em; sklearn's
+        BayesianGaussianMixture with covariance_type='full').  None selects the prior's default (sklearn's).
+        Returns (clusters, posterior dict, lower bound, bounds per iteration or None, iterations, converged)."""
+        out = out or self.new_clusters()
+        p, keep = _vb_prior(self.D, prior_type, weight_concentration, mean_precision, dof, mean, covariance, reg_covar)
+        post, ps = _vb_posterior(K, self.D, prior_type)
+        lbs = np.full(max(int(max_iters), 1), np.nan) if lower_bounds else None
+        lb, it, conv = C.c_double(), C.c_int(), C.c_int()
+        s = out.struct()
+        _check(self.lib.gmm_vb_em(self.h, K, C.byref(p), int(min_iters), int(max_iters), float(tol), C.byref(s), C.byref(ps), C.byref(lb),
+                                  lbs.ctypes.data_as(_DP) if lbs is not None else None, C.byref(it), C.byref(conv)))
+        del keep
+        return out, post, lb.value, (lbs[:it.value] if lbs is not None else None), it.value, bool(conv.value)
+
+    def vb_profile(self, reset=False):
+        out = (C.c_double * 3)()
+        _check(self.lib.gmm_get_vb_profile(self.h, out, int(reset)))
+        return dict(entropy_ms=out[0], finalize_ms=out[1], wall_ms=out[2])
 
     def comm_rank(self):
         r, n = C.c_int(), C.c_int()

@@ -422,6 +422,93 @@ int  gmm_condition_stats(gmm_ctx*, int K, const int* obs_dims, int n_obs, const 
  * chunks whose statistics came from the wgmma / FP64 SIMT M-step.                                                    */
 int  gmm_get_condition_stats_profile(gmm_ctx*, double out[4], int reset);
 
+/* ---- variational Bayesian mixture (sklearn's BayesianGaussianMixture, covariance_type='full') ------------------------
+ * One fit at an upper bound K; a Dirichlet-process (or Dirichlet) prior on the weights empties the components the data do
+ * not need, where gmm_fit instead runs EM at every model order and keeps the smallest Rissanen score.                */
+#define GMM_VB_DIRICHLET_PROCESS      0   /* sklearn's default weight_concentration_prior_type */
+#define GMM_VB_DIRICHLET_DISTRIBUTION 1
+
+typedef struct {
+    int           weight_prior_type;      /* GMM_VB_*                                                    */
+    double        weight_concentration;   /* gamma0 > 0;  <= 0 selects 1/K                               */
+    double        mean_precision;         /* beta0 > 0;   <= 0 selects 1                                 */
+    double        dof;                    /* nu0 > D-1;   <= 0 selects D                                 */
+    const double* mean;                   /* [D] m0;      NULL selects the events' mean                  */
+    const double* covariance;             /* [D][D] Psi0, symmetric positive definite; NULL selects the
+                                             events' covariance with ddof = 1 (np.cov(X.T))              */
+    double        reg_covar;              /* >= 0 added to each sk's diagonal; < 0 selects 1e-6          */
+} gmm_vb_prior;
+
+typedef struct {                          /* every pointer may be NULL                                   */
+    double* weights;                      /* [K]  sklearn's weights_ (normalised E[pi])                  */
+    double* weight_concentration;         /* [2][K] (DP: the Beta parameters) or [K] (Dirichlet)         */
+    double* mean_precision;               /* [K]  beta                                                   */
+    double* dof;                          /* [K]  nu                                                     */
+    double* mean_prior;                   /* [D]  the m0 used (after defaults)                           */
+    double* covariance_prior;             /* [D][D] the Psi0 used                                        */
+} gmm_vb_posterior;
+
+/* Variational Bayesian EM at K components.  Collective over the ranks of a communicator, like gmm_em (same arguments on
+ * every rank).  Semantics (restated in float64 numpy by tests/_vb_ref.py):
+ *   - start: the context's current parameter set for K (gmm_seed, gmm_seed_kmeans, gmm_set_clusters or an earlier fit).
+ *     One E-step under it gives the responsibilities g0 (sklearn's initial resp); a VB M-step on g0 gives posterior 0.
+ *     Iteration i = 1, 2, ...: an E-step under posterior i-1, the VB M-step that gives posterior i, the lower bound LB_i of
+ *     that E-step's responsibilities and posterior i.  The loop stops after iteration i when i >= min_iters and
+ *     |LB_i - LB_{i-1}| < tol (LB_0 = -inf), or at max_iters; a last E-step under the final posterior leaves valid
+ *     memberships: iters + 2 E-steps and iters + 1 M-steps.  tol is absolute on the total bound (sklearn's tol).
+ *   - VB M-step, in double, from the packed statistics S0, S1, S2 about the centre s that the E- and M-step kernels
+ *     form (wgmma or FP64 SIMT, weights included, summed over the ranks): nk = S0 + 10 * 2^-52, xk = (S0 s + S1) / nk,
+ *     nk sk = sum g (x - xk)(x - xk)^T + nk reg_covar I (expanded about s); then sklearn's _estimate_weights,
+ *     _estimate_means, _estimate_wishart_full: beta = beta0 + nk, m = (beta0 m0 + nk xk) / beta, nu = nu0 + nk,
+ *     C = (Psi0 + nk sk + nk beta0 / beta (xk - m0)(xk - m0)^T) / nu, and weights_ as _set_parameters forms it.
+ *   - the parameter set left in the context and in host_out: N = nk, means = m, R = C (float), Rinv from the reverse
+ *     Cholesky factorisation of the float R (as the host finalisation forms it), pi = weights_ rounded to float and
+ *     floored at FLT_MIN, and constant such that constant + ln pi (the additive term every E-step packs) is sklearn's
+ *       -D/2 ln 2 pi - 1/2 ln det R - D/2 ln nu + 1/2 (D ln 2 + sum_{i<D} psi((nu - i) / 2)) - D / (2 beta) + E[ln pi_k]
+ *     with ln det R from the same factorisation.  So gmm_estep, gmm_score and gmm_score_stats on the fitted context give
+ *     sklearn's predict_proba, predict and score_samples, and gmm_sample draws from weights_.  avgvar is left as it was.
+ *   - bound: LB = -sum_n w_n sum_k g ln g (0 ln 0 = 0) - log_wishart - log_norm_weight - D/2 sum_k ln beta_k
+ *     (sklearn's _compute_lower_bound, with ln det C from a Cholesky factorisation of the double C); psi is the library's
+ *     own double digamma (recurrence + asymptotic series), lgamma / betaln from libm.  The entropy term is one pass of
+ *     resp_entropy_kernel over the memberships (block partials added in block order, then one ncclAllReduce of one
+ *     double), run only in iterations whose bound is used (i >= min_iters - 1, or all when lower_bounds_out != NULL).
+ *   - weights (gmm_set_weights) enter the statistics as in gmm_em, the entropy as w_n, and the default prior as the
+ *     weighted mean and covariance with denominator sum w - 1: integer weights give the fit of replicated rows.
+ *   - the default m0 / Psi0 come from the context's own M-step at K = 1 on unit responsibilities (written by the k-means
+ *     assignment kernel with one centre), which allocates gmm_seed_kmeans' buffers.
+ *   - afterwards: cur_K = K, memberships valid, gmm_get_profile counts the iterations; the set counts as one given from
+ *     outside (as after gmm_set_clusters): a later replay of the device-side finalisation keeps its Rinv and constant.
+ *   host_out          all clusters_t arrays except memberships (may be NULL)
+ *   post_out          the posterior (may be NULL; so may each of its pointers)
+ *   lower_bound_out   LB of the last iteration (-inf when max_iters = 0); lower_bounds_out [max_iters]: LB_1 .. LB_iters
+ *   iters_out         iterations run; converged_out 1 when the tol test stopped the loop
+ * Errors: K outside [1, Kmax], a NULL prior, an unknown prior type, gamma0 / beta0 / reg_covar / m0 not finite, nu0 in
+ * (0, D - 1] or NaN, Psi0 not symmetric positive definite, min_iters < 0, max_iters < min_iters, or tol < 0 or NaN ->
+ * GMM_ERR_ARG; a default prior over a total weight <= 1 -> GMM_ERR_ARG; K != the K of the current parameters, a call
+ * between gmm_mstep and gmm_constants, or a posterior whose float covariance is not positive definite -> GMM_ERR_STATE;
+ * a failed collective -> GMM_ERR_NCCL.
+ * Device memory: [4 x SMs + 1] doubles of entropy partials (and their pinned mirror), allocated on first use, freed by
+ * gmm_destroy.                                                                                                        */
+int  gmm_vb_em(gmm_ctx*, int K, const gmm_vb_prior* prior, int min_iters, int max_iters, double tol,
+               clusters_t* host_out, gmm_vb_posterior* post_out,
+               double* lower_bound_out, double* lower_bounds_out /* [max_iters] or NULL */,
+               int* iters_out, int* converged_out);
+
+/* Host-only, usable without a GPU (as gmm_host_finalize): packed statistics about `shift` (gmm_stats_len(K, D) doubles,
+ * e.g. the sum of gmm_score_stats over batches) -> the VB parameter set of gmm_vb_em in `out` (N, pi, constant, means,
+ * R, Rinv; avgvar untouched) and the posterior; *bound_out (may be NULL) = -log_wishart - log_norm_weight
+ * - D/2 sum ln beta (the lower bound without its entropy term).  prior->mean and prior->covariance are required.
+ * Errors: as gmm_vb_em's argument errors, NULL stats / shift / out / prior mean or covariance -> GMM_ERR_ARG; a float
+ * covariance that is not positive definite -> GMM_ERR_STATE.                                                          */
+int  gmm_host_vb_finalize(const double* stats, const double* shift, int K, int D, const gmm_vb_prior* prior,
+                          clusters_t* out, gmm_vb_posterior* post_out, double* bound_out);
+
+/* The library's digamma in double (recurrence to x >= 10, then the asymptotic series): n values, x > 0.             */
+int  gmm_host_digamma(const double* x, double* out, long long n);
+
+/* Since the last reset: out[0] entropy-kernel ms, out[1] host VB finalisation ms, out[2] wall ms inside gmm_vb_em.    */
+int  gmm_get_vb_profile(gmm_ctx*, double out[3], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
