@@ -605,6 +605,19 @@ static int check_path(const gmm_ctx* c, int K) {
 
 static int ensure_moments(gmm_ctx* c);
 
+// The worker team of the host finalisation, created on first use and resized to the context's host_threads.
+static HostPool* host_pool(gmm_ctx* c) {
+    if (!c->pool) c->pool = new HostPool(c->host_threads);
+    else c->pool->resize(c->host_threads);
+    return c->pool;
+}
+
+// fn(i) for i in [0, n), the items of a loop over K clusters: on the worker team when K >= 8, serially below.
+static void run_clusters(gmm_ctx* c, int K, int n, const std::function<void(int)>& fn) {
+    if (K >= 8) host_pool(c)->run(n, fn);
+    else for (int i = 0; i < n; i++) fn(i);
+}
+
 // Upload the current host parameters in the form the E-step kernels consume
 // (gaussian.cu:446-452 / 935-941 upload the seven raw arrays; here the E-step
 // operand is pre-packed on the host once per iteration).
@@ -628,8 +641,6 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
             if (with_constants) mixing_weights(K, &c->host);
             const int kp = tc_params_padded(c->tc, K), D = c->D;
             std::atomic<int> bad_all{0};
-            if (!c->pool) c->pool = new HostPool(c->host_threads);
-            else c->pool->resize(c->host_threads);
             const std::function<void(int)> per_cluster = [&](int k) {
                 if (with_finalize && k < K) finalize_cluster(c->h_stats, c->shift, k, D, &c->host);
                 int b;
@@ -643,8 +654,7 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
                 int cur = bad_all.load(std::memory_order_relaxed);
                 while (b > cur && !bad_all.compare_exchange_weak(cur, b)) {}
             };
-            if (K >= 8) c->pool->run(kp, per_cluster);
-            else for (int k = 0; k < kp; k++) per_cluster(k);
+            run_clusters(c, K, kp, per_cluster);
             const int bad = bad_all.load();
             with_constants = with_finalize = false;
             rc = tc_params_commit(c->tc, K, bad, c->stream);
@@ -901,6 +911,49 @@ static int check_K(const gmm_ctx* c, int K, const char* who) {
     if (!c) return fail(GMM_ERR_ARG, std::string(who) + ": null context");
     if (K < 1 || K > c->Kmax) return fail(GMM_ERR_ARG, std::string(who) + ": K out of range");
     return GMM_OK;
+}
+
+// The calls that apply the current parameter set to new events need a complete one for this K.
+static int check_fitted(const gmm_ctx* c, int K, const char* who) {
+    if (K != c->cur_K) return fail(GMM_ERR_STATE, std::string(who) + ": parameters for this K have not been set");
+    if (c->params_partial)
+        return fail(GMM_ERR_STATE, std::string(who) + ": gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    return GMM_OK;
+}
+
+// obs_dims of the conditioning calls (strictly increasing indices in [0, D), 1 to D of them), and the rest of [0, D): the
+// missing dimensions mis[0 .. *nm) and a bit per observed dimension in *obs_mask.
+static int split_obs(const gmm_ctx* c, const int* obs_dims, int n_obs, const char* who, int* mis, int* nm, unsigned* obs_mask) {
+    if (!obs_dims || n_obs < 1 || n_obs > c->D)
+        return fail(GMM_ERR_ARG, std::string(who) + ": obs_dims must hold between 1 and D dimension indices");
+    for (int i = 0; i < n_obs; i++)
+        if (obs_dims[i] < 0 || obs_dims[i] >= c->D || (i > 0 && obs_dims[i] <= obs_dims[i - 1]))
+            return fail(GMM_ERR_ARG, std::string(who) + ": obs_dims must be strictly increasing indices in [0, D)");
+    *nm = 0;
+    *obs_mask = 0;
+    for (int d = 0, i = 0; d < c->D; d++) {
+        if (i < n_obs && obs_dims[i] == d) { *obs_mask |= 1u << d; i++; }
+        else mis[(*nm)++] = d;
+    }
+    return GMM_OK;
+}
+
+// The centre the statistics of new events are taken about.  Before the context's first M-step it comes from the global
+// column moments, an all-reduce over the ranks: computed here on one rank, never issued from here on several.
+static int ensure_centre(gmm_ctx* c, const char* who) {
+    if (c->have_shift) return GMM_OK;
+    if (c->nranks > 1)
+        return fail(GMM_ERR_STATE, std::string(who) + ": the context's centre is not fixed yet (run gmm_mstep or gmm_em first on every rank)");
+    return ensure_moments(c);
+}
+
+// Nothing of a streaming call may still be in flight when it returns (also after a failure): both streams are drained, and
+// an error they report becomes the call's when rc is still GMM_OK.
+static int drain_streams(gmm_ctx* c, int rc, const char* who) {
+    const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
+    if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
+        rc = fail(GMM_ERR_CUDA, std::string(who) + ": " + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+    return rc;
 }
 
 }  // namespace gmm
@@ -1645,28 +1698,110 @@ static TcScoreIo score_io(gmm_ctx* c, char* base, int b, int n) {
     return io;
 }
 
-// Chunks of the batch go through slot i & 1: host rows -> pinned stage -> (copy stream) device chunk -> (compute stream)
-// score kernel -> (copy stream) outputs -> pinned mirror -> caller's arrays.  Chunk i's H2D and the host staging of
-// chunk i + 1 overlap chunk i - 1's kernel and D2H; a chunk is finished (outputs handed over, re-scored if needed)
-// while the next one is already queued.
-static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, int* labels, float* max_resp, float* logp, double* ll_sum) {
+// Kernel time of slot b's last launch (between its timing events), added to *acc.
+static void add_slot_ms(gmm_ctx* c, int b, double* acc) {
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, c->score.t0[b], c->score.t1[b]) == cudaSuccess) *acc += ms;
+}
+
+// Input half of slot b: m host rows of `width` floats -> pinned stage -> (copy stream) device chunk.
+static int stage_chunk(gmm_ctx* c, int b, const float* rows, int m, int width) {
+    ScoreBuffers& s = c->score;
+    CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
+    std::memcpy(s.h_in[b], rows, sizeof(float) * (size_t)m * width);
+    CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the device chunk's previous readers are done with it
+    CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * width, cudaMemcpyHostToDevice, s.copy));
+    CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
+    return GMM_OK;
+}
+
+// The chunk pipeline of the calls that stream outputs back (gmm_score, gmm_condition, gmm_sample).  Chunk i of
+// c->score_chunk events goes through slot b = i & 1: with `in`, its host rows (`width` floats each) -> pinned stage ->
+// (copy stream) device chunk; then (compute stream) launch(b, e0, m), which records the slot's timing events around its
+// kernels -> (copy stream) fetch(b, m, stream) into the slot's pinned mirrors -> hand_over(b, e0, m) to the caller's
+// arrays.  Chunk i is issued before chunk i - 1 is finished, so chunk i's H2D and the host staging of chunk i + 1 overlap
+// chunk i - 1's kernel and D2H.  Finishing a chunk adds its kernel time to *kernel_ms before the hand-over.
+using ChunkFn = std::function<int(int b, long long e0, int m)>;
+static int stream_chunks(gmm_ctx* c, long long n, const float* in, int width, double* kernel_ms, const ChunkFn& launch,
+                         const std::function<int(int b, int m, cudaStream_t st)>& fetch, const ChunkFn& hand_over) {
+    ScoreBuffers& s = c->score;
+    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;     // (the buffers hold at least this many)
+    auto rows_of = [&](long long i) { return (int)std::min(chunk, n - i * chunk); };
+    for (long long i = 0; i <= nchunks; i++) {
+        if (i < nchunks) {                                        // issue chunk i
+            const int b = (int)(i & 1), m = rows_of(i);
+            if (in) {
+                if (int rc = stage_chunk(c, b, in + (size_t)(i * chunk) * width, m, width)) return rc;
+                CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
+            }
+            CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous outputs have left the device
+            if (int rc = launch(b, i * chunk, m)) return rc;
+            CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
+            CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
+            if (int rc = fetch(b, m, s.copy)) return rc;
+            CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
+        }
+        if (i > 0) {                                              // finish chunk i - 1
+            const int b = (int)((i - 1) & 1);
+            CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
+            add_slot_ms(c, b, kernel_ms);
+            if (int rc = hand_over(b, (i - 1) * chunk, rows_of(i - 1))) return rc;
+        }
+    }
+    return GMM_OK;
+}
+
+// The outputs gmm_score and gmm_condition return per event (NULL: not requested) and the sum of the chunks' log-likelihoods.
+struct ScoreOut {
+    int* labels;
+    float* max_resp;
+    float* logp;
+    double* ll_sum;
+};
+
+// D2H of slot b's header and requested outputs on stream st.
+static int fetch_scores(gmm_ctx* c, const ScoreOut& o, int b, int m, cudaStream_t st) {
+    ScoreBuffers& s = c->score;
+    const TcScoreIo dv = score_io(c, s.d_out[b], b, m), hv = score_io(c, s.h_out[b], b, m);
+    CUDA_TRY(cudaMemcpyAsync(s.h_out[b], s.d_out[b], ScoreBuffers::kHeader, cudaMemcpyDeviceToHost, st));
+    if (o.labels) CUDA_TRY(cudaMemcpyAsync(hv.labels, dv.labels, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, st));
+    if (o.max_resp) CUDA_TRY(cudaMemcpyAsync(hv.max_resp, dv.max_resp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
+    if (o.logp) CUDA_TRY(cudaMemcpyAsync(hv.logp, dv.logp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
+    return GMM_OK;
+}
+
+// Slot b's fetched outputs of the chunk at event e0 to the caller.
+static void hand_over_scores(gmm_ctx* c, const ScoreOut& o, int b, long long e0, int m) {
+    const TcScoreIo hv = score_io(c, c->score.h_out[b], b, m);
+    *o.ll_sum += *hv.ll;
+    if (o.labels) std::memcpy(o.labels + e0, hv.labels, sizeof(int) * (size_t)m);
+    if (o.max_resp) std::memcpy(o.max_resp + e0, hv.max_resp, sizeof(float) * (size_t)m);
+    if (o.logp) std::memcpy(o.logp + e0, hv.logp, sizeof(float) * (size_t)m);
+}
+
+// d_epack of the current parameters for a SIMT kernel: while the tensor operand serves them it is not maintained, so the
+// first SIMT kernel of a call builds it from the host copy (*ready: it is current).
+static int ensure_epack(gmm_ctx* c, int K, bool* ready) {
+    if (*ready) return GMM_OK;
+    const int D = c->D;
+    build_epack(K, D, &c->host, c->h_epack);
+    CUDA_TRY(cudaMemcpyAsync(c->d_epack, c->h_epack, sizeof(float) * (size_t)K * epack_stride(D), cudaMemcpyHostToDevice, c->stream));
+    *ready = true;
+    return GMM_OK;
+}
+
+// gmm_score's chunks through the pipeline, on the E-step's kernel family for the current parameters.  A tensor chunk that
+// flags an event is scored again by the SIMT kernel before it is handed over.
+static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, const ScoreOut& out) {
     ScoreBuffers& s = c->score;
     const int D = c->D;
-    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;     // (the buffers hold at least this many)
     const bool tensor = c->estep_tensor_ready;
-    bool epack_ready = !tensor;            // while the tensor operand serves the parameters d_epack is not maintained
-    auto ensure_epack = [&]() -> int {
-        if (epack_ready) return GMM_OK;
-        build_epack(K, D, &c->host, c->h_epack);
-        CUDA_TRY(cudaMemcpyAsync(c->d_epack, c->h_epack, sizeof(float) * (size_t)K * epack_stride(D), cudaMemcpyHostToDevice, c->stream));
-        epack_ready = true;
-        return GMM_OK;
-    };
+    bool epack_ready = !tensor;
     auto launch = [&](int b, int m, bool on_tensor) -> int {
         const TcScoreIo io = score_io(c, s.d_out[b], b, m);
         CUDA_TRY(cudaMemsetAsync(s.d_out[b], 0, ScoreBuffers::kHeader, c->stream));
         if (!on_tensor)
-            if (int rc = ensure_epack()) return rc;
+            if (int rc = ensure_epack(c, K, &epack_ready)) return rc;
         CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
         int rc = on_tensor ? tc_launch_score(c->tc, K, io, c->stream) : launch_score_simt(c, D, K, c->d_epack, io);
         if (rc) return rc;
@@ -1674,45 +1809,9 @@ static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, int* lab
         (on_tensor ? s.tensor_chunks : s.simt_chunks)++;
         return GMM_OK;
     };
-    // D2H of the header and of the requested outputs of slot b
-    auto fetch = [&](int b, int m, cudaStream_t st) -> int {
-        const TcScoreIo dv = score_io(c, s.d_out[b], b, m), hv = score_io(c, s.h_out[b], b, m);
-        CUDA_TRY(cudaMemcpyAsync(s.h_out[b], s.d_out[b], ScoreBuffers::kHeader, cudaMemcpyDeviceToHost, st));
-        if (labels) CUDA_TRY(cudaMemcpyAsync(hv.labels, dv.labels, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, st));
-        if (max_resp) CUDA_TRY(cudaMemcpyAsync(hv.max_resp, dv.max_resp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
-        if (logp) CUDA_TRY(cudaMemcpyAsync(hv.logp, dv.logp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, st));
-        return GMM_OK;
-    };
-    auto kernel_ms = [&](int b) {
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) s.kernel_ms += ms;
-    };
-    auto issue = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
-        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
-        std::memcpy(s.h_in[b], ev + (size_t)e0 * D, sizeof(float) * (size_t)m * D);
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the chunk buffer's previous kernel is done with it
-        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyHostToDevice, s.copy));
-        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous outputs have left the device
-        if (int rc = launch(b, m, tensor)) return rc;
-        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
-        if (int rc = fetch(b, m, s.copy)) return rc;
-        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
-        return GMM_OK;
-    };
-    auto finish = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
-        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
-        kernel_ms(b);
-        const TcScoreIo hv = score_io(c, s.h_out[b], b, m);
-        if (tensor && *hv.flag) {
+    auto fetch = [&](int b, int m, cudaStream_t st) { return fetch_scores(c, out, b, m, st); };
+    auto hand_over = [&](int b, long long e0, int m) -> int {
+        if (tensor && *score_io(c, s.h_out[b], b, m).flag) {
             // an event beyond the FP16 event operand's range (or not finite): the SIMT kernel scores the chunk again
             // (its rows are still in the slot's device buffer: the next H2D into it is issued after this)
             if (estep_path_of(c) == GMM_PATH_TENSOR)
@@ -1722,39 +1821,26 @@ static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, int* lab
             if (int rc = launch(b, m, false)) return rc;
             if (int rc = fetch(b, m, c->stream)) return rc;
             CUDA_TRY(cudaStreamSynchronize(c->stream));
-            kernel_ms(b);
+            add_slot_ms(c, b, &s.kernel_ms);
         }
-        *ll_sum += *hv.ll;
-        if (labels) std::memcpy(labels + e0, hv.labels, sizeof(int) * (size_t)m);
-        if (max_resp) std::memcpy(max_resp + e0, hv.max_resp, sizeof(float) * (size_t)m);
-        if (logp) std::memcpy(logp + e0, hv.logp, sizeof(float) * (size_t)m);
+        hand_over_scores(c, out, b, e0, m);
         return GMM_OK;
     };
-    for (long long i = 0; i < nchunks; i++) {
-        if (int rc = issue(i)) return rc;
-        if (i > 0)
-            if (int rc = finish(i - 1)) return rc;
-    }
-    return finish(nchunks - 1);
+    return stream_chunks(c, n, ev, D, &s.kernel_ms, [&](int b, long long, int m) { return launch(b, m, tensor); }, fetch, hand_over);
 }
 
 int gmm_score(gmm_ctx* c, int K, const float* events_aos, long long n, int* labels, float* max_resp, float* logp, double* loglik_out) {
     if (int rc = check_K(c, K, "gmm_score")) return rc;
     if (n < 0 || (n > 0 && !events_aos)) return fail(GMM_ERR_ARG, "gmm_score: bad events (n < 0, or no rows)");
-    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_score: parameters for this K have not been set");
-    if (c->params_partial)
-        return fail(GMM_ERR_STATE, "gmm_score: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    if (int rc = check_fitted(c, K, "gmm_score")) return rc;
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
     double ll = 0.0;
     int rc = GMM_OK;
     if (n > 0) {
         rc = score_buffers(c);
-        if (rc == GMM_OK) rc = score_batch(c, K, events_aos, n, labels, max_resp, logp, &ll);
-        // nothing of this call may still be in flight when it returns (also after a failure)
-        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
-        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-            rc = fail(GMM_ERR_CUDA, std::string("gmm_score: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        if (rc == GMM_OK) rc = score_batch(c, K, events_aos, n, {labels, max_resp, logp, &ll});
+        rc = drain_streams(c, rc, "gmm_score");
     }
     c->score.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     if (rc == GMM_OK && loglik_out) *loglik_out = ll;
@@ -1800,33 +1886,24 @@ static int score_stats_buffers(gmm_ctx* c, bool with_memberships, bool with_obse
     return GMM_OK;
 }
 
-// Per chunk i (slot b = i & 1 of gmm_score's input stage), in order on the compute stream: prep kernel (SoA copies + range
-// flag) -> flag to the host, while chunk i + 1 is staged and its H2D issued -> the kernels the flag allows -> E-step into the
+// The chunk loop of the calls that return E- and M-step statistics of streamed events (gmm_score_stats,
+// gmm_condition_stats).  Per chunk i (slot b = i & 1 of gmm_score's input stage, rows of `width` floats), in order on the
+// compute stream: prep(b, m), the call's prep kernel (its SoA copies and the range flag) -> flag to the host, while chunk
+// i + 1 is staged and its H2D issued -> estep(b, m, ce, cm), the fallback image the flag calls for and the E-step into the
 // chunk's responsibilities -> M-step adding into the call's statistics -> (memberships) pitched D2H and rows to the caller.
-static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bool with_stats, float* memberships, StatsProfile& pr) {
+// e_tensor / m_tensor: the call puts the wgmma E- / M-step on the chunks whose flag allows it (ce / cm).  `who` names the
+// call in errors.
+static int stats_batch(gmm_ctx* c, int K, const float* ev, int width, long long n, bool with_stats, float* memberships,
+                       bool e_tensor, bool m_tensor, StatsProfile& pr, const char* who, const std::function<int(int b, int m)>& prep,
+                       const std::function<int(int b, int m, bool ce, bool cm)>& estep) {
     ScoreBuffers& s = c->score;
     ScoreStatsBuffers& t = c->sstats;
-    const int D = c->D;
     const size_t KF = (size_t)K * c->F;
     const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
-    const bool e_tensor = c->estep_tensor_ready;
-    const bool m_tensor = with_stats && use_tensor_mstep(c, K);
-    const bool raw_always = !e_tensor || (with_stats && !m_tensor);   // the context's own selection puts a SIMT kernel on every chunk
-    const float* shift_f = (e_tensor || m_tensor) ? tc_shift_f(c->tc) : nullptr;
-    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
-    if ((e_tensor || m_tensor) && !shift_f) return fail(GMM_ERR_STATE, "gmm_score_stats: the tensor kernels have no centre");
-    bool epack_ready = !e_tensor;          // while the tensor operand serves the parameters d_epack is not maintained
+    bool epack_ready = !e_tensor;          // (a chunk the wgmma E-step cannot take runs the SIMT one on d_epack)
     CUDA_TRY(cudaMemsetAsync(t.d_stats, 0, sizeof(double) * (KF + 1), c->stream));
     auto rows_of = [&](long long i) { return (int)std::min(chunk, n - i * chunk); };
-    auto stage = [&](long long i) -> int {
-        const int b = (int)(i & 1), m = rows_of(i);
-        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
-        std::memcpy(s.h_in[b], ev + (size_t)(i * chunk) * D, sizeof(float) * (size_t)m * D);
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the device chunk's previous readers are done with it
-        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyHostToDevice, s.copy));
-        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
-        return GMM_OK;
-    };
+    auto stage = [&](long long i) { return stage_chunk(c, (int)(i & 1), ev + (size_t)(i * chunk) * width, rows_of(i), width); };
     auto collect = [&](int b) {                                   // timings of a chunk whose kernels have finished
         float a = 0, k = 0, w = 0;
         if (cudaEventElapsedTime(&a, t.p0[b], t.p1[b]) == cudaSuccess && cudaEventElapsedTime(&k, t.k0[b], t.k1[b]) == cudaSuccess)
@@ -1841,10 +1918,7 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
         CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
         CUDA_TRY(cudaMemsetAsync(t.d_flag, 0, sizeof(int), c->stream));
         CUDA_TRY(cudaEventRecord(t.p0[b], c->stream));
-        score_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(
-            s.d_in[b], m, D, shift_f, shift_f ? tc_inv_scale_f(c->tc) : nullptr, zb, m_tensor ? t.d_z : nullptr,
-            raw_always ? t.d_xs : nullptr, t.pitch, t.d_flag);
-        CUDA_TRY(cudaGetLastError());
+        if (int rc = prep(b, m)) return rc;
         CUDA_TRY(cudaEventRecord(t.p1[b], c->stream));
         CUDA_TRY(cudaMemcpyAsync(t.h_flag, t.d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(cudaEventRecord(t.ev_flag, c->stream));
@@ -1853,27 +1927,19 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
         CUDA_TRY(cudaEventSynchronize(t.ev_flag));
         if (i > 0) collect(b ^ 1);                                // (the prep of chunk i ran after chunk i - 1's kernels)
         const int flag = *t.h_flag;
-        if (flag & kScoreStatsNotFinite) return fail(GMM_ERR_ARG, "gmm_score_stats: an event has a coordinate that is not finite");
+        if (flag & kScoreStatsNotFinite) return fail(GMM_ERR_ARG, std::string(who) + ": an event has a coordinate that is not finite");
         const bool ce = e_tensor && !(flag & kScoreStatsBeyondFp16);
         const bool cm = m_tensor && !(flag & kScoreStatsBeyondZb);
         if (e_tensor && !ce && estep_path_of(c) == GMM_PATH_TENSOR)
-            return fail(GMM_ERR_STATE, "gmm_score_stats: an event lies beyond 2^14 standard deviations (the tensor E-step's FP16 "
-                                       "operand range) and estep_path is GMM_PATH_TENSOR");
+            return fail(GMM_ERR_STATE, std::string(who) + ": an event lies beyond 2^14 standard deviations (the tensor E-step's "
+                                                           "FP16 operand range) and estep_path is GMM_PATH_TENSOR");
         if (m_tensor && !cm && mstep_path_of(c) == GMM_PATH_TENSOR)
-            return fail(GMM_ERR_STATE, "gmm_score_stats: an event lies beyond the tensor M-step's fixed-point range (|z| >= the "
-                                       "training data's bound) and mstep_path is GMM_PATH_TENSOR");
-        if (!ce && !epack_ready) {
-            build_epack(K, D, &c->host, c->h_epack);
-            CUDA_TRY(cudaMemcpyAsync(c->d_epack, c->h_epack, sizeof(float) * (size_t)K * epack_stride(D), cudaMemcpyHostToDevice, c->stream));
-            epack_ready = true;
-        }
+            return fail(GMM_ERR_STATE, std::string(who) + ": an event lies beyond the tensor M-step's fixed-point range (|z| >= "
+                                                           "the training data's bound) and mstep_path is GMM_PATH_TENSOR");
+        if (!ce)
+            if (int rc = ensure_epack(c, K, &epack_ready)) return rc;
         CUDA_TRY(cudaEventRecord(t.k0[b], c->stream));
-        if (!raw_always && (!ce || (with_stats && !cm))) {       // a fallback of this chunk only: its raw SoA copy now
-            transpose_aos_to_soa_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], t.d_xs, t.pitch, m, D);
-            CUDA_TRY(cudaGetLastError());
-        }
-        int rc = ce ? tc_launch_estep_on(c->tc, K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
-                    : launch_estep_simt_on(c, D, K, c->d_epack, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
+        int rc = estep(b, m, ce, cm);
         if (rc) return rc;
         (ce ? pr.e_tensor : pr.e_simt)++;
         CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
@@ -1898,31 +1964,53 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
     return GMM_OK;
 }
 
+// gmm_score_stats' chunks through the statistics loop, on the context's own kernel selection: the prep kernel writes the
+// standardised SoA copy for the wgmma M-step and the raw one when the selection already puts a SIMT kernel on every chunk;
+// a chunk that falls back only because of its flag gets its raw copy after the flag is read.
+static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bool with_stats, float* memberships, StatsProfile& pr) {
+    ScoreBuffers& s = c->score;
+    ScoreStatsBuffers& t = c->sstats;
+    const int D = c->D;
+    const size_t KF = (size_t)K * c->F;
+    const bool e_tensor = c->estep_tensor_ready;
+    const bool m_tensor = with_stats && use_tensor_mstep(c, K);
+    const bool raw_always = !e_tensor || (with_stats && !m_tensor);   // the context's own selection puts a SIMT kernel on every chunk
+    const float* shift_f = (e_tensor || m_tensor) ? tc_shift_f(c->tc) : nullptr;
+    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
+    if ((e_tensor || m_tensor) && !shift_f) return fail(GMM_ERR_STATE, "gmm_score_stats: the tensor kernels have no centre");
+    auto prep = [&](int b, int m) -> int {
+        score_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(
+            s.d_in[b], m, D, shift_f, shift_f ? tc_inv_scale_f(c->tc) : nullptr, zb, m_tensor ? t.d_z : nullptr,
+            raw_always ? t.d_xs : nullptr, t.pitch, t.d_flag);
+        CUDA_TRY(cudaGetLastError());
+        return GMM_OK;
+    };
+    auto estep = [&](int b, int m, bool ce, bool cm) -> int {
+        if (!raw_always && (!ce || (with_stats && !cm))) {       // a fallback of this chunk only: its raw SoA copy now
+            transpose_aos_to_soa_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], t.d_xs, t.pitch, m, D);
+            CUDA_TRY(cudaGetLastError());
+        }
+        return ce ? tc_launch_estep_on(c->tc, K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
+                  : launch_estep_simt_on(c, D, K, c->d_epack, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
+    };
+    return stats_batch(c, K, ev, D, n, with_stats, memberships, e_tensor, m_tensor, pr, "gmm_score_stats", prep, estep);
+}
+
 int gmm_score_stats(gmm_ctx* c, int K, const float* events_aos, long long n, double* stats_out, double* shift_out, float* memberships) {
     if (int rc = check_K(c, K, "gmm_score_stats")) return rc;
     if (n < 0 || (n > 0 && !events_aos)) return fail(GMM_ERR_ARG, "gmm_score_stats: bad events (n < 0, or no rows)");
     if (!stats_out && !memberships) return fail(GMM_ERR_ARG, "gmm_score_stats: neither statistics nor memberships requested");
-    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_score_stats: parameters for this K have not been set");
-    if (c->params_partial)
-        return fail(GMM_ERR_STATE, "gmm_score_stats: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    if (int rc = check_fitted(c, K, "gmm_score_stats")) return rc;
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
-    if (!c->have_shift) {
-        // the centre comes from the global column moments, an all-reduce over the ranks: never issued from here
-        if (c->nranks > 1)
-            return fail(GMM_ERR_STATE, "gmm_score_stats: the context's centre is not fixed yet (run gmm_mstep or gmm_em first on every rank)");
-        if (int rc = ensure_moments(c)) return rc;
-    }
+    if (int rc = ensure_centre(c, "gmm_score_stats")) return rc;
     const size_t len = (size_t)K * c->F + 1;
     int rc = GMM_OK;
     if (n > 0) {
         rc = score_buffers(c);
         if (rc == GMM_OK) rc = score_stats_buffers(c, memberships != nullptr);
         if (rc == GMM_OK) rc = score_stats_batch(c, K, events_aos, n, stats_out != nullptr, memberships, c->sstats.prof);
-        // nothing of this call may still be in flight when it returns (also after a failure)
-        const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
-        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-            rc = fail(GMM_ERR_CUDA, std::string("gmm_score_stats: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        rc = drain_streams(c, rc, "gmm_score_stats");
     }
     if (rc == GMM_OK) {
         if (stats_out) {
@@ -2296,14 +2384,7 @@ static int vb_entropy_sum(gmm_ctx* c, int grid, double* out) {
 static int vb_finalize_upload(gmm_ctx* c, int K, const VbPrior& p, std::vector<VbCluster>& cl, gmm_vb_posterior* post, double* bound) {
     auto t0 = std::chrono::steady_clock::now();
     const int D = c->D;
-    const std::function<void(int)> per_cluster = [&](int k) { vb_finalize_cluster(c->h_stats, c->shift, k, D, p, &c->host, &cl[(size_t)k]); };
-    if (K >= 8) {
-        if (!c->pool) c->pool = new HostPool(c->host_threads);
-        else c->pool->resize(c->host_threads);
-        c->pool->run(K, per_cluster);
-    } else {
-        for (int k = 0; k < K; k++) per_cluster(k);
-    }
+    run_clusters(c, K, K, [&](int k) { vb_finalize_cluster(c->h_stats, c->shift, k, D, p, &c->host, &cl[(size_t)k]); });
     int bad = -1;
     const int rc = vb_finalize_weights(K, D, p, cl.data(), &c->host, post, bound, &bad);
     c->vb_final_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -2422,15 +2503,12 @@ static int sample_params(gmm_ctx* c, int K, int* klast) {
     return GMM_OK;
 }
 
-// Chunks of c->score_chunk events through gmm_score's slots: sample_kernel writes slot i & 1's device chunk (rows) and
-// label area, the copy stream brings them to the slot's pinned stages, the host copies them to the caller's arrays.  The
-// order is score_batch's: chunk i is issued before chunk i - 1 is handed over, so chunk i's kernel runs while chunk
-// i - 1's D2H and the host copy of chunk i - 2 proceed.
+// gmm_sample's chunks through the pipeline without its input half: sample_kernel writes the slot's device chunk (rows) and
+// label area, the copy stream brings them to the slot's pinned stages, the host copies them to the caller's arrays.
 static int sample_batch(gmm_ctx* c, int K, int klast, unsigned long long seed, long long first, long long n, float* events,
                         int* labels) {
     ScoreBuffers& s = c->score;
     const int D = c->D;
-    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
     CUDA_TRY(cudaMemcpyAsync(c->sample.d_block, c->sample.h_block, sample_block_bytes(K, D), cudaMemcpyHostToDevice, c->stream));
     // the parameters go to shared memory when they fit beside the output tile with two blocks per SM (D = 24: K <= 66)
     const size_t staged = sample_tile_bytes(D) + sample_block_bytes(K, D);
@@ -2446,13 +2524,9 @@ static int sample_batch(gmm_ctx* c, int K, int klast, unsigned long long seed, l
 #undef GMM_CALL
     const long long max_grid = (long long)std::max(per_sm, 1) * c->num_sms;
     auto labels_of = [&](char* base) { return reinterpret_cast<int*>(base + ScoreBuffers::kHeader); };
-    auto issue = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
+    auto launch = [&](int b, long long e0, int m) -> int {
         const int grid = (int)std::min<long long>((m + kSampleThreads - 1) / kSampleThreads, max_grid);
         int* d_lab = labels_of(s.d_out[b]);
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous chunk has left the device
         CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
 #define GMM_CALL(d) \
     sample_kernel<d><<<grid, kSampleThreads, smem, c->stream>>>(c->sample.d_block, K, klast, stage, seed, first + e0, m, s.d_in[b], d_lab)
@@ -2460,30 +2534,19 @@ static int sample_batch(gmm_ctx* c, int K, int klast, unsigned long long seed, l
 #undef GMM_CALL
         CUDA_TRY(cudaGetLastError());
         CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
-        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
-        CUDA_TRY(cudaMemcpyAsync(s.h_in[b], s.d_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyDeviceToHost, s.copy));
-        if (labels) CUDA_TRY(cudaMemcpyAsync(labels_of(s.h_out[b]), d_lab, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
-        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
         return GMM_OK;
     };
-    auto finish = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
-        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) c->sample.kernel_ms += ms;
+    auto fetch = [&](int b, int m, cudaStream_t st) -> int {
+        CUDA_TRY(cudaMemcpyAsync(s.h_in[b], s.d_in[b], sizeof(float) * (size_t)m * D, cudaMemcpyDeviceToHost, st));
+        if (labels) CUDA_TRY(cudaMemcpyAsync(labels_of(s.h_out[b]), labels_of(s.d_out[b]), sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, st));
+        return GMM_OK;
+    };
+    auto hand_over = [&](int b, long long e0, int m) -> int {
         std::memcpy(events + (size_t)e0 * D, s.h_in[b], sizeof(float) * (size_t)m * D);
         if (labels) std::memcpy(labels + e0, labels_of(s.h_out[b]), sizeof(int) * (size_t)m);
         return GMM_OK;
     };
-    for (long long i = 0; i < nchunks; i++) {
-        if (int rc = issue(i)) return rc;
-        if (i > 0)
-            if (int rc = finish(i - 1)) return rc;
-    }
-    return finish(nchunks - 1);
+    return stream_chunks(c, n, nullptr, 0, &c->sample.kernel_ms, launch, fetch, hand_over);
 }
 #undef GMM_SEED_CASE
 #undef GMM_SEED_DISPATCH
@@ -2492,9 +2555,7 @@ int gmm_sample(gmm_ctx* c, int K, long long n, unsigned long long seed, long lon
     if (int rc = check_K(c, K, "gmm_sample")) return rc;
     if (n < 0 || first < 0 || first > (1LL << 62) - n || (n > 0 && !events_out))
         return fail(GMM_ERR_ARG, "gmm_sample: bad range or output (n < 0, first < 0, first + n > 2^62, or no event array)");
-    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_sample: parameters for this K have not been set");
-    if (c->params_partial)
-        return fail(GMM_ERR_STATE, "gmm_sample: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    if (int rc = check_fitted(c, K, "gmm_sample")) return rc;
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
     SampleBuffers& sb = c->sample;
@@ -2505,10 +2566,7 @@ int gmm_sample(gmm_ctx* c, int K, long long n, unsigned long long seed, long lon
     if (rc == GMM_OK && n > 0) {
         rc = score_buffers(c);
         if (rc == GMM_OK) rc = sample_batch(c, K, klast, seed, first, n, events_out, labels_out);
-        // nothing of this call may still be in flight when it returns (also after a failure)
-        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
-        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-            rc = fail(GMM_ERR_CUDA, std::string("gmm_sample: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        rc = drain_streams(c, rc, "gmm_sample");
     }
     sb.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
     return rc;
@@ -2531,6 +2589,14 @@ static size_t condition_block_floats(int Kmax, int D) {
     int rec = epack_stride(D);
     for (int o = 1; o < D; o++) rec = std::max(rec, condition_rec_floats(o, D - o, true));
     return (size_t)Kmax * rec;
+}
+
+// gmm_condition's parameter block and its pinned mirror, allocated on the first call of either conditioning call.
+static int condition_block(gmm_ctx* c) {
+    ConditionBuffers& cb = c->cond;
+    if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
+    if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
+    return GMM_OK;
 }
 
 // The parameter block of the current K clusters in the pinned mirror (gmm.h): the marginal set (mu_O, P_O, constant_O,
@@ -2561,13 +2627,7 @@ static int condition_params(gmm_ctx* c, int K, const int* obs, int n_obs, const 
             for (int b = 0; b < n_obs; b++) po[(size_t)k * DO * DO + a * DO + b] = p[(size_t)a * n_obs + b];
         }
     };
-    if (K >= 8) {
-        if (!c->pool) c->pool = new HostPool(c->host_threads);
-        else c->pool->resize(c->host_threads);
-        c->pool->run(K, per_cluster);
-    } else {
-        for (int k = 0; k < K; k++) per_cluster(k);
-    }
+    run_clusters(c, K, K, per_cluster);
     if (first_bad.load() < K)
         return fail(GMM_ERR_STATE, std::string(who) + ": the block P_MM of cluster " + std::to_string(first_bad.load()) +
                                        " (inverse covariance on the missing dimensions) is not positive definite");
@@ -2621,96 +2681,53 @@ static int launch_condition(gmm_ctx* c, int n_obs, int nm, int K, const float* b
     return GMM_OK;
 }
 
-// Chunks of c->score_chunk events through gmm_score's slots, in score_batch's order: host rows -> pinned stage -> (copy
-// stream) device chunk -> (compute stream) kernel -> (copy stream) outputs and imputations -> pinned mirrors -> caller's
-// arrays; chunk i is issued before chunk i - 1 is handed over.
-static int condition_batch(gmm_ctx* c, int K, int n_obs, int nm, bool impute, const float* ev, long long n, int* labels,
-                           float* max_resp, float* logp, float* cmean, float* cvar, double* ll_sum) {
+// gmm_condition's chunks through the pipeline: the marginal score kernel, or the imputing one whose conditional means and
+// variances come back beside the scores.
+static int condition_batch(gmm_ctx* c, int K, int n_obs, int nm, bool impute, const float* ev, long long n, const ScoreOut& out,
+                           float* cmean, float* cvar) {
     ScoreBuffers& s = c->score;
     ConditionBuffers& cb = c->cond;
-    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
-    const size_t var_off = (size_t)chunk * nm;             // cond_var's offset in a slot's imputation buffer
+    const size_t var_off = (size_t)c->score_chunk * nm;    // cond_var's offset in a slot's imputation buffer
     CUDA_TRY(cudaMemcpyAsync(cb.d_block, cb.h_block, sizeof(float) * (size_t)K * condition_rec_floats(n_obs, nm, impute),
                              cudaMemcpyHostToDevice, c->stream));
-    auto issue = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
-        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
-        std::memcpy(s.h_in[b], ev + (size_t)e0 * n_obs, sizeof(float) * (size_t)m * n_obs);
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the chunk buffer's previous kernel is done with it
-        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * n_obs, cudaMemcpyHostToDevice, s.copy));
-        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.d2h[b], 0));    // the slot's previous outputs have left the device
-        const TcScoreIo dv = score_io(c, s.d_out[b], b, m), hv = score_io(c, s.h_out[b], b, m);
+    auto launch = [&](int b, long long, int m) -> int {
+        const TcScoreIo dv = score_io(c, s.d_out[b], b, m);
         CUDA_TRY(cudaMemsetAsync(s.d_out[b], 0, ScoreBuffers::kHeader, c->stream));
         CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
         const int rc = impute ? launch_condition(c, n_obs, nm, K, cb.d_block, dv, cb.d_imp[b], cvar ? cb.d_imp[b] + var_off : nullptr)
                               : launch_score_simt(c, n_obs, K, cb.d_block, dv);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
-        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));
-        CUDA_TRY(cudaMemcpyAsync(s.h_out[b], s.d_out[b], ScoreBuffers::kHeader, cudaMemcpyDeviceToHost, s.copy));
-        if (labels) CUDA_TRY(cudaMemcpyAsync(hv.labels, dv.labels, sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
-        if (max_resp) CUDA_TRY(cudaMemcpyAsync(hv.max_resp, dv.max_resp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
-        if (logp) CUDA_TRY(cudaMemcpyAsync(hv.logp, dv.logp, sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, s.copy));
-        if (impute && cmean)
-            CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b], cb.d_imp[b], sizeof(float) * (size_t)m * nm, cudaMemcpyDeviceToHost, s.copy));
-        if (impute && cvar)
-            CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b] + var_off, cb.d_imp[b] + var_off, sizeof(float) * (size_t)m * nm,
-                                     cudaMemcpyDeviceToHost, s.copy));
-        CUDA_TRY(cudaEventRecord(s.d2h[b], s.copy));
         return GMM_OK;
     };
-    auto finish = [&](long long i) -> int {
-        const int b = (int)(i & 1);
-        const long long e0 = i * chunk;
-        const int m = (int)std::min(chunk, n - e0);
-        CUDA_TRY(cudaEventSynchronize(s.d2h[b]));
-        float ms = 0;
-        if (cudaEventElapsedTime(&ms, s.t0[b], s.t1[b]) == cudaSuccess) cb.kernel_ms += ms;
-        const TcScoreIo hv = score_io(c, s.h_out[b], b, m);
-        *ll_sum += *hv.ll;
-        if (labels) std::memcpy(labels + e0, hv.labels, sizeof(int) * (size_t)m);
-        if (max_resp) std::memcpy(max_resp + e0, hv.max_resp, sizeof(float) * (size_t)m);
-        if (logp) std::memcpy(logp + e0, hv.logp, sizeof(float) * (size_t)m);
+    auto fetch = [&](int b, int m, cudaStream_t st) -> int {
+        if (int rc = fetch_scores(c, out, b, m, st)) return rc;
+        if (impute && cmean) CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b], cb.d_imp[b], sizeof(float) * (size_t)m * nm, cudaMemcpyDeviceToHost, st));
+        if (impute && cvar)
+            CUDA_TRY(cudaMemcpyAsync(cb.h_imp[b] + var_off, cb.d_imp[b] + var_off, sizeof(float) * (size_t)m * nm, cudaMemcpyDeviceToHost, st));
+        return GMM_OK;
+    };
+    auto hand_over = [&](int b, long long e0, int m) -> int {
+        hand_over_scores(c, out, b, e0, m);
         if (impute && cmean) std::memcpy(cmean + (size_t)e0 * nm, cb.h_imp[b], sizeof(float) * (size_t)m * nm);
         if (impute && cvar) std::memcpy(cvar + (size_t)e0 * nm, cb.h_imp[b] + var_off, sizeof(float) * (size_t)m * nm);
         return GMM_OK;
     };
-    for (long long i = 0; i < nchunks; i++) {
-        if (int rc = issue(i)) return rc;
-        if (i > 0)
-            if (int rc = finish(i - 1)) return rc;
-    }
-    return finish(nchunks - 1);
+    return stream_chunks(c, n, ev, n_obs, &cb.kernel_ms, launch, fetch, hand_over);
 }
 
 int gmm_condition(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n, int* labels,
                   float* max_resp, float* logp, float* cond_mean, float* cond_var, double* loglik_out) {
     if (int rc = check_K(c, K, "gmm_condition")) return rc;
     if (n < 0 || (n > 0 && !events_obs)) return fail(GMM_ERR_ARG, "gmm_condition: bad events (n < 0, or no rows)");
-    if (!obs_dims || n_obs < 1 || n_obs > c->D)
-        return fail(GMM_ERR_ARG, "gmm_condition: obs_dims must hold between 1 and D dimension indices");
-    for (int i = 0; i < n_obs; i++)
-        if (obs_dims[i] < 0 || obs_dims[i] >= c->D || (i > 0 && obs_dims[i] <= obs_dims[i - 1]))
-            return fail(GMM_ERR_ARG, "gmm_condition: obs_dims must be strictly increasing indices in [0, D)");
-    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_condition: parameters for this K have not been set");
-    if (c->params_partial)
-        return fail(GMM_ERR_STATE, "gmm_condition: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    int mis[GMM_MAX_DIMENSIONS], nm = 0;
+    unsigned obs_mask = 0;
+    if (int rc = split_obs(c, obs_dims, n_obs, "gmm_condition", mis, &nm, &obs_mask)) return rc;
+    if (int rc = check_fitted(c, K, "gmm_condition")) return rc;
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
     ConditionBuffers& cb = c->cond;
-    if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
-    if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
-    int mis[GMM_MAX_DIMENSIONS];
-    int nm = 0;
-    for (int d = 0, i = 0; d < c->D; d++) {
-        if (i < n_obs && obs_dims[i] == d) i++;
-        else mis[nm++] = d;
-    }
+    if (int rc = condition_block(c)) return rc;
     const bool impute = nm > 0 && (cond_mean || cond_var);
     double ll = 0.0;
     int rc = condition_params(c, K, obs_dims, n_obs, mis, nm, impute);
@@ -2727,11 +2744,9 @@ int gmm_condition(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float
             if (rc == GMM_OK) cb.imp_floats = want;
             else cb.release_imp();
         }
-        if (rc == GMM_OK) rc = condition_batch(c, K, n_obs, nm, impute, events_obs, n, labels, max_resp, logp, cond_mean, cond_var, &ll);
-        // nothing of this call may still be in flight when it returns (also after a failure)
-        const cudaError_t e1 = cudaStreamSynchronize(c->score.copy), e2 = cudaStreamSynchronize(c->stream);
-        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-            rc = fail(GMM_ERR_CUDA, std::string("gmm_condition: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        if (rc == GMM_OK)
+            rc = condition_batch(c, K, n_obs, nm, impute, events_obs, n, {labels, max_resp, logp, &ll}, cond_mean, cond_var);
+        rc = drain_streams(c, rc, "gmm_condition");
         if (rc == GMM_OK && loglik_out) *loglik_out = ll;
     }
     cb.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -2746,19 +2761,16 @@ int gmm_get_condition_profile(gmm_ctx* c, double out[2], int reset) {
 }
 
 // ---- M-step statistics of events measured on a subset of the dimensions ----------------------------------------------------
-// Per chunk i (slot b = i & 1 of gmm_score's input stage), in order on the compute stream: prep kernel (observed SoA copy, the
-// D-row image of the M-step that will run, range flag) -> flag to the host, while chunk i + 1 is staged and its H2D issued ->
-// marginal SIMT E-step of the observed copy into the chunk's responsibilities -> the context's M-step on the D-row image,
-// adding into the call's statistics -> (memberships) pitched D2H and rows to the caller.  The statistics hold T0, T1 and T2 in
-// the entries of the observed dimensions; the caller expands the others on the host (condition_stats_cluster).
+// gmm_condition_stats' chunks through the statistics loop: the prep kernel writes the observed SoA copy and the D-row image
+// of the M-step that will run (a chunk that falls back only because of its flag gets the raw image after the flag is read),
+// then the marginal SIMT E-step of the observed copy and the context's M-step on the D-row image.  The statistics hold T0,
+// T1 and T2 in the entries of the observed dimensions; the caller expands the others on the host (condition_stats_cluster).
 static int condition_stats_batch(gmm_ctx* c, int K, int n_obs, unsigned obs_mask, const float* ev, long long n, bool with_stats,
                                  float* memberships) {
     ScoreBuffers& s = c->score;
     ScoreStatsBuffers& t = c->sstats;
-    StatsProfile& pr = t.cond_prof;
     const int D = c->D;
     const size_t KF = (size_t)K * c->F;
-    const long long chunk = c->score_chunk, nchunks = (n + chunk - 1) / chunk;
     const bool m_tensor = with_stats && use_tensor_mstep(c, K);
     const float* inv_scale_f = m_tensor ? tc_inv_scale_f(c->tc) : nullptr;
     const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
@@ -2768,115 +2780,40 @@ static int condition_stats_batch(gmm_ctx* c, int K, int n_obs, unsigned obs_mask
     CUDA_TRY(cudaMemcpyAsync(t.d_shift_f, shift_f, sizeof(shift_f), cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaMemcpyAsync(c->cond.d_block, c->cond.h_block, sizeof(float) * (size_t)K * epack_stride(n_obs), cudaMemcpyHostToDevice,
                              c->stream));
-    CUDA_TRY(cudaMemsetAsync(t.d_stats, 0, sizeof(double) * (KF + 1), c->stream));
-    auto rows_of = [&](long long i) { return (int)std::min(chunk, n - i * chunk); };
-    auto stage = [&](long long i) -> int {
-        const int b = (int)(i & 1), m = rows_of(i);
-        CUDA_TRY(cudaEventSynchronize(s.h2d[b]));                 // the stage's previous H2D has left it
-        std::memcpy(s.h_in[b], ev + (size_t)(i * chunk) * n_obs, sizeof(float) * (size_t)m * n_obs);
-        CUDA_TRY(cudaStreamWaitEvent(s.copy, s.kern[b], 0));      // the device chunk's previous readers are done with it
-        CUDA_TRY(cudaMemcpyAsync(s.d_in[b], s.h_in[b], sizeof(float) * (size_t)m * n_obs, cudaMemcpyHostToDevice, s.copy));
-        CUDA_TRY(cudaEventRecord(s.h2d[b], s.copy));
-        return GMM_OK;
-    };
     auto prep = [&](int b, int m, float* xo, float* z, float* x) -> int {
         condition_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], m, n_obs, D, obs_mask, t.d_shift_f, inv_scale_f,
                                                                                    zb, xo, z, x, t.pitch, t.d_flag);
         CUDA_TRY(cudaGetLastError());
         return GMM_OK;
     };
-    auto collect = [&](int b) {                                   // timings of a chunk whose kernels have finished
-        float a = 0, k = 0, w = 0;
-        if (cudaEventElapsedTime(&a, t.p0[b], t.p1[b]) == cudaSuccess && cudaEventElapsedTime(&k, t.k0[b], t.k1[b]) == cudaSuccess)
-            pr.kernel_ms += (double)a + (double)k;
-        if (cudaEventElapsedTime(&w, t.p1[b], t.k0[b]) == cudaSuccess) pr.wait_ms += w;
-    };
-    if (nchunks > 0)
-        if (int rc = stage(0)) return rc;
-    for (long long i = 0; i < nchunks; i++) {
-        const int b = (int)(i & 1), m = rows_of(i);
-        const long long e0 = i * chunk;
-        CUDA_TRY(cudaStreamWaitEvent(c->stream, s.h2d[b], 0));
-        CUDA_TRY(cudaMemsetAsync(t.d_flag, 0, sizeof(int), c->stream));
-        CUDA_TRY(cudaEventRecord(t.p0[b], c->stream));
-        if (int rc = prep(b, m, t.d_xo, m_tensor ? t.d_z : nullptr, with_stats && !m_tensor ? t.d_xs : nullptr)) return rc;
-        CUDA_TRY(cudaEventRecord(t.p1[b], c->stream));
-        CUDA_TRY(cudaMemcpyAsync(t.h_flag, t.d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
-        CUDA_TRY(cudaEventRecord(t.ev_flag, c->stream));
-        if (i + 1 < nchunks)
-            if (int rc = stage(i + 1)) return rc;
-        CUDA_TRY(cudaEventSynchronize(t.ev_flag));
-        if (i > 0) collect(b ^ 1);                                // (the prep of chunk i ran after chunk i - 1's kernels)
-        const int flag = *t.h_flag;
-        if (flag & kScoreStatsNotFinite) return fail(GMM_ERR_ARG, "gmm_condition_stats: an event has a coordinate that is not finite");
-        const bool cm = m_tensor && !(flag & kScoreStatsBeyondZb);
-        if (m_tensor && !cm && mstep_path_of(c) == GMM_PATH_TENSOR)
-            return fail(GMM_ERR_STATE, "gmm_condition_stats: an event lies beyond the tensor M-step's fixed-point range (|z| >= the "
-                                       "training data's bound) and mstep_path is GMM_PATH_TENSOR");
-        CUDA_TRY(cudaEventRecord(t.k0[b], c->stream));
+    auto estep = [&](int b, int m, bool, bool cm) -> int {
         if (m_tensor && !cm)                                      // a fallback of this chunk only: its raw image now
             if (int rc = prep(b, m, nullptr, nullptr, t.d_xs)) return rc;
-        int rc = launch_estep_simt_on(c, n_obs, K, c->cond.d_block, t.d_xo, m, t.d_memb, t.pitch, t.d_stats + KF);
-        if (rc) return rc;
-        pr.e_simt++;
-        CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
-        if (with_stats) {
-            rc = cm ? tc_launch_mstep_on(c->tc, K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
-                    : launch_mstep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats);
-            if (rc) return rc;
-            (cm ? pr.m_tensor : pr.m_simt)++;
-        }
-        CUDA_TRY(cudaEventRecord(t.k1[b], c->stream));
-        if (memberships) {
-            CUDA_TRY(cudaMemcpy2DAsync(t.h_memb, sizeof(float) * (size_t)m, t.d_memb, sizeof(float) * t.pitch, sizeof(float) * (size_t)m, K,
-                                       cudaMemcpyDeviceToHost, c->stream));
-            CUDA_TRY(cudaStreamSynchronize(c->stream));
-            for (int k = 0; k < K; k++)
-                std::memcpy(memberships + (size_t)k * n + e0, t.h_memb + (size_t)k * m, sizeof(float) * (size_t)m);
-        }
-    }
-    if (with_stats) CUDA_TRY(cudaMemcpyAsync(t.h_stats, t.d_stats, sizeof(double) * (KF + 1), cudaMemcpyDeviceToHost, c->stream));
-    CUDA_TRY(cudaStreamSynchronize(c->stream));
-    if (nchunks > 0) collect((int)((nchunks - 1) & 1));
-    return GMM_OK;
+        return launch_estep_simt_on(c, n_obs, K, c->cond.d_block, t.d_xo, m, t.d_memb, t.pitch, t.d_stats + KF);
+    };
+    return stats_batch(c, K, ev, n_obs, n, with_stats, memberships, false, m_tensor, t.cond_prof, "gmm_condition_stats",
+                       [&](int b, int m) { return prep(b, m, t.d_xo, m_tensor ? t.d_z : nullptr, with_stats && !m_tensor ? t.d_xs : nullptr); },
+                       estep);
 }
 
 int gmm_condition_stats(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float* events_obs, long long n, double* stats_out,
                         double* shift_out, float* memberships) {
     if (int rc = check_K(c, K, "gmm_condition_stats")) return rc;
     if (n < 0 || (n > 0 && !events_obs)) return fail(GMM_ERR_ARG, "gmm_condition_stats: bad events (n < 0, or no rows)");
-    if (!obs_dims || n_obs < 1 || n_obs > c->D)
-        return fail(GMM_ERR_ARG, "gmm_condition_stats: obs_dims must hold between 1 and D dimension indices");
-    for (int i = 0; i < n_obs; i++)
-        if (obs_dims[i] < 0 || obs_dims[i] >= c->D || (i > 0 && obs_dims[i] <= obs_dims[i - 1]))
-            return fail(GMM_ERR_ARG, "gmm_condition_stats: obs_dims must be strictly increasing indices in [0, D)");
+    int mis[GMM_MAX_DIMENSIONS], nm = 0;
+    unsigned obs_mask = 0;
+    if (int rc = split_obs(c, obs_dims, n_obs, "gmm_condition_stats", mis, &nm, &obs_mask)) return rc;
     if (!stats_out && !memberships) return fail(GMM_ERR_ARG, "gmm_condition_stats: neither statistics nor memberships requested");
-    if (K != c->cur_K) return fail(GMM_ERR_STATE, "gmm_condition_stats: parameters for this K have not been set");
-    if (c->params_partial)
-        return fail(GMM_ERR_STATE, "gmm_condition_stats: gmm_mstep has updated N, means and R but not the inverses; run gmm_constants first");
+    if (int rc = check_fitted(c, K, "gmm_condition_stats")) return rc;
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
-    if (!c->have_shift) {
-        // the centre comes from the global column moments, an all-reduce over the ranks: never issued from here
-        if (c->nranks > 1)
-            return fail(GMM_ERR_STATE, "gmm_condition_stats: the context's centre is not fixed yet (run gmm_mstep or gmm_em first on every rank)");
-        if (int rc = ensure_moments(c)) return rc;
-    }
+    if (int rc = ensure_centre(c, "gmm_condition_stats")) return rc;
     const int D = c->D;
-    int mis[GMM_MAX_DIMENSIONS];
-    int nm = 0;
-    unsigned obs_mask = 0;
-    for (int d = 0, i = 0; d < D; d++) {
-        if (i < n_obs && obs_dims[i] == d) { obs_mask |= 1u << d; i++; }
-        else mis[nm++] = d;
-    }
     const size_t len = (size_t)K * c->F + 1;
     std::vector<double> g, cm;                              // per cluster G [nm][n_obs] and C = S_MM^-1 [nm][nm], in double
     int rc = GMM_OK;
-    ConditionBuffers& cb = c->cond;
     if (nm > 0) {
-        if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, D)));
-        if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, D)));
+        if (int rc = condition_block(c)) return rc;
         g.resize((size_t)K * nm * n_obs);
         cm.resize((size_t)K * nm * nm);
         rc = condition_params(c, K, obs_dims, n_obs, mis, nm, false, "gmm_condition_stats", g.data(), cm.data());
@@ -2887,28 +2824,17 @@ int gmm_condition_stats(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const
         if (rc == GMM_OK)
             rc = nm > 0 ? condition_stats_batch(c, K, n_obs, obs_mask, events_obs, n, stats_out != nullptr, memberships)
                         : score_stats_batch(c, K, events_obs, n, stats_out != nullptr, memberships, c->sstats.cond_prof);
-        // nothing of this call may still be in flight when it returns (also after a failure)
-        const cudaError_t e1 = c->score.copy ? cudaStreamSynchronize(c->score.copy) : cudaSuccess, e2 = cudaStreamSynchronize(c->stream);
-        if (rc == GMM_OK && (e1 != cudaSuccess || e2 != cudaSuccess))
-            rc = fail(GMM_ERR_CUDA, std::string("gmm_condition_stats: ") + cudaGetErrorString(e1 != cudaSuccess ? e1 : e2));
+        rc = drain_streams(c, rc, "gmm_condition_stats");
     }
     if (rc == GMM_OK) {
         if (stats_out) {
             if (n > 0) std::memcpy(stats_out, c->sstats.h_stats, sizeof(double) * len);
             else std::fill(stats_out, stats_out + len, 0.0);
-            if (n > 0 && nm > 0) {
-                const std::function<void(int)> per_cluster = [&](int k) {
+            if (n > 0 && nm > 0)
+                run_clusters(c, K, K, [&](int k) {
                     condition_stats_cluster(stats_out + (size_t)k * c->F, D, obs_dims, n_obs, mis, nm, c->host.means + (size_t)k * D, c->shift,
                                             &g[(size_t)k * nm * n_obs], &cm[(size_t)k * nm * nm]);
-                };
-                if (K >= 8) {
-                    if (!c->pool) c->pool = new HostPool(c->host_threads);
-                    else c->pool->resize(c->host_threads);
-                    c->pool->run(K, per_cluster);
-                } else {
-                    for (int k = 0; k < K; k++) per_cluster(k);
-                }
-            }
+                });
         }
         if (shift_out) std::memcpy(shift_out, c->shift, sizeof(double) * (size_t)D);
     }
@@ -3007,9 +2933,8 @@ int gmm_fit(gmm_ctx* c, int K0, int target_K, int min_iters, int max_iters, clus
         }
         if (K > stop_number) {                                            // :860-950
             const auto t0 = now();
-            if (!c->pool) c->pool = new HostPool(c->host_threads);
-            else c->pool->resize(c->host_threads);
-            const ParallelFor pfor = [&](int n, const std::function<void(int)>& fn) { c->pool->run(n, fn); };
+            HostPool* pool = host_pool(c);
+            const ParallelFor pfor = [&](int n, const std::function<void(int)>& fn) { pool->run(n, fn); };
             K = reduce_order(&c->host, K, D, nullptr, nullptr, c->host_threads, &pfor);
             c->fit_reduce_ms += ms_since(t0);
             if (K < 1) break;
