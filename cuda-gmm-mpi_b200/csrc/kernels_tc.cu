@@ -612,6 +612,51 @@ template <int D> struct ECfg {
     static constexpr int THREADS = 128 * NWG;
 };
 
+// Launch configuration of estep_tc_kernel (score_tc_kernel keeps ECfg's): two MMA warpgroups and two epilogue warpgroups
+// per CTA.  An MMA warpgroup writes the base-2 logits of its tile to a slot of a ring in shared memory; epilogue warpgroup
+// j takes the tiles of MMA warpgroup j from the ring and does their log-sum-exp, log-likelihood and stores.
+//   slot   [64 events][64 clusters] fp32, 256 B per event; the 4-cluster chunk c of event e at chunk c ^ slot_swz(e)
+//   stat   [slot][64 events] fp32 subtrahend (the row maximum, or the known log-denominator in base 2), then the scale
+//   full / empty  [slot][use parity] mbarriers, 128 arrivals each (the writing MMA warpgroup / the reading epilogue
+//                 warpgroup).  Use u of slot s is tile 3 u + s, so successive uses of a slot alternate between the two
+//                 warpgroup pairs; with one barrier per use parity each barrier serves one pair only and no waiter can
+//                 be two phases behind it (a parity wait on a barrier two phases behind would pass at once).
+// D = 8 keeps the fused schedule (estep_fused) and ECfg's configuration.
+template <int D> struct EsCfg {
+    using E = ECfg<D>;
+    static constexpr bool SPLIT = D > 8;
+    static constexpr int NMMA = 2;                             // MMA warpgroups, and as many epilogue warpgroups
+    static constexpr int THREADS = SPLIT ? 128 * 2 * NMMA : E::THREADS;
+    static constexpr int NSLOT = 3;
+    static constexpr int SLOT = 64 * 64 * 4;
+    static constexpr int OFF_SLOT = (E::SMEM_BYTES + 127) / 128 * 128;
+    static constexpr int OFF_STAT = OFF_SLOT + NSLOT * SLOT;
+    static constexpr int OFF_EBAR = OFF_STAT + NSLOT * 2 * 64 * 4;
+    static constexpr int SMEM_BYTES = SPLIT ? OFF_EBAR + 4 * NSLOT * 8 : E::SMEM_BYTES;
+    // register pools (setmaxnreg redistributes the launch allocation of REG_LAUNCH per thread, see MCfg)
+    static constexpr int REG_LAUNCH = 65536 / (128 * 2 * NMMA) / 8 * 8;
+    static constexpr int REG_MMA = 184;
+    static constexpr int REG_EPI = 72;
+    static_assert(128 * NMMA * (REG_MMA + REG_EPI) <= 128 * 2 * NMMA * REG_LAUNCH, "register pools");
+    static_assert(SMEM_BYTES <= 232448, "shared memory budget");
+};
+
+// Physical chunk offset of event e in a logit slot.  Conflict-free (one wavefront per 8 lanes of a 16-byte access) for
+// the three access patterns: the MMA lanes' writes (a quarter warp: events e, e + 1, every chunk of a supergroup), the
+// epilogue's row reads (4 consecutive events, chunks c, c ^ 1) and its block reads (one chunk, events 4a + j, 8 values of a).
+__device__ __forceinline__ uint32_t slot_swz(int e) { return (uint32_t)(((e & 1) << 2 | (e & 2)) ^ ((e >> 2) & 7)); }
+
+__device__ __forceinline__ void sts_f4(uint32_t addr, float a, float b, float c, float d) {
+    asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+}
+__device__ __forceinline__ float4 lds_f4(uint32_t addr) {
+    float4 v;
+    asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+// named barrier 1 + j of epilogue warpgroup j alone (barrier 0 is __syncthreads)
+__device__ __forceinline__ void epi_bar(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
 // Timing variants of the E-step for scripts/prof_estep.py (`make variant DEFS=-DGMM_ESTEP_CUT=n`); the default build is 0.
 //   1  MMA only: the accumulators feed one sum per block, no squares, log-sum-exp, exp, log or stores (results are wrong)
 //   2  no stores: the full epilogue, but the responsibilities are not written
@@ -771,9 +816,81 @@ __device__ __forceinline__ void tc_tile_logits(const uint32_t (&zh)[D / 8][2], c
     }
 }
 
-template <int D, int NSG, bool WT = false>
-__global__ void __launch_bounds__(ECfg<D>::THREADS, 1)
-estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
+// The MMA side of one 64-event tile of the E-step: the groups, squares and quad transpose of tc_tile_logits in the same
+// order, over a ring of two accumulators (group g + 1 is issued and committed before group g is waited for and squared; a
+// third accumulator fits the register pool without spills but measured slower), and each supergroup's 8 base-2 logits per thread written to the logit slot at `slot` (two 16-byte
+// stores: 4 clusters of one event each) instead of being kept in registers.  Supergroups >= NSG are not written: the
+// epilogue does not read them.
+template <int D, int NSG>
+__device__ __forceinline__ void estep_tile_logits(const uint32_t (&zh)[D / 8][2], const uint32_t (&zl)[D / 8][2], uint32_t bsm,
+                                                  const float* ck_s, int qd, uint32_t ones, uint32_t slot, int r0, float& cut_sum) {
+    using C = ECfg<D>;
+    constexpr int CP = C::CP, NG = NSG * CP * 2;
+    float acc[2][32];
+    tc_issue_group<D>(acc[0], zh, zl, bsm, 0, 0, ones);
+    wgmma_commit();
+    const uint32_t cq = 2 * (qd & 1) + (qd >> 1);             // this lane's chunk of 4 clusters within a supergroup
+    const uint32_t row0 = slot + (uint32_t)r0 * 256, row1 = row0 + 8 * 256;
+    const uint32_t sw0 = slot_swz(r0), sw1 = slot_swz(r0 + 8);
+    float sq[32];                                             // sums of squares of a supergroup: [cluster 0..15][row]
+#pragma unroll
+    for (int g = 0; g < NG; g++) {
+        const int sg = g / (2 * CP), c = (g / 2) % CP, h = g & 1;
+        if (c == 0 && h == 0) {
+#pragma unroll
+            for (int u = 0; u < 32; u++) sq[u] = 0.f;
+        }
+        // queue group g + 1, then wait for group g (all conditions are compile-time)
+        if (g + 1 < NG) {
+            const int gn = g + 1;
+            tc_issue_group<D>(acc[gn & 1], zh, zl, bsm + (uint32_t)(gn / (2 * CP)) * C::B_SG, (gn / 2) % CP, gn & 1, ones);
+            wgmma_commit();
+            wgmma_wait<1>();
+        } else {
+            wgmma_wait<0>();
+        }
+        wgmma_pin(acc[g & 1]);
+        const float(&a)[32] = acc[g & 1];
+#if GMM_ESTEP_CUT == 1
+        cut_sum += a[0];
+#else
+#pragma unroll
+        for (int i = 0; i < 8; i++) {
+            float& s0 = sq[16 * h + 2 * i];
+            float& s1 = sq[16 * h + 2 * i + 1];
+            s0 = fmaf(a[4 * i], a[4 * i], fmaf(a[4 * i + 1], a[4 * i + 1], s0));
+            s1 = fmaf(a[4 * i + 2], a[4 * i + 2], fmaf(a[4 * i + 3], a[4 * i + 3], s1));
+        }
+        if (c == CP - 1 && h == 1) {
+            // sum over the quad, transposing as it goes (tc_tile_logits): lane qd ends with clusters cb .. cb+3 of the
+            // supergroup, cb = 8 (qd & 1) + 4 (qd >> 1) = 4 cq, both rows
+            float w[16];
+            const bool b1 = qd & 1, b2 = (qd >> 1) & 1;
+#pragma unroll
+            for (int u = 0; u < 16; u++) {
+                const float send = b1 ? sq[u] : sq[16 + u], keep = b1 ? sq[16 + u] : sq[u];
+                w[u] = keep + __shfl_xor_sync(0xffffffffu, send, 1);
+            }
+            float l[8];
+#pragma unroll
+            for (int u = 0; u < 8; u++) {
+                const float send = b2 ? w[u] : w[8 + u], keep = b2 ? w[8 + u] : w[u];
+                const float qv = keep + __shfl_xor_sync(0xffffffffu, send, 2);
+                const int k = sg * C::GB + 8 * (qd & 1) + 4 * (qd >> 1) + (u >> 1);
+                l[u] = fmaf(ck_s[64 + k], qv, ck_s[k]);
+            }
+            const uint32_t ch = 4 * (uint32_t)sg + cq;
+            sts_f4(row0 + ((ch ^ sw0) << 4), l[0], l[2], l[4], l[6]);
+            sts_f4(row1 + ((ch ^ sw1) << 4), l[1], l[3], l[5], l[7]);
+        }
+#endif
+    }
+}
+
+// The fused schedule (D = 8): two warpgroups, each doing the MMAs, log-sum-exp and stores of its own tiles, with
+// ECfg's launch configuration.  Called by estep_tc_kernel; see there for the modes.
+template <int D, int NSG, bool WT>
+__device__ __forceinline__ void estep_fused(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
                 const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float* __restrict__ memb,
                 size_t pitch, int n, int K, double* __restrict__ ll_out, int mode, const float* den_in, float* den_out,
                 const float* __restrict__ wts) {
@@ -909,6 +1026,204 @@ estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
         ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 2);
         ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 1);
         if (lane == 0) atomicAdd(ll_out, ll_acc);
+    }
+}
+
+template <int D, int NSG, bool WT = false>
+__global__ void __launch_bounds__(EsCfg<D>::THREADS, 1)
+estep_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_img, const float* __restrict__ ck,
+                const float* __restrict__ shift_f, const float* __restrict__ inv_scale_f, float* __restrict__ memb,
+                size_t pitch, int n, int K, double* __restrict__ ll_out, int mode, const float* den_in, float* den_out,
+                const float* __restrict__ wts) {
+    // K / NSG (= ceil(K / 16)) / b_img / ck / memb describe ONE pass of at most 64 clusters.  More than 64 clusters take 2P - 1 launches
+    // for P passes, and every responsibility is written exactly once:
+    //   mode 1 (passes 0 .. P-2)  log-denominator only: den_out[e] = ln(sum_k exp(logit)) (+ den_in[e] in log space), no stores
+    //   mode 2 (pass P-1)         its own log-sum-exp joined with den_in[e] (all other passes): final responsibilities of this
+    //                             pass, den_out[e] = the event's total log-denominator, log-likelihood
+    //   mode 3 (passes 0 .. P-2)  responsibilities against the known total den_in[e]: no log-sum-exp
+    //   mode 0                    single pass (K <= 64)
+    // WT (gmm_set_weights): the log-likelihood adds wts[e] * denominator; the responsibilities do not depend on the weights.
+    if constexpr (!EsCfg<D>::SPLIT) {
+        estep_fused<D, NSG, WT>(x_aos, b_img, ck, shift_f, inv_scale_f, memb, pitch, n, K, ll_out, mode, den_in, den_out, wts);
+        return;
+    } else {
+    // The CTA's tile i (i = 0, 1, ...) is tile blockIdx.x * NMMA + i % NMMA + (i / NMMA) * stride of the grid; MMA
+    // warpgroup i % NMMA writes its logits to slot i % NSLOT, and epilogue warpgroup i % NMMA reads them from there.
+    using E = ECfg<D>;
+    using C = EsCfg<D>;
+    constexpr int CP = E::CP;
+    extern __shared__ __align__(1024) uint8_t smem[];
+    uint64_t* b_full = reinterpret_cast<uint64_t*>(smem + E::OFF_BAR);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + C::OFF_EBAR);   // [NSLOT][2] logits written
+    uint64_t* empty = full + 2 * C::NSLOT;                              // [NSLOT][2] logits read
+    const float* ck_s = reinterpret_cast<const float*>(smem + E::OFF_CK);   // [64] additive logit constants, [64] multipliers
+    const float* sh_s = reinterpret_cast<const float*>(smem + E::OFF_SH);   // [32] shift, [32] inverse scale
+    const float* isc_s = sh_s + 32;
+    const uint32_t slots = smem_u32(smem + C::OFF_SLOT);
+
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int ntiles = (n + 63) / 64;
+    const int stride = (int)gridDim.x * C::NMMA;
+    if (threadIdx.x == 0) {
+        for (int b = 0; b < 2 * C::NSLOT; b++) { mbar_init(&full[b], 128); mbar_init(&empty[b], 128); }
+    }
+    tc_stage_operand<D>(smem, b_img, ck, shift_f, inv_scale_f, NSG);   // fences the barrier inits, then __syncthreads
+
+    if (wg < C::NMMA) {
+        // ---- MMA warpgroup: logits of tiles wg, wg + NMMA, ... of the CTA ----
+        set_regs<C::REG_MMA, C::REG_LAUNCH>();
+        const int gid = lane >> 2, qd = lane & 3;
+        // rows r0 = 16 warp + gid and r1 = r0 + 8 of each 64-event tile; K positions 2 qd, 2 qd + 1 of every 8-wide chunk
+        const int r0 = warp * 16 + gid;
+        float2 xa[CP], xb[CP];                     // raw coordinates of the two rows (prefetched one tile ahead)
+        auto load_rows = [&](int t) {
+            const long long e0 = (long long)t * 64 + r0, e1 = e0 + 8;
+#pragma unroll
+            for (int j = 0; j < CP; j++) {
+                xa[j] = e0 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e0 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+                xb[j] = e1 < n ? __ldg(reinterpret_cast<const float2*>(x_aos + (size_t)e1 * D + 8 * j + 2 * qd)) : make_float2(0.f, 0.f);
+            }
+        };
+        int t = (int)blockIdx.x * C::NMMA + wg;
+        if (t < ntiles) load_rows(t);
+        const uint32_t ones = qd == 0 ? 0x3C003C00u : 0u;         // chunk {1, 1, 0 ...}: K elements 0 and 1 are held by qd == 0
+        const uint32_t bsm = smem_u32(smem + E::OFF_B);
+        float cut_sum = 0.f;
+        mbar_wait(b_full, 0);
+        for (int i = wg; t < ntiles; t += stride, i += C::NMMA) {
+            uint32_t zh[CP][2], zl[CP][2];                         // [chunk][row]: FP16 pairs, hi and lo parts
+            tc_split_rows<D>(xa, xb, sh_s, isc_s, qd, zh, zl);
+            if (t + stride < ntiles) load_rows(t + stride);
+            const int s = i % C::NSLOT, u = i / C::NSLOT;           // use u of slot s
+#if GMM_ESTEP_CUT != 1
+            if (u > 0) mbar_wait(&empty[2 * s + ((u - 1) & 1)], ((u - 1) >> 1) & 1);   // use u - 1 read
+#endif
+            estep_tile_logits<D, NSG>(zh, zl, bsm, ck_s, qd, ones, slots + (uint32_t)s * C::SLOT, r0, cut_sum);
+#if GMM_ESTEP_CUT != 1
+            mbar_arrive(&full[2 * s + (u & 1)]);
+#endif
+        }
+        if (GMM_ESTEP_CUT == 1 && cut_sum == -1.f) atomicAdd(ll_out, 0.0);   // keeps the variant's MMAs alive
+        return;
+    }
+
+    // ---- epilogue warpgroup ew: the tiles of MMA warpgroup ew ----
+    set_regs<C::REG_EPI, C::REG_LAUNCH>();
+    if (GMM_ESTEP_CUT == 1) return;
+    const int ew = wg - C::NMMA, et = threadIdx.x & 127;
+    // log-sum-exp: two threads per event (ev = et / 2); thread hh holds the P sums of lanes qd = 2 hh and 2 hh + 1 of the
+    // MMA quad, i.e. the chunks 4 sg + hh and 4 sg + 2 + hh of every supergroup
+    const int ev = et >> 1, hh = et & 1;
+    const uint32_t evrow = (uint32_t)ev * 256, evswz = slot_swz(ev);
+    float* stat = reinterpret_cast<float*>(smem + C::OFF_STAT);          // [NSLOT][subtrahend 64 | scale 64]
+    const uint32_t stat_u = smem_u32(stat);
+    double ll_acc = 0.0;
+    constexpr float kLn2 = 0.6931471805599453f, kLog2e = 1.4426950408889634f;
+    for (int i = ew;; i += C::NMMA) {
+        const int t = (int)blockIdx.x * C::NMMA + i % C::NMMA + (i / C::NMMA) * stride;
+        if (t >= ntiles) break;
+        const int s = i % C::NSLOT;
+        const uint32_t slot = slots + (uint32_t)s * C::SLOT;
+        const int u = i / C::NSLOT, sb2 = 2 * s + (u & 1);
+        mbar_wait(&full[sb2], (u >> 1) & 1);
+        const long long e = (long long)t * 64 + ev;
+        float sub, scl = 1.f, dep = 0.f;
+        if (mode == 3) {
+            // the event's total log-denominator is known: gamma = 2^(l2 - denom * log2 e)
+            sub = e < n ? den_in[e] * kLog2e : 0.f;
+        } else {
+            // log-sum-exp over the clusters (estep2, gaussian_kernel.cu:481-503)
+            float mx = -INFINITY;
+#pragma unroll
+            for (int sg = 0; sg < NSG; sg++)
+#pragma unroll
+                for (int j = 0; j < 2; j++) {
+                    const float4 v = lds_f4(slot + evrow + (((uint32_t)(4 * sg + 2 * j + hh) ^ evswz) << 4));
+                    mx = fmaxf(fmaxf(mx, v.x), fmaxf(fmaxf(v.y, v.z), v.w));
+                }
+            mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+            // S = (P0 + P1) + (P2 + P3), each P_qd = 0 + its 16 terms in (supergroup, cluster) order: the sums of the
+            // MMA quad's lanes and of its two shuffle steps, bit for bit
+            float p0 = 0.f, p1 = 0.f;
+#pragma unroll
+            for (int sg = 0; sg < NSG; sg++) {
+                const float4 v0 = lds_f4(slot + evrow + (((uint32_t)(4 * sg + hh) ^ evswz) << 4));
+                const float4 v1 = lds_f4(slot + evrow + (((uint32_t)(4 * sg + 2 + hh) ^ evswz) << 4));
+                p0 += ex2_approx(v0.x - mx); p0 += ex2_approx(v0.y - mx); p0 += ex2_approx(v0.z - mx); p0 += ex2_approx(v0.w - mx);
+                p1 += ex2_approx(v1.x - mx); p1 += ex2_approx(v1.y - mx); p1 += ex2_approx(v1.z - mx); p1 += ex2_approx(v1.w - mx);
+            }
+            const float a = p0 + p1;
+            const float S = a + __shfl_xor_sync(0xffffffffu, a, 1);
+            sub = mx;
+            dep = S;
+            if (hh == 0) {
+                float denom = fmaf(mx, kLn2, logf(S));              // :490-494, back in natural units
+                scl = 1.0f / S;                                     // exp(l - denom) = 2^(l2 - M) / S
+                if (mode != 0 && e < n) {
+                    if (den_in != nullptr) {                        // join with the other passes' log-denominator
+                        const float dx = den_in[e];                 // den_in may alias den_out: read before the write
+                        const float g = fmaxf(denom, dx);
+                        const float tot = g + logf(__expf(denom - g) + __expf(dx - g));
+                        scl *= __expf(denom - tot);
+                        denom = tot;
+                    }
+                    den_out[e] = denom;
+                }
+                if constexpr (WT) {
+                    if (e < n && (mode == 0 || mode == 2)) ll_acc += (double)wts[e] * (double)denom;
+                } else {
+                    if (e < n && (mode == 0 || mode == 2)) ll_acc += (double)denom;
+                }
+            }
+        }
+        if (mode == 1 || GMM_ESTEP_CUT == 2) {
+            mbar_arrive_after(&empty[sb2], dep);
+            continue;
+        }
+        if (hh == 0) { stat[s * 128 + ev] = sub; stat[s * 128 + 64 + ev] = scl; }
+        epi_bar(1 + ew);
+        // responsibilities (:498-501) in blocks of 4 events x 4 clusters: lanes 16 b .. 16 b + 15 of a warp hold the 64
+        // events of one chunk, so each 16-byte store instruction writes 256 contiguous bytes of each of two cluster rows.
+        // Rows [K, 8*ceil(K/8)) are written too (zeros of the padding clusters): the buffer is allocated in multiples of 8 rows.
+#pragma unroll 1
+        for (int j = 0; j < 2; j++) {
+            const int b = et + 128 * j, c = b >> 4, a = b & 15;
+            if (c >= 4 * NSG || (4 * c & ~7) >= K) continue;
+            float4 v[4];
+#pragma unroll
+            for (int m = 0; m < 4; m++) v[m] = lds_f4(slot + (uint32_t)(4 * a + m) * 256 + (((uint32_t)c ^ slot_swz(4 * a + m)) << 4));
+            const float4 sb = lds_f4(stat_u + (uint32_t)s * 512 + 16 * a), sc = lds_f4(stat_u + (uint32_t)s * 512 + 256 + 16 * a);
+            dep += (v[0].x + v[1].x) + (v[2].x + v[3].x);
+            const long long e0 = (long long)t * 64 + 4 * a;
+            float* dst = memb + (size_t)(4 * c) * pitch + e0;
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+                const float l0 = q == 0 ? v[0].x : q == 1 ? v[0].y : q == 2 ? v[0].z : v[0].w;
+                const float l1 = q == 0 ? v[1].x : q == 1 ? v[1].y : q == 2 ? v[1].z : v[1].w;
+                const float l2 = q == 0 ? v[2].x : q == 1 ? v[2].y : q == 2 ? v[2].z : v[2].w;
+                const float l3 = q == 0 ? v[3].x : q == 1 ? v[3].y : q == 2 ? v[3].z : v[3].w;
+                const float4 gm = make_float4(ex2_approx(l0 - sb.x) * sc.x, ex2_approx(l1 - sb.y) * sc.y, ex2_approx(l2 - sb.z) * sc.z,
+                                              ex2_approx(l3 - sb.w) * sc.w);
+                float* row = dst + (size_t)q * pitch;
+                if (e0 + 3 < n) {
+                    *reinterpret_cast<float4*>(row) = gm;
+                } else {
+                    if (e0 < n) row[0] = gm.x;
+                    if (e0 + 1 < n) row[1] = gm.y;
+                    if (e0 + 2 < n) row[2] = gm.z;
+                }
+            }
+        }
+        mbar_arrive_after(&empty[sb2], dep);
+    }
+    if (mode == 0 || mode == 2) {
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 16);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 8);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 4);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 2);
+        ll_acc = ll_acc + __shfl_down_sync(0xffffffffu, ll_acc, 1);
+        if (lane == 0) atomicAdd(ll_out, ll_acc);
+    }
     }
 }
 
@@ -1744,7 +2059,7 @@ template <int D>
 static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb, size_t pitch, float* den, double* d_ll, const float* w,
                           cudaStream_t stream) {
     using C = ECfg<D>;
-    static_assert(C::SMEM_BYTES <= 232448, "shared memory budget");
+    using L = EsCfg<D>;
     // one instance per number of resident supergroups (1 .. 4) of a pass, unweighted and weighted
     using KernFn = void (*)(const float*, const uint8_t*, const float*, const float*, const float*, float*, size_t, int, int, double*, int,
                             const float*, float*, const float*);
@@ -1753,8 +2068,8 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
                                            estep_tc_kernel<D, 4, true>};
     static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_estep) {
-        for (auto* k : kern0) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
-        for (auto* k : kern1) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern0) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
+        for (auto* k : kern1) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
         t->attr_estep = true;
     }
     const KernFn* kern = w ? kern1 : kern0;
@@ -1769,7 +2084,7 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
     // theirs against those totals (mode 3): 2P - 1 launches, every responsibility stored once
     auto launch = [&](int p, int mode, const float* den_in, float* den_out) {
         const int Kp = K - 64 * p < 64 ? K - 64 * p : 64;
-        kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
+        kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, L::THREADS, L::SMEM_BYTES, stream>>>(
             x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f,
             memb + (size_t)(64 * p) * pitch, pitch, n, Kp, d_ll, mode, den_in, den_out, w);
         return cudaGetLastError();

@@ -10,12 +10,19 @@ then
 Per library and shape: the parameters of the seed (valid whatever the variant computes: the E-step alone is timed, no
 M-step runs), 5 warm-up launches, then the CUDA-event time of `--launches` E-step launches (the engine's per-phase timer
 brackets the kernel launches only); the median of 3 such blocks is printed as ms per launch, with the tensor floor of the
-MMAs at the card's maximum SM clock for comparison.  The card's name, power limit, maximum SM clock and the SM clock read
-right after the timed blocks are printed first.  Needs a GPU; the E-step runs on the tensor path only (no SIMT fall-back).
+MMAs at the card's maximum SM clock for comparison and the measured fraction of that floor.  The card's name, power limit,
+maximum SM clock and the SM clock read right after the timed blocks are printed first.  Needs a GPU; the E-step runs on the
+tensor path only (no SIMT fall-back).
+
+A variant is only a valid cut when it issues every MMA of the full build: the compiler may drop the MMAs whose results a
+variant no longer uses.  Each library's `HGMMA` count over the estep_tc_kernel instances (`cuobjdump -sass`) is printed
+and a library whose count differs from the in-tree build's is flagged `"valid": false`.
 """
 import argparse
 import json
 import os
+import re
+import shutil
 import subprocess
 import sys
 
@@ -44,6 +51,26 @@ def mma_cycles_per_sm(N, D, K, sms):
     ksteps = sum((cp - c) + (cp - c + 2) // 2 for c in range(cp)) * ((K + 15) // 16)
     tiles = (N + 63) // 64
     return tiles * ksteps * 64 / sms
+
+
+def lib_path(lib):
+    return os.path.join(ROOT, "cuda-gmm-mpi_b200", "libgmm_b200.so") if lib == "default" else os.path.abspath(lib)
+
+
+def estep_hgmma(path):
+    """HGMMA instructions in the SASS of the library's estep_tc_kernel instances (None when cuobjdump is not found)."""
+    tool = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
+    if not os.path.exists(tool):
+        return None
+    sass = subprocess.run([tool, "-sass", path], capture_output=True, text=True, timeout=600).stdout
+    count, inside = 0, False
+    for ln in sass.splitlines():
+        m = re.search(r"Function : (\S+)", ln)
+        if m:
+            inside = "estep_tc_kernel" in m.group(1)
+        elif inside and re.search(r"\bHGMMA\.", ln):
+            count += 1
+    return count
 
 
 def run_one(shape, launches):
@@ -84,13 +111,18 @@ def main():
     except ValueError:
         max_mhz = float("nan")
     sms = torch.cuda.get_device_properties(0).multi_processor_count
+    full = estep_hgmma(lib_path("default"))
+    hgmma = {lib: estep_hgmma(lib_path(lib)) for lib in a.libs}
+    for lib in a.libs:
+        print(json.dumps(dict(lib=os.path.basename(lib), estep_hgmma=hgmma[lib], in_tree_hgmma=full,
+                              valid=hgmma[lib] is not None and hgmma[lib] == full)), flush=True)
     for shape in a.shapes.split(","):
         N, D, K = SHAPES[shape]
         floor = mma_cycles_per_sm(N, D, K, sms) / (max_mhz * 1e3)
         for lib in a.libs:
             env = dict(os.environ)
             if lib != "default":
-                env["GMM_B200_LIB"] = os.path.abspath(lib)
+                env["GMM_B200_LIB"] = lib_path(lib)
             r = subprocess.run([sys.executable, os.path.abspath(__file__), "--one", shape, "--launches", str(a.launches)], env=env,
                                capture_output=True, text=True, timeout=1200)
             lines = r.stdout.strip().splitlines()
@@ -100,6 +132,8 @@ def main():
             res = json.loads(lines[-1])
             res["lib"] = os.path.basename(lib)
             res["mma_floor_ms_at_max_clock"] = round(floor, 4)
+            res["floor_fraction"] = round(floor / res["estep_ms"], 3)
+            res["valid"] = hgmma[lib] is not None and hgmma[lib] == full
             print(json.dumps(res), flush=True)
 
 
