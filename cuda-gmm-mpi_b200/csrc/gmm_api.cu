@@ -604,6 +604,9 @@ static int check_path(const gmm_ctx* c, int K) {
 }
 
 static int ensure_moments(gmm_ctx* c);
+// Doubles of d_stats / h_stats: the packed statistics and the log-likelihood slot, and at least the 4 D column moments
+// that ensure_moments stages there (more than K F + 1 at Kmax = 1 and D = 2 or 3)
+static size_t stats_capacity(const gmm_ctx* c) { return std::max((size_t)c->Kmax * c->F + 1, 4 * (size_t)c->D); }
 
 // The worker team of the host finalisation, created on first use and resized to the context's host_threads.
 static HostPool* host_pool(gmm_ctx* c) {
@@ -875,7 +878,7 @@ static int ensure_moments(gmm_ctx* c) {
     // d_stats[0..D) sum x, [D..2D) sum x^2, [2D..3D) max x, [3D..4D) max (-x)
     std::vector<double> init(4 * (size_t)D, 0.0);
     for (int d = 0; d < 2 * D; d++) init[2 * D + d] = -std::numeric_limits<double>::max();
-    if (4 * (size_t)D > (size_t)c->Kmax * c->F + 1) return fail(GMM_ERR_STATE, "stats buffer too small for the column moments");
+    if (4 * (size_t)D > stats_capacity(c)) return fail(GMM_ERR_STATE, "stats buffer too small for the column moments");
     CUDA_TRY(cudaMemcpyAsync(c->d_stats, init.data(), sizeof(double) * 4 * D, cudaMemcpyHostToDevice, c->stream));
     if (c->n > 0) {
         dim3 grid(std::min(4 * c->num_sms, (c->n + 255) / 256), D);
@@ -1014,9 +1017,9 @@ int gmm_create(gmm_ctx** out, int device, int n_local, int D, int Kmax, const fl
     CREATE_TRY(cudaMalloc(&c->d_memb, sizeof(float) * c->memb_pitch * (size_t)((Kmax + 7) / 8 * 8)));
     CREATE_TRY(cudaMalloc(&c->d_epack, sizeof(float) * (size_t)Kmax * epack_stride(D)));
     CREATE_TRY(cudaMallocHost(&c->h_epack, sizeof(float) * (size_t)Kmax * epack_stride(D)));
-    CREATE_TRY(cudaMalloc(&c->d_stats, sizeof(double) * ((size_t)Kmax * c->F + 1)));
+    CREATE_TRY(cudaMalloc(&c->d_stats, sizeof(double) * stats_capacity(c)));
     CREATE_TRY(cudaMemsetAsync(c->d_stats, 0, sizeof(double) * ((size_t)Kmax * c->F + 1), c->stream));
-    CREATE_TRY(cudaMallocHost(&c->h_stats, sizeof(double) * ((size_t)Kmax * c->F + 1)));
+    CREATE_TRY(cudaMallocHost(&c->h_stats, sizeof(double) * stats_capacity(c)));
     CREATE_TRY(cudaMalloc(&c->d_shift, sizeof(double) * GMM_MAX_DIMENSIONS));
     CREATE_TRY(cudaMemsetAsync(c->d_shift, 0, sizeof(double) * GMM_MAX_DIMENSIONS, c->stream));
     if (n_local > 0 && events_aos) {

@@ -192,9 +192,12 @@ score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __
 // reference (gaussian_kernel.cu:522-677) as ONE pass over the events and the
 // responsibilities:  stats[k][f] += sum_n g[k][n] * phi_f(x_n - shift), with
 // phi = [1, x, x_i x_j (i>=j)].  This is a (K x n) . (n x F) product; here it
-// runs on the FP64 CUDA cores (products of two floats are exact in double, so
-// the statistics are exact up to the final double rounding) — it is the
-// accuracy anchor for the wgmma path, not the fast path.
+// runs on the FP64 CUDA cores — it is the accuracy anchor for the wgmma path,
+// not the fast path.  Where the shift is a float (the wgmma M-step's D) x - s
+// and the product of two such differences are exact in double; at the other D
+// the shift is the double mean, so x - s and its products round, and the
+// statistics carry the rounding of the per-block fma chains and the atomics
+// (tests/test_gpu_simt.py holds them to that bound).
 // Thread layout: 256 threads = 16 (cluster groups of CPT) x 16 (feature lanes,
 // JMAX features each); TE events per shared-memory tile.  WT (gmm_set_weights): the responsibility operand is
 // g * w[e], formed in double (exact: a product of two floats).
