@@ -10,6 +10,7 @@ it as ``cuda_gmm_mpi_b200``.
 from .clusters import Clusters, clusters_t          # noqa: F401
 from .engine import (Engine, GmmError, build_library, load_library, library_path,   # noqa: F401
                      host_invert, host_finalize, host_vb_finalize, host_digamma, host_rissanen, host_epsilon,
+                     host_combine_groups, host_combine_elbow,
                      host_reduce_order, shard_range, stats_len, read_data,
                      write_summary, write_results, nccl_unique_id,
                      PATH_AUTO, PATH_SIMT, PATH_TENSOR, VB_DIRICHLET_PROCESS, VB_DIRICHLET_DISTRIBUTION)

@@ -36,6 +36,7 @@
 #include "kernels_seed.cuh"
 #include "kernels_tc.cuh"
 #include "kernels_vb.cuh"
+#include "kernels_combine.cuh"
 
 namespace gmm {
 
@@ -429,6 +430,32 @@ struct ConditionBuffers {
     }
 };
 
+// gmm_combine / gmm_combine_labels: per-(range, value) partials of the passes, their reduced sums and pinned mirror (sized
+// for the largest pass seen), the live groups' member lists, and the labels' device outputs; allocated on first use, freed
+// by gmm_destroy.
+struct CombineBuffers {
+    double* d_part = nullptr;
+    size_t part_doubles = 0;
+    double* d_sum = nullptr;
+    double* h_sum = nullptr;
+    size_t sum_doubles = 0;
+    int* d_groups = nullptr;                    // [2 kCombMaxK + 1]: members, then offsets
+    int* h_groups = nullptr;                    // pinned
+    int* d_lab = nullptr;                       // [memb_pitch]
+    float* d_max = nullptr;                     // [memb_pitch]
+    cudaEvent_t t0 = nullptr, t1 = nullptr;
+    double kernel_ms = 0, wall_ms = 0, labels_wall_ms = 0;   // gmm_get_combine_profile
+    void destroy() {
+        cudaFree(d_part); cudaFree(d_sum); cudaFree(d_groups); cudaFree(d_lab); cudaFree(d_max);
+        if (h_sum) cudaFreeHost(h_sum);
+        if (h_groups) cudaFreeHost(h_groups);
+        if (t0) cudaEventDestroy(t0);
+        if (t1) cudaEventDestroy(t1);
+        d_part = d_sum = h_sum = nullptr; d_groups = h_groups = d_lab = nullptr; d_max = nullptr; t0 = t1 = nullptr;
+        part_doubles = sum_doubles = 0;
+    }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -519,6 +546,7 @@ struct gmm_ctx {
     int ent_blocks = 0;
     PhaseTimer t_entropy;
     double vb_final_ms = 0, vb_wall_ms = 0;   // gmm_get_vb_profile
+    CombineBuffers comb;         // gmm_combine / gmm_combine_labels: allocated on first use
 };
 
 namespace gmm {
@@ -1141,6 +1169,7 @@ void gmm_destroy(gmm_ctx* c) {
     c->kmeans.destroy();
     c->sample.destroy();
     c->cond.destroy();
+    c->comb.destroy();
     delete c->pool;
     cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
     cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
@@ -2343,8 +2372,8 @@ static int vb_default_moments(gmm_ctx* c, double* mean, double* cov) {
 }
 
 // resp_entropy_kernel over the current memberships, its partials queued to the pinned mirror (read after the next stream
-// synchronisation by vb_entropy_sum).
-static int vb_entropy_launch(gmm_ctx* c, int K, int* grid_out) {
+// synchronisation by vb_entropy_sum).  timer: the profile the kernel counts in (NULL: none).
+static int vb_entropy_launch(gmm_ctx* c, int K, int* grid_out, PhaseTimer* timer) {
     if (!c->d_ent) {
         c->ent_blocks = kEntropyBlocksPerSm * c->num_sms;
         CUDA_TRY(cudaMalloc(&c->d_ent, sizeof(double) * (size_t)(c->ent_blocks + 1)));
@@ -2355,10 +2384,10 @@ static int vb_entropy_launch(gmm_ctx* c, int K, int* grid_out) {
     *grid_out = c->n > 0 ? grid : 0;
     if (c->n == 0) return GMM_OK;
     const float* w = step_weights(c);
-    timer_begin(c, c->t_entropy);
+    if (timer) timer_begin(c, *timer);
     if (w) resp_entropy_kernel<true><<<grid, kEntropyThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, c->n, K, w, c->d_ent);
     else resp_entropy_kernel<false><<<grid, kEntropyThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, c->n, K, nullptr, c->d_ent);
-    timer_end(c, c->t_entropy);
+    if (timer) timer_end(c, *timer);
     CUDA_TRY(cudaGetLastError());
     CUDA_TRY(cudaMemcpyAsync(c->h_ent, c->d_ent, sizeof(double) * grid, cudaMemcpyDeviceToHost, c->stream));
     return GMM_OK;
@@ -2439,7 +2468,7 @@ int gmm_vb_em(gmm_ctx* c, int K, const gmm_vb_prior* prior, int min_iters, int m
         const bool need_bound = lower_bounds_out != nullptr || i >= min_iters - 1;
         int grid = 0;
         if (need_bound)
-            if (int rc = vb_entropy_launch(c, K, &grid)) return rc;
+            if (int rc = vb_entropy_launch(c, K, &grid, &c->t_entropy)) return rc;
         if (int rc = reduce_stats_to_host(c, K)) return rc;
         if (int rc = vb_finalize_upload(c, K, p, cl, post_out, &bound_par)) return rc;
         iters = i;
@@ -2472,6 +2501,230 @@ int gmm_get_vb_profile(gmm_ctx* c, double out[3], int reset) {
     collect_all(c);
     out[0] = c->t_entropy.total_ms; out[1] = c->vb_final_ms; out[2] = c->vb_wall_ms;
     if (reset) { c->t_entropy.total_ms = 0; c->vb_final_ms = c->vb_wall_ms = 0; }
+    return GMM_OK;
+}
+
+// ---- combining mixture components (gmm_combine) ----------------------------------------------------------------------
+// The memberships of the last E-step for K, complete and current.
+static int check_memberships(const gmm_ctx* c, int K, const char* who) {
+    if (int rc = check_fitted(c, K, who)) return rc;
+    if (!c->memb_valid) return fail(GMM_ERR_STATE, std::string(who) + ": no E-step has run for the current parameters and weights");
+    return GMM_OK;
+}
+
+static int combine_buffers(gmm_ctx* c, size_t part, size_t sum) {
+    CombineBuffers& b = c->comb;
+    if (!b.d_groups) {
+        CUDA_TRY(cudaMalloc(&b.d_groups, sizeof(int) * (2 * kCombMaxK + 1)));
+        CUDA_TRY(cudaMallocHost(&b.h_groups, sizeof(int) * (2 * kCombMaxK + 1)));
+        CUDA_TRY(cudaEventCreate(&b.t0));
+        CUDA_TRY(cudaEventCreate(&b.t1));
+    }
+    if (part > b.part_doubles) {
+        cudaFree(b.d_part);
+        b.d_part = nullptr;
+        b.part_doubles = 0;
+        CUDA_TRY(cudaMalloc(&b.d_part, sizeof(double) * part));
+        b.part_doubles = part;
+    }
+    if (sum > b.sum_doubles) {
+        cudaFree(b.d_sum);
+        if (b.h_sum) cudaFreeHost(b.h_sum);
+        b.d_sum = b.h_sum = nullptr;
+        b.sum_doubles = 0;
+        CUDA_TRY(cudaMalloc(&b.d_sum, sizeof(double) * sum));
+        CUDA_TRY(cudaMallocHost(&b.h_sum, sizeof(double) * sum));
+        b.sum_doubles = sum;
+    }
+    return GMM_OK;
+}
+
+// Groups as member lists for the step and label kernels: members of group i at [off[i], off[i + 1]) of the pinned staging,
+// offsets after the kCombMaxK member slots; queued to the device.
+static int combine_upload_groups(gmm_ctx* c, const std::vector<std::vector<int>>& groups) {
+    int* h = c->comb.h_groups;
+    int* off = h + kCombMaxK;
+    int pos = 0;
+    for (size_t i = 0; i < groups.size(); i++) {
+        off[i] = pos;
+        for (int k : groups[i]) h[pos++] = k;
+    }
+    off[groups.size()] = pos;
+    CUDA_TRY(cudaMemcpyAsync(c->comb.d_groups, h, sizeof(int) * (2 * kCombMaxK + 1), cudaMemcpyHostToDevice, c->stream));
+    return GMM_OK;
+}
+
+// partial [ranges][P] -> d_sum [P] summed in range order, all-reduced over the ranks, -> h_sum; the kernels since t0 are
+// timed to t1 and the host waits.
+static int combine_finish(gmm_ctx* c, int ranges, int P) {
+    CombineBuffers& b = c->comb;
+    if (ranges > 0) {
+        const int grid = std::max(1, std::min(c->num_sms, (P + kCombSumThreads - 1) / kCombSumThreads));
+        combine_sum_ranges_kernel<<<grid, kCombSumThreads, 0, c->stream>>>(b.d_part, ranges, P, b.d_sum);
+        CUDA_TRY(cudaGetLastError());
+    } else {
+        CUDA_TRY(cudaMemsetAsync(b.d_sum, 0, sizeof(double) * P, c->stream));
+    }
+    if (c->nranks > 1) {
+        ncclResult_t r = nccl().AllReduce(b.d_sum, b.d_sum, (size_t)P, ncclDouble, ncclSum, c->comm, c->stream);
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+    }
+    CUDA_TRY(cudaEventRecord(b.t1, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(b.h_sum, b.d_sum, sizeof(double) * P, cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, b.t0, b.t1) == cudaSuccess) b.kernel_ms += ms;
+    return GMM_OK;
+}
+
+static int combine_run(gmm_ctx* c, int K, int* merges_out, double* gain_out, double* entropy_out, double* mass_out) {
+    CombineBuffers& b = c->comb;
+    const int n = c->n, npairs = K * (K - 1) / 2, P = npairs + K;
+    const float* w = step_weights(c);
+    // all-pairs pass: ranges of 64-event multiples, about 4 CTAs per SM in all
+    const int T = (K + kCombTile - 1) / kCombTile, tiles = T * (T + 1) / 2;
+    const int max_ranges = std::max(1, (4 * c->num_sms + tiles - 1) / tiles);
+    const long long n_units = ((long long)n + kCombPairEvents - 1) / kCombPairEvents;
+    const int range_events = (int)std::max<long long>(1, (n_units + max_ranges - 1) / max_ranges) * kCombPairEvents;
+    const int ranges1 = n > 0 ? (n + range_events - 1) / range_events : 0;
+    // step pass: blocks of kCombStepEvents grid-strided over the CTAs one wave holds
+    int per_sm = 0;
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, w ? combine_step_kernel<true> : combine_step_kernel<false>,
+                                                           kCombStepThreads, 0));
+    const int nblocks = (n + kCombStepEvents - 1) / kCombStepEvents;
+    const int ranges2 = std::min(nblocks, std::max(per_sm, 1) * c->num_sms);
+    if (int rc = combine_buffers(c, std::max({(size_t)ranges1 * P, (size_t)ranges2 * K, (size_t)1}), (size_t)P)) return rc;
+
+    CUDA_TRY(cudaEventRecord(b.t0, c->stream));
+    int egrid = 0;
+    if (int rc = vb_entropy_launch(c, K, &egrid, nullptr)) return rc;
+    if (ranges1 > 0) {
+        const dim3 grid(tiles, ranges1);
+        if (w) combine_pairs_kernel<true><<<grid, kCombPairThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, n, K, w, range_events, b.d_part, P);
+        else combine_pairs_kernel<false><<<grid, kCombPairThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, n, K, nullptr, range_events, b.d_part, P);
+        CUDA_TRY(cudaGetLastError());
+    }
+    if (int rc = combine_finish(c, ranges1, P)) return rc;
+    double ent = 0.0;
+    if (int rc = vb_entropy_sum(c, egrid, &ent)) return rc;
+    std::vector<double> mk(b.h_sum + npairs, b.h_sum + P);
+    for (int k = 0; k < K; k++)
+        if (!std::isfinite(mk[(size_t)k]))
+            return fail(GMM_ERR_STATE, "gmm_combine: the memberships of component " + std::to_string(k) + " are not finite");
+    std::vector<double> gain((size_t)K * K, 0.0);           // gain[a K + b], a < b the groups' smallest components
+    for (int a = 0; a < K; a++)
+        for (int bb = a + 1; bb < K; bb++) gain[(size_t)a * K + bb] = b.h_sum[combine_pair_index(a, bb, K)];
+    std::vector<std::vector<int>> members((size_t)K);
+    for (int k = 0; k < K; k++) members[(size_t)k] = {k};
+    std::vector<int> live((size_t)K);
+    for (int k = 0; k < K; k++) live[(size_t)k] = k;
+    std::vector<double> gains((size_t)std::max(K - 1, 0));
+    auto group_mass = [&](int r) {
+        double m = 0.0;
+        for (int k : members[(size_t)r]) m += mk[(size_t)k];
+        return m;
+    };
+    for (int s = 0; s < K - 1; s++) {
+        // the live pair of largest gain; strict > over the pairs in lexicographic order keeps the smallest (a, b) of a tie
+        int ba = -1, bb = -1;
+        double bg = 0.0;
+        for (size_t i = 0; i < live.size(); i++)
+            for (size_t j = i + 1; j < live.size(); j++) {
+                const double g = gain[(size_t)live[i] * K + live[j]];
+                if (ba < 0 || g > bg) { ba = live[i]; bb = live[j]; bg = g; }
+            }
+        merges_out[2 * s] = ba;
+        merges_out[2 * s + 1] = bb;
+        gains[(size_t)s] = bg;
+        if (mass_out) mass_out[s] = group_mass(ba) + group_mass(bb);
+        std::vector<int>& ma = members[(size_t)ba];
+        ma.insert(ma.end(), members[(size_t)bb].begin(), members[(size_t)bb].end());
+        std::sort(ma.begin(), ma.end());
+        members[(size_t)bb].clear();
+        live.erase(std::find(live.begin(), live.end(), bb));
+        if (s == K - 2) break;
+        // step pass: the merged group against every other live group
+        const int L = (int)live.size();
+        const int gi = (int)(std::find(live.begin(), live.end(), ba) - live.begin());
+        std::vector<std::vector<int>> groups((size_t)L);
+        for (int i = 0; i < L; i++) groups[(size_t)i] = members[(size_t)live[(size_t)i]];
+        if (int rc = combine_upload_groups(c, groups)) return rc;
+        CUDA_TRY(cudaEventRecord(b.t0, c->stream));
+        if (ranges2 > 0) {
+            const int* mem = b.d_groups;
+            const int* off = b.d_groups + kCombMaxK;
+            if (w) combine_step_kernel<true><<<ranges2, kCombStepThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, n, w, mem, off, L, gi, b.d_part);
+            else combine_step_kernel<false><<<ranges2, kCombStepThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, n, nullptr, mem, off, L, gi, b.d_part);
+            CUDA_TRY(cudaGetLastError());
+        }
+        if (int rc = combine_finish(c, ranges2, L)) return rc;
+        for (int i = 0; i < L; i++) {
+            if (i == gi) continue;
+            const int h = live[(size_t)i];
+            gain[(size_t)std::min(ba, h) * K + std::max(ba, h)] = b.h_sum[i];
+        }
+    }
+    if (gain_out) std::copy(gains.begin(), gains.end(), gain_out);
+    if (entropy_out) {
+        entropy_out[K - 1] = -ent;
+        for (int L = K; L >= 2; L--) entropy_out[L - 2] = entropy_out[L - 1] - gains[(size_t)(K - L)];
+    }
+    return GMM_OK;
+}
+
+int gmm_combine(gmm_ctx* c, int K, int* merges_out, double* gain_out, double* entropy_out, double* mass_out) {
+    if (int rc = check_K(c, K, "gmm_combine")) return rc;
+    if (K >= 2 && !merges_out) return fail(GMM_ERR_ARG, "gmm_combine: NULL merges_out with K >= 2");
+    if (int rc = check_memberships(c, K, "gmm_combine")) return rc;
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc = combine_run(c, K, merges_out, gain_out, entropy_out, mass_out);
+    c->comb.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_combine_labels(gmm_ctx* c, int K, const int* group, int G, int* labels_out, float* max_out) {
+    if (int rc = check_K(c, K, "gmm_combine_labels")) return rc;
+    if (!group || G < 1 || G > K || (c->n > 0 && !labels_out))
+        return fail(GMM_ERR_ARG, "gmm_combine_labels: bad argument (need group, 1 <= G <= K and labels_out)");
+    std::vector<std::vector<int>> groups((size_t)G);
+    for (int k = 0; k < K; k++) {
+        if (group[k] < 0 || group[k] >= G)
+            return fail(GMM_ERR_ARG, "gmm_combine_labels: group[" + std::to_string(k) + "] is outside [0, G)");
+        groups[(size_t)group[k]].push_back(k);
+    }
+    if (int rc = check_memberships(c, K, "gmm_combine_labels")) return rc;
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    CombineBuffers& b = c->comb;
+    if (int rc = combine_buffers(c, 1, 1)) return rc;
+    if (!b.d_lab) {
+        CUDA_TRY(cudaMalloc(&b.d_lab, sizeof(int) * c->memb_pitch));
+        CUDA_TRY(cudaMalloc(&b.d_max, sizeof(float) * c->memb_pitch));
+    }
+    if (c->n > 0) {
+        if (int rc = combine_upload_groups(c, groups)) return rc;
+        const int nq = (c->n + 3) / 4;
+        const int grid = std::max(1, std::min(8 * c->num_sms, (nq + kCombLabelThreads - 1) / kCombLabelThreads));
+        CUDA_TRY(cudaEventRecord(b.t0, c->stream));
+        combine_labels_kernel<<<grid, kCombLabelThreads, 0, c->stream>>>(c->d_memb, c->memb_pitch, c->n, b.d_groups, b.d_groups + kCombMaxK,
+                                                                         G, b.d_lab, b.d_max);
+        CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaEventRecord(b.t1, c->stream));
+        CUDA_TRY(cudaMemcpyAsync(labels_out, b.d_lab, sizeof(int) * c->n, cudaMemcpyDeviceToHost, c->stream));
+        if (max_out) CUDA_TRY(cudaMemcpyAsync(max_out, b.d_max, sizeof(float) * c->n, cudaMemcpyDeviceToHost, c->stream));
+        CUDA_TRY(cudaStreamSynchronize(c->stream));
+        float ms = 0;
+        if (cudaEventElapsedTime(&ms, b.t0, b.t1) == cudaSuccess) b.kernel_ms += ms;
+    }
+    b.labels_wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return GMM_OK;
+}
+
+int gmm_get_combine_profile(gmm_ctx* c, double out[3], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_combine_profile: bad argument");
+    out[0] = c->comb.kernel_ms; out[1] = c->comb.wall_ms; out[2] = c->comb.labels_wall_ms;
+    if (reset) c->comb.kernel_ms = c->comb.wall_ms = c->comb.labels_wall_ms = 0;
     return GMM_OK;
 }
 

@@ -681,6 +681,67 @@ int gmm_host_digamma(const double* x, double* out, long long n) {
     return GMM_OK;
 }
 
+int gmm_host_combine_groups(const int* merges, int K, int L, int* group_out) {
+    if (K < 1 || K > GMM_MAX_CLUSTERS || L < 1 || L > K || !group_out || (K >= 2 && !merges))
+        return gmm::fail(GMM_ERR_ARG, "gmm_host_combine_groups: bad argument (need 1 <= L <= K <= 512, merges and group_out)");
+    // rep[k] = the component k was merged into (itself while its group is live); a merge joins two live groups a < b
+    std::vector<int> rep((size_t)K);
+    for (int k = 0; k < K; k++) rep[(size_t)k] = k;
+    for (int s = 0; s < K - 1; s++) {
+        const int a = merges[2 * s], b = merges[2 * s + 1];
+        if (a < 0 || b >= K || a >= b || rep[(size_t)a] != a || rep[(size_t)b] != b)
+            return gmm::fail(GMM_ERR_ARG, "gmm_host_combine_groups: merge " + std::to_string(s) + " is not a pair a < b of live groups");
+        if (s < K - L) rep[(size_t)b] = a;
+    }
+    // a group's smallest component is its root, met first in increasing k: clusters numbered in that order
+    std::vector<int> label((size_t)K, -1);
+    int next = 0;
+    for (int k = 0; k < K; k++) {
+        int r = k;
+        while (rep[(size_t)r] != r) r = rep[(size_t)r];
+        if (label[(size_t)r] < 0) label[(size_t)r] = next++;
+        group_out[k] = label[(size_t)r];
+    }
+    return GMM_OK;
+}
+
+// Residual sum of squares of the least-squares line through points [b, e) (the mean when their x are all equal):
+// centred sums, in index order.
+static double elbow_sse(const double* x, const double* y, int b, int e) {
+    const int m = e - b;
+    double sx = 0.0, sy = 0.0;
+    for (int i = b; i < e; i++) { sx += x[i]; sy += y[i]; }
+    const double mx = sx / m, my = sy / m;
+    double sxx = 0.0, sxy = 0.0;
+    for (int i = b; i < e; i++) { sxx += (x[i] - mx) * (x[i] - mx); sxy += (x[i] - mx) * (y[i] - my); }
+    const double beta = sxx > 0.0 ? sxy / sxx : 0.0;
+    double sse = 0.0;
+    for (int i = b; i < e; i++) {
+        const double r = (y[i] - my) - beta * (x[i] - mx);
+        sse += r * r;
+    }
+    return sse;
+}
+
+int gmm_host_combine_elbow(const double* entropy, const double* x, int K, int* L_out) {
+    if (!entropy || !L_out || K < 3) return gmm::fail(GMM_ERR_ARG, "gmm_host_combine_elbow: bad argument (need entropy, L_out and K >= 3)");
+    std::vector<double> xs((size_t)K);
+    for (int i = 0; i < K; i++) {
+        xs[(size_t)i] = x ? x[i] : (double)(i + 1);
+        if (!std::isfinite(xs[(size_t)i]) || !std::isfinite(entropy[i]))
+            return gmm::fail(GMM_ERR_ARG, "gmm_host_combine_elbow: a value that is not finite");
+    }
+    // point L = i + 1 is index i; change point c joins the segments [0, c) and [c - 1, K)
+    int best = 2;
+    double best_sse = 0.0;
+    for (int c = 2; c <= K - 1; c++) {
+        const double sse = elbow_sse(xs.data(), entropy, 0, c) + elbow_sse(xs.data(), entropy, c - 1, K);
+        if (c == 2 || sse < best_sse) { best = c; best_sse = sse; }
+    }
+    *L_out = best;
+    return GMM_OK;
+}
+
 float gmm_host_rissanen(float loglik, int K, int D, long long N) { return gmm::rissanen(loglik, K, D, (double)N); }
 float gmm_host_epsilon(int D, long long N) { return gmm::em_epsilon(D, (double)N); }
 

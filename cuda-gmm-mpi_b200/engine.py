@@ -134,6 +134,11 @@ def load_library():
     L.gmm_host_vb_finalize.argtypes = [_DP, _DP, C.c_int, C.c_int, C.POINTER(gmm_vb_prior), _CP, C.POINTER(gmm_vb_posterior), _DP]
     L.gmm_host_digamma.argtypes = [_DP, _DP, C.c_longlong]
     L.gmm_get_vb_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_combine.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.gmm_combine_labels.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
+    L.gmm_host_combine_groups.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
+    L.gmm_host_combine_elbow.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _IP]
+    L.gmm_get_combine_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
     L.gmm_stats_len.argtypes = [C.c_int, C.c_int]
@@ -205,6 +210,27 @@ def host_digamma(x):
     out = np.empty_like(x)
     _check(load_library().gmm_host_digamma(x.ctypes.data_as(_DP), out.ctypes.data_as(_DP), x.size))
     return out
+
+
+def host_combine_groups(merges, K, L):
+    """The cluster of each of K components at level L of a gmm_combine hierarchy (gmm_host_combine_groups): int32 [K],
+    clusters numbered 0 .. L-1 in increasing order of their smallest component."""
+    m = np.ascontiguousarray(merges, np.int32).reshape(-1)
+    out = np.empty(max(int(K), 1), np.int32)
+    _check(load_library().gmm_host_combine_groups(m.ctypes.data if m.size else None, int(K), int(L), out.ctypes.data))
+    return out[:K]
+
+
+def host_combine_elbow(entropy, x=None):
+    """The level L of the change point of entropy [K] against x [K] (default 1 .. K) (gmm_host_combine_elbow)."""
+    e = np.ascontiguousarray(entropy, np.float64).reshape(-1)
+    xa = None if x is None else np.ascontiguousarray(x, np.float64).reshape(-1)
+    if xa is not None and xa.size != e.size:
+        raise ValueError(f"x must have {e.size} values, got {xa.size}")
+    L = C.c_int()
+    _check(load_library().gmm_host_combine_elbow(e.ctypes.data if e.size else None, xa.ctypes.data if xa is not None else None,
+                                                 int(e.size), C.byref(L)))
+    return L.value
 
 
 def host_rissanen(ll, K, D, N):
@@ -517,6 +543,34 @@ class Engine:
         out = (C.c_double * 3)()
         _check(self.lib.gmm_get_vb_profile(self.h, out, int(reset)))
         return dict(entropy_ms=out[0], finalize_ms=out[1], wall_ms=out[2])
+
+    def combine(self, K):
+        """Entropy-criterion hierarchy of the K components over the memberships of the last E-step (gmm_combine).
+        Returns dict(merges int32 [K-1][2], gain [K-1], entropy [K] (entropy[L-1] at L clusters), mass [K-1])."""
+        merges = np.zeros((max(K - 1, 1), 2), np.int32)
+        gain, mass = np.zeros(max(K - 1, 1)), np.zeros(max(K - 1, 1))
+        ent = np.zeros(K)
+        _check(self.lib.gmm_combine(self.h, K, merges.ctypes.data, gain.ctypes.data, ent.ctypes.data, mass.ctypes.data))
+        return dict(merges=merges[:K - 1], gain=gain[:K - 1], entropy=ent, mass=mass[:K - 1])
+
+    def combine_labels(self, K, group, G=None, max_sum=True):
+        """Labels of this shard's events under a grouping of the K components (gmm_combine_labels): group int [K] with
+        values in [0, G), G = max + 1 by default.  Returns (labels int32 [n], the group sum of the label float32 [n] or
+        None)."""
+        g = np.ascontiguousarray(group, np.int32).reshape(-1)
+        if g.size != K:
+            raise ValueError(f"group must have {K} values, got {g.size}")
+        if G is None:
+            G = int(g.max()) + 1 if g.size else 0
+        lab = np.empty(max(self.n, 1), np.int32)
+        mx = np.empty(max(self.n, 1), np.float32) if max_sum else None
+        _check(self.lib.gmm_combine_labels(self.h, K, g.ctypes.data, G, lab.ctypes.data, mx.ctypes.data if mx is not None else None))
+        return lab[:self.n], (mx[:self.n] if mx is not None else None)
+
+    def combine_profile(self, reset=False):
+        out = (C.c_double * 3)()
+        _check(self.lib.gmm_get_combine_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], wall_ms=out[1], labels_wall_ms=out[2])
 
     def comm_rank(self):
         r, n = C.c_int(), C.c_int()

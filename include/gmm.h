@@ -509,6 +509,76 @@ int  gmm_host_digamma(const double* x, double* out, long long n);
 /* Since the last reset: out[0] entropy-kernel ms, out[1] host VB finalisation ms, out[2] wall ms inside gmm_vb_em.    */
 int  gmm_get_vb_profile(gmm_ctx*, double out[3], int reset);
 
+/* ---- combining mixture components into clusters (Baudry, Raftery, Celeux, Lo and Gottardo, JCGS 19 (2010); mclust's
+ * clustCombi, flowMerge) ----------------------------------------------------------------------------------------------
+ * A population that is skewed, curved or heavy-tailed is fitted by several Gaussian components.  These calls keep the
+ * K-component density and merge components into clusters hierarchically, each merge chosen by the largest drop in
+ * classification entropy; a cluster is a union of components, so the density never changes (unlike the order reduction
+ * of gmm_fit, which re-fits one Gaussian per merged pair).  Workflow: a fit (gmm_em, gmm_fit, gmm_vb_em), gmm_estep,
+ * gmm_combine, a level L (gmm_host_combine_elbow or the caller's choice), gmm_host_combine_groups, gmm_combine_labels.
+ * After gmm_fit the current memberships are those of the last order it ran, not of ideal_K: to combine the best model,
+ * call gmm_set_clusters(ideal_K, saved) and gmm_estep first.
+ * Notation (restated in float64 / float32 numpy by tests/_combine_ref.py):
+ *   - tau_k(n) is the stored float membership of event n in component k; w_n the weight of gmm_set_weights (1 without).
+ *   - group sum: tau_A(n) of a group A is the float sum of its members' rows, added left to right in increasing component
+ *     index (no FMA, no reassociation); a singleton is the stored value.
+ *   - pair gain: dEnt(A, B) = sum_n w_n phi(tau_A(n), tau_B(n)), phi(a, b) = (a+b) ln(a+b) - a ln a - b ln b, computed in
+ *     float as M h(m / M) with M = max(a, b), m = min(a, b), h(r) = (1 + r) log1pf(r) - r logf(r), and phi = 0 when
+ *     m = 0; both terms of h are >= 0 on (0, 1], so nothing cancels.  Events are summed in double.
+ *   - hierarchy: step s = 0 .. K-2 merges the live pair (A, B) of largest all-reduced gain, ties between equal doubles to
+ *     the lexicographically smallest (a, b).  A group is named by its smallest component: a < b, and the merged group
+ *     keeps a.  The choice is made from the reduced gains, identically on every rank.
+ * Kernels (csrc/kernels_combine.cuh, sm_90a): one all-pairs pass over the singletons (32 x 32 component tiles times event
+ * ranges, the rows staged in shared memory), then after each merge one pass of the merged group against every live group,
+ * each group sum formed on the fly from the original rows (one read of all K rows per step).  The memberships are never
+ * copied or rewritten.  No atomics: repeated calls give the same bits.
+ * Device memory: per-(range, value) partials of at most about 4 MB (K = 512), the reduced values with a pinned mirror
+ * (K(K-1)/2 + K doubles), the group lists (2 x 512 + 1 ints, pinned mirror), allocated on the first call and grown with
+ * K; gmm_combine_labels adds an int and a float per event (the pitched row length).  gmm_destroy frees them.          */
+
+/* The entropy-criterion hierarchy over the memberships of the last E-step for K.  Collective over the ranks of a
+ * communicator, like gmm_em (same K on every rank).
+ *   merges_out  [K-1][2]: step s merged groups {a, b}, a < b
+ *   gain_out    [K-1]:    that pair's gain dEnt
+ *   entropy_out [K]:      entropy_out[L-1] = the classification entropy at L clusters; entropy_out[K-1] =
+ *                         -sum_n w_n sum_k tau ln tau (0 ln 0 = 0) from resp_entropy_kernel, as gmm_vb_em sums it;
+ *                         entropy_out[L-2] = entropy_out[L-1] - gain_out[K-L] in double
+ *   mass_out    [K-1]:    m_A + m_B, where m_k = sum_n w_n tau_k(n) in double and a group's mass is the sum of its
+ *                         members' masses in member order (Baudry's abscissa: entropy against cumulative merged mass)
+ * Every output except merges_out may be NULL; K = 1 writes only entropy_out[0] (and merges_out may be NULL).
+ * Nothing of the state changes: not the memberships, not the parameters, not gmm_get_profile nor any other profile.
+ * Errors: K outside [1, Kmax] or a NULL merges_out with K >= 2 -> GMM_ERR_ARG; K != the K of the current parameters,
+ * memberships that are not valid (before any E-step, or after gmm_set_clusters or gmm_set_weights), a call between
+ * gmm_mstep and gmm_constants, or a membership that is not finite (the first component concerned is named) ->
+ * GMM_ERR_STATE; a failed collective -> GMM_ERR_NCCL.                                                                */
+int  gmm_combine(gmm_ctx*, int K, int* merges_out, double* gain_out, double* entropy_out, double* mass_out);
+
+/* Labels of THIS shard's events under a grouping of the K components into G clusters (group[k] in [0, G), e.g. from
+ * gmm_host_combine_groups): label = argmax over g of the group sum of {k : group[k] = g} (a cluster without members sums
+ * to 0), the lowest g on ties, -1 when every sum is NaN; max_out = that sum (NaN for -1).  One read of the K rows.  No
+ * collective; nothing of the state changes.  labels_out [n_local] (may be NULL only when n_local = 0), max_out [n_local]
+ * or NULL.
+ * Errors: K outside [1, Kmax], a NULL group, G outside [1, K], a group index outside [0, G) or a NULL labels_out ->
+ * GMM_ERR_ARG; the state errors of gmm_combine -> GMM_ERR_STATE.                                                     */
+int  gmm_combine_labels(gmm_ctx*, int K, const int* group, int G, int* labels_out, float* max_out);
+
+/* Host-only, no GPU needed.  The cluster of each component at level L (1 <= L <= K) of a hierarchy: the first K-L
+ * merges of merges [K-1][2] applied; clusters numbered 0 .. L-1 in increasing order of their smallest component.
+ * Errors: K outside [1, 512], L outside [1, K], a NULL group_out, a NULL merges with K >= 2, or a merge list that is
+ * not a valid hierarchy (every step a pair a < b of groups still live, named by their smallest components) -> GMM_ERR_ARG. */
+int  gmm_host_combine_groups(const int* merges, int K, int L, int* group_out);
+
+/* Host-only.  The change point flowMerge and Baudry use to pick the level: points P_L = (x_L, entropy[L-1]) for L = 1 .. K,
+ * x_L = L when x is NULL.  For each c in 2 .. K-1, least-squares lines are fitted to {P_L : L <= c} and to {P_L : L >= c}
+ * (a segment whose x are all equal uses its mean); *L_out = the c of the smallest total residual sum of squares, the
+ * smaller c on ties.  Sums are centred and in index order, in double.
+ * Errors: K < 3, a NULL entropy or L_out, or a value that is not finite -> GMM_ERR_ARG.                              */
+int  gmm_host_combine_elbow(const double* entropy, const double* x /* [K] or NULL */, int K, int* L_out);
+
+/* Since the last reset: out[0] kernel ms (gmm_combine's and gmm_combine_labels' passes), out[1] wall ms inside
+ * gmm_combine, out[2] wall ms inside gmm_combine_labels.                                                             */
+int  gmm_get_combine_profile(gmm_ctx*, double out[3], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
