@@ -42,7 +42,7 @@ condition_simt_kernel(const float* __restrict__ x_obs, int n, int n_obs, int n_m
 #pragma unroll
     for (int d = 0; d < NO; d++) x[d] = (valid && d < n_obs) ? x_obs[(size_t)e * n_obs + d] : 0.0f;
 
-    float run_max = -INFINITY, run_sum = 0.0f, best_l = -INFINITY;
+    float run_max = -FLT_MAX, run_sum = 0.0f, best_l = -INFINITY;        // -FLT_MAX: pi = 0 adds 0 (estep_simt_kernel)
     int best_k = -1;
     float mean[NM], m2[NM];
 #pragma unroll
@@ -66,8 +66,10 @@ condition_simt_kernel(const float* __restrict__ x_obs, int n, int n_obs, int n_m
             // run_sum * rescale + w, which then is no longer contracted to one fma and differs from score_simt_kernel's
             const float w0 = __fmul_rn(sum0, rescale);
             // run_sum is in [1, K] (the maximum's own term is 1): the fast division is safe and its 2 ulp are harmless here;
-            // the IEEE division's slow-path call would make ptxas spill around it (also below)
-            const float f = __fdividef(w, run_sum), g = __fdividef(w0, run_sum);
+            // the IEEE division's slow-path call would make ptxas spill around it (also below).  It is 0 while every logit so
+            // far is -inf (pi = 0): the floor at FLT_MIN then makes f = g = 0 (not 0 / 0) and leaves mean and M2 at 0
+            const float rs = fmaxf(run_sum, FLT_MIN);
+            const float f = __fdividef(w, rs), g = __fdividef(w0, rs);
             const float* mu = p + EP;
             const float* G = mu + NM;
             const float* cv = G + NM * NO;

@@ -11,6 +11,7 @@
 //           [ sum g | sum g (x-s)_d | sum g (x-s)_i (x-s)_j, i>=j ] then 1 LL slot
 #pragma once
 #include <cuda_runtime.h>
+#include <cfloat>
 #include <cstdint>
 
 namespace gmm {
@@ -54,7 +55,10 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
 #pragma unroll
     for (int d = 0; d < D; d++) x[d] = valid ? xs[(size_t)d * xpitch + e] : 0.0f;
 
-    float run_max = -INFINITY, run_sum = 0.0f;
+    // the running maximum starts at -FLT_MAX, not -inf: a cluster with pi = 0 (logit -inf) ahead of every finite logit then
+    // adds expf(-inf) = 0 to run_sum instead of expf(-inf - -inf) = NaN.  Once a logit is finite the maximum is that logit
+    // either way, so the bits do not change
+    float run_max = -FLT_MAX, run_sum = 0.0f;
     for (int k0 = 0; k0 < K; k0 += kEstepClusterChunk) {
         const int kc = min(kEstepClusterChunk, K - k0);
         __syncthreads();
@@ -110,7 +114,8 @@ estep_simt_kernel(const float* __restrict__ xs, size_t xpitch, int n, int K, con
 // One cluster of the scoring loop, shared by score_simt_kernel and condition_simt_kernel (kernels_condition.cuh), on the
 // record p (epack layout) of cluster k: dx = x - mu and the logit l = constant + ln pi - q / 2 with the E-step's
 // operations, the running arg-max (lowest k on ties; NaN logits never win) and the online log-sum-exp.  It declares
-// dx[D] and l in the enclosing scope, where the caller reads them.  A macro rather than a function: expanded in place,
+// dx[D] and l in the enclosing scope, where the caller reads them.  The caller starts run_max at -FLT_MAX, so that a
+// leading cluster with pi = 0 adds expf(-inf) = 0 to run_sum rather than NaN.  A macro rather than a function: expanded in place,
 // score_simt_kernel keeps the statements, and so the machine code, it had when they were written out in it (an inlined
 // function with reference parameters reorders ptxas's output).
 // ---------------------------------------------------------------------------
@@ -153,7 +158,7 @@ score_simt_kernel(const float* __restrict__ x_aos, int n, int K, const float* __
 #pragma unroll
     for (int d = 0; d < D; d++) x[d] = valid ? x_aos[(size_t)e * D + d] : 0.0f;
 
-    float run_max = -INFINITY, run_sum = 0.0f, best_l = -INFINITY;
+    float run_max = -FLT_MAX, run_sum = 0.0f, best_l = -INFINITY;        // -FLT_MAX: pi = 0 adds 0 (estep_simt_kernel)
     int best_k = -1;
     for (int k0 = 0; k0 < K; k0 += kEstepClusterChunk) {
         const int kc = min(kEstepClusterChunk, K - k0);

@@ -210,7 +210,11 @@ int  gmm_get_clusters(gmm_ctx*, int K, clusters_t* host_out, int with_membership
 
 /* estep1 + estep2 + likelihood reduction (gaussian_kernel.cu:383-512,
  * gaussian.cu:713-746).  Writes memberships (device), returns the GLOBAL
- * log-likelihood (summed over ranks).                                       */
+ * log-likelihood (summed over ranks).  A cluster with pi = 0 (logit constant
+ * + ln pi = -inf) gets a membership of exactly 0 and adds nothing to any
+ * event's density, as in estep2, on every path and at every K, also when it
+ * comes first or fills a whole 64-cluster pass.  Every pi = 0 (no finite
+ * logit) is not supported.                                                   */
 int  gmm_estep(gmm_ctx*, int K, float* loglik_out);
 
 /* mstep_N + mstep_means + mstep_covariance1 + the three reductions and host
@@ -251,7 +255,8 @@ int  gmm_em_iterations(gmm_ctx*, int K, int iters, float* loglik_out);
  * beyond 2^14 standard deviations of the training data (or not finite) is
  * re-scored by the SIMT kernel, or fails with GMM_ERR_STATE under
  * GMM_PATH_TENSOR.  On the training shard the outputs equal the E-step's
- * (max_resp bit for bit at K <= 64).  The batch streams through two pinned
+ * (max_resp bit for bit).  A cluster with pi = 0 is never a label and adds
+ * nothing to logp (gmm_estep).  The batch streams through two pinned
  * buffers in chunks of option "score_chunk" events; nothing of the EM state
  * (memberships, statistics, log-likelihood, gmm_get_profile) changes.
  * Errors: K outside [1, Kmax], n < 0 or events_aos == NULL with n > 0 ->

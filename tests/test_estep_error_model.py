@@ -35,7 +35,16 @@ The module asserts, on the parameter sets and (D, K) of tests/test_gpu_estep_tc.
      event's swizzle; this fault passes the per-operator 1e-4 / 1e-6 bar of tests/test_gpu_parity.py), and a wrong
      per-cluster 4^-e2 (cluster k scaled with cluster k ^ 1's);
   3. the emulated y stays within the bound of the dropped lo * lo product (and the FP16 / FP32 roundings of the lo
-     parts) of a float64 evaluation with the unsplit double factor, so the emulator models the same mathematics.
+     parts) of a float64 evaluation with the unsplit double factor, so the emulator models the same mathematics;
+  4. with components at pi = 0 (ck = -inf; one ahead of the others, one alone in the last pass, a whole pass) the
+     emulation gives them gamma = 0 exactly and the log-sum-exp of the others, and the faithful epilogue stays within a
+     quarter of the bar.
+  5. the scoring epilogue (fp32_score) on SCORE_SHAPES: faithful within a quarter of the bars (max_resp against gbar of
+     its label, logp against lbar, no sure label differing) and max_resp equal to fp32_gamma's value of the label; each of
+     SCORE_FAULTS fails at one shape at least (a later pass winning ties, kbase dropped, an earlier winner with the current
+     pass's M and S, the __expf(den - tot) factor dropped, a pass left out of the join).
+The shapes include D = 8, whose fused epilogue (estep_fused) forms the split epilogue's values (fp32_gamma); every fault
+exceeds the bar at a D = 8 shape.
 Run it as a script (python tests/test_estep_error_model.py) for the table of worst error / bar per shape.
 """
 import os
@@ -52,6 +61,7 @@ U = 2.0 ** -24
 LOG2E, LN2 = 1.4426950408889634, 0.6931471805599453
 LOG2E_F, LN2_F = float(np.float32(LOG2E)), float(np.float32(LN2))
 FTZ = 2.0 ** -126
+FLT_MAX = float(np.finfo(np.float32).max)
 FTZ_SLACK = 2.0 ** -122   # absolute slack of the bar: a responsibility (or a term of the denominator) below 2^-126 may be 0
 VARIANTS = ("faithful_rn", "faithful_trunc", "drop_zl_wh", "drop_zh_wl", "drop_vl", "chunk_swap", "wrong_e2")
 FAULTS = VARIANTS[2:]
@@ -197,18 +207,50 @@ def _ex2(a):
 
 
 def fp32_gamma(l, K):
-    """The split epilogue's FP32 operations per 64-cluster pass and, at K > 64, the join of the passes (modes 1, 2, 3)."""
+    """The split epilogue's FP32 operations per 64-cluster pass and, at K > 64, the join of the passes (modes 1, 2, 3).
+    The fused D = 8 epilogue (estep_fused) forms the same values: its lane qd sums the 4-cluster chunk 4 sg + cq of every
+    supergroup (cq = 0, 2, 1, 3 for qd = 0 .. 3) in (supergroup, cluster) order, starting from 0 and adding the exact 0 of
+    the supergroups past NSG; the two quad shuffles then give (P0 + P1) + (P2 + P3) on every lane (each addition is
+    commutative), which is a0 + a1 below with a_hh = p0 + p1 over the chunks hh and 2 + hh.  Its 1 / S, the join and the
+    mode 3 subtrahend fl32(tot * log2 e) (an FMUL of its own in the SASS, not contracted into the subtraction) are the
+    split kernel's operations.  Both start the maximum at -FLT_MAX: a pass without a finite logit (every pi 0) has S = 0,
+    a log-denominator of -inf and responsibilities of 0."""
+    passes, t_all, den, S_all, M_all = fp32_passes(l, K)
+    if len(passes) == 1:
+        g = f32(t_all[0] * f32(1.0 / S_all[0])[:, None])
+        return np.where(np.abs(g) < FTZ, 0.0, g), den[0]
+    tot = fp32_join(den)
+    out = []
+    sub = f32(tot * LOG2E_F)
+    for p, (k0, k1) in enumerate(passes):
+        if p == len(passes) - 1:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                scl = np.where(S_all[p] == 0, 0.0, f32(f32(1.0 / S_all[p]) * f32(np.exp(den[p] - tot))))
+            g = f32(t_all[p] * scl[:, None])
+        else:
+            g = _ex2(f32(l[:, k0:k1] - sub[:, None]))
+        out.append(np.where(np.abs(g) < FTZ, 0.0, g))
+    return np.concatenate(out, 1), tot
+
+
+PAD_L2 = float(np.float32(np.float32(-1e30) * np.float32(LOG2E_F)))   # a padding cluster's logit: ck = -1e30, multiplier 0
+
+
+def fp32_passes(l, K):
+    """Per 64-cluster pass: (k0, k1), the terms ex2(l - M) of its clusters, its log-denominator, S and M, with the
+    epilogue's FP32 operations.  The pass's padding clusters (up to a multiple of 16, tc_params_begin) are in M and S: their
+    logit is PAD_L2, so they add 0 unless no cluster of the pass has a finite logit (then S counts them); M starts at
+    -FLT_MAX, so a pass of 16 n clusters without a finite logit has S = 0 and a log-denominator of -inf."""
     N = l.shape[0]
     passes = [(p * 64, min(K, p * 64 + 64)) for p in range((K + 63) // 64)]
     t_all, den, S_all, M_all = [], [], [], []
     for k0, k1 in passes:
-        lp = l[:, k0:k1]
-        M = lp.max(1)
-        t = _ex2(f32(lp - M[:, None]))
         Kp = k1 - k0
         nsg = (Kp + 15) // 16
-        tt = np.zeros((N, nsg * 16))
-        tt[:, :Kp] = t
+        lp = np.concatenate([l[:, k0:k1], np.full((N, nsg * 16 - Kp), PAD_L2)], 1)
+        M = np.maximum(lp.max(1), -FLT_MAX)
+        tt = _ex2(f32(lp - M[:, None]))
+        t = tt[:, :Kp]
         a = []
         for hh in range(2):
             p0 = np.zeros(N)
@@ -220,27 +262,67 @@ def fp32_gamma(l, K):
                     p1 = f32(p1 + tt[:, 16 * sg + 8 + 4 * hh + i])
             a.append(f32(p0 + p1))
         S = f32(a[0] + a[1])
-        den.append(f32(M * LN2_F + f32(np.log(S))))
+        with np.errstate(divide="ignore"):
+            den.append(f32(M * LN2_F + f32(np.log(S))))
         t_all.append(t)
         S_all.append(S)
         M_all.append(M)
-    if len(passes) == 1:
-        g = f32(t_all[0] * f32(1.0 / S_all[0])[:, None])
-        return np.where(np.abs(g) < FTZ, 0.0, g), den[0]
+    return passes, t_all, den, S_all, M_all
+
+
+def join1(d, run):
+    """One join of a pass's log-denominator d with the running one (E-step modes 1 / 2, score_tc_kernel)."""
+    gm = np.maximum(np.maximum(d, run), -FLT_MAX)
+    with np.errstate(invalid="ignore"):
+        return f32(gm + f32(np.log(f32(f32(np.exp(d - gm)) + f32(np.exp(run - gm))))))
+
+
+def fp32_join(den):
     tot = den[0]
     for d in den[1:]:
-        gm = np.maximum(d, tot)
-        tot = f32(gm + f32(np.log(f32(f32(np.exp(d - gm)) + f32(np.exp(tot - gm))))))
-    out = []
-    sub = f32(tot * LOG2E_F)
+        tot = join1(d, tot)
+    return tot
+
+
+# ---- the scoring epilogue (score_tc_kernel) ----------------------------------------------------------------------------------
+SCORE_FAULTS = ("later_pass_wins_ties", "kbase_dropped", "earlier_winner_current_pass", "join_factor_dropped", "pass_left_out")
+
+
+def fp32_score(l, K, fault=None):
+    """(labels, max_resp, logp) of score_tc_kernel on the base-2 logits l [N][K], with its FP32 operations.
+    Per pass the arg-max runs over the lane's 16 logits in increasing k, then over the quad with (value, index) pairs and
+    the lower index on equal values: the first maximum in k order, numpy's argmax.  Across passes the running best is
+    replaced only by a strictly larger logit (an earlier pass wins ties), the label is kbase + k.  max_resp at K <= 64 is
+    ex2(bl - M) (1 / S); at K > 64 the last pass's winner takes ex2(bl - M) ((1 / S) __expf(den - tot)) (E-step mode 2) and
+    an earlier pass's winner ex2(bl - fl(tot log2 e)) (mode 3); logp is the joined log-denominator.  `fault` is one of
+    SCORE_FAULTS."""
+    N = l.shape[0]
+    passes, _, den, S_all, M_all = fp32_passes(l, K)
+    rows = np.arange(N)
+    rbl = rbk = rden = None
     for p, (k0, k1) in enumerate(passes):
-        if p == len(passes) - 1:
-            scl = f32(f32(1.0 / S_all[p]) * f32(np.exp(den[p] - tot)))
-            g = f32(t_all[p] * scl[:, None])
+        lp = l[:, k0:k1]
+        idx = np.argmax(lp, 1)
+        bl = lp[rows, idx]
+        bk = idx + (0 if fault == "kbase_dropped" else k0)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            inv_s = f32(1.0 / S_all[p])
+        if p == 0:
+            rbl, rbk, rden = bl, bk, den[0]
+            mr = f32(_ex2(f32(bl - M_all[0])) * inv_s)
+            continue
+        tot = den[p] if (fault == "pass_left_out" and p == 1) else join1(den[p], rden)
+        wins = bl >= rbl if fault == "later_pass_wins_ties" else bl > rbl
+        with np.errstate(invalid="ignore"):
+            sc = inv_s if fault == "join_factor_dropped" else f32(inv_s * f32(np.exp(den[p] - tot)))
+        mine = f32(_ex2(f32(bl - M_all[p])) * sc)
+        if fault == "earlier_winner_current_pass":
+            theirs = f32(_ex2(f32(rbl - M_all[p])) * f32(inv_s * f32(np.exp(den[p] - tot))))
         else:
-            g = _ex2(f32(l[:, k0:k1] - sub[:, None]))
-        out.append(np.where(np.abs(g) < FTZ, 0.0, g))
-    return np.concatenate(out, 1), tot
+            theirs = _ex2(f32(rbl - f32(tot * LOG2E_F)))
+        mr = np.where(wins, mine, theirs)
+        rbl, rbk, rden = np.where(wins, bl, rbl), np.where(wins, bk, rbk), tot
+    return rbk, np.where(np.abs(mr) < FTZ, 0.0, mr), rden
 
 
 def logits64(op, y):
@@ -248,11 +330,12 @@ def logits64(op, y):
 
 
 def lse2(l):
-    """gamma and the natural log-sum-exp of base-2 logits [N][K], in float64."""
-    M = l.max(1)
+    """gamma and the natural log-sum-exp of base-2 logits [N][K], in float64 (-inf, and gamma 0, where no logit is finite)."""
+    M = np.maximum(l.max(1), -FLT_MAX)
     t = np.exp2(l - M[:, None])
     S = t.sum(1)
-    return t / S[:, None], (M + np.log2(S)) * LN2
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.where(S[:, None] > 0, t / S[:, None], 0.0), (M + np.log2(S)) * LN2
 
 
 # ---- the bar --------------------------------------------------------------------------------------------------------------
@@ -264,7 +347,7 @@ def estep_bar(op, y, T, l, gamma, lse):
     qv = (y * y).sum(2)
     dqv = (2 * np.abs(y) * E + E * E).sum(2) + (2 * CP + 3) * U * qv
     dl = np.abs(op["mult"])[None] * dqv + U * np.abs(l)
-    M = l.max(1)
+    M = np.maximum(l.max(1), -FLT_MAX)
     r = LN2 * (dl + U * np.abs(l - M[:, None])) + 2.0 ** -22
     multi = K > 64
     if multi:                                              # the join of the passes' log-denominators and its base-2 conversion
@@ -279,10 +362,13 @@ def estep_bar(op, y, T, l, gamma, lse):
     hi = np.exp(r) * (1 + U) ** 2 / ((1 - rho) * (1 - s))[:, None] - 1
     lo = 1 - np.exp(-r) * (1 - U) ** 2 / ((1 + rho) * (1 + s))[:, None]
     gbar = np.where(live, gamma * np.maximum(hi, lo), 0.0) + FTZ_SLACK
+    # rho >= 1 (logits off by about an ulp of a logit near 2^23 or more, e.g. events 2^10 standard deviations out): the
+    # model bounds no responsibility of the event (it would give a negative bar), only its log-density
+    gbar = np.where((rho < 1.0)[:, None], gbar, np.inf)
     lbar = rho + s + 2.0 ** -22 * (np.abs(lse) + np.abs(M * LN2) + 1.0)
     if multi:
         lbar = lbar + 2.0 ** -20 * (1.0 + np.abs(lse))
-    return gbar, lbar
+    return gbar, lbar, dl
 
 
 class Emulation:
@@ -295,7 +381,7 @@ class Emulation:
         self.y, self.T = kept_y(self.op, self.zh, self.zl)
         self.l = logits64(self.op, self.y)
         self.gamma, self.lse = lse2(self.l)
-        self.gbar, self.lbar = estep_bar(self.op, self.y, self.T, self.l, self.gamma, self.lse)
+        self.gbar, self.lbar, self.dl = estep_bar(self.op, self.y, self.T, self.l, self.gamma, self.lse)
 
     def ratio(self, gamma):
         """Worst |gamma - gamma_emu| / bar over all events and clusters; gamma is [K][N] or [N][K]."""
@@ -305,7 +391,25 @@ class Emulation:
         return float((np.abs(g - self.gamma) / self.gbar).max())
 
     def lse_ratio(self, logp):
-        return float((np.abs(np.asarray(logp, np.float64) - self.lse) / self.lbar).max())
+        d = np.abs(np.asarray(logp, np.float64) - self.lse) / self.lbar
+        return float(np.where(np.isnan(d), np.inf, d).max())
+
+    def score_check(self, labels, max_resp, logp):
+        """gmm_score's outputs against the emulation: (worst |max_resp - gamma_emu[label]| / gbar[label], worst
+        |logp - lse| / lbar, events whose label differs from the emulated arg-max where that label is sure).  A label is
+        sure where the emulated top-two gap exceeds both logits' bars (dl, base 2), or where the top logits are exactly
+        equal (identical operands, identical FP32 logits: the lowest k wins)."""
+        lab = np.asarray(labels)
+        rows = np.arange(len(lab))
+        mr = np.asarray(max_resp, np.float64)
+        d = np.abs(mr - self.gamma[rows, lab]) / self.gbar[rows, lab]
+        r_mr = float(np.where(np.isnan(d), np.inf, d).max())      # a NaN max_resp fails
+        r_lp = self.lse_ratio(logp)
+        order = np.argsort(-self.l, axis=1, kind="stable")
+        top, second = order[:, 0], order[:, 1] if self.K > 1 else order[:, 0]
+        gap = self.l[rows, top] - self.l[rows, second]
+        sure = (gap > self.dl[rows, top] + self.dl[rows, second]) | (gap == 0) if self.K > 1 else np.ones(len(lab), bool)
+        return r_mr, r_lp, int((sure & (lab != top)).sum())
 
     def old_bar_passes(self, gamma):
         g = np.asarray(gamma, np.float64)
@@ -364,7 +468,7 @@ def oracle_y_ratio(em):
 
 # ---- parameter sets and shapes (shared with tests/test_gpu_estep_tc.py) ---------------------------------------------------
 KINDS = ("fitted", "spd", "needle")
-ERR_D = (16, 24)
+ERR_D = (8, 16, 24)
 ERR_K = (17, 64, 129)
 N_FIT = 20_000
 N_DATA = 480_000          # the deep shapes of the GPU test use a prefix of these events
@@ -444,6 +548,84 @@ def test_each_kernel_fault_exceeds_the_bar():
         assert worst[v] > 1.0, (v, worst[v])
     # a chunk swap the per-operator bar (1e-4 relative, 1e-6 absolute) passes, and this bar does not
     assert any(r["chunk_swap"] > 1.0 and r["chunk_swap_old_bar_passes"] for r in res.values())
+
+
+# ---- the scoring epilogue: shapes, faithful emulation and faults ------------------------------------------------------------
+SCORE_SHAPES = [(kind, D, K) for kind in ("fitted", "spd") for D in ERR_D for K in (7, 65, 129)] + [("dup", D, 129) for D in ERR_D]
+_score_cache = {}
+
+
+def score_shape(kind, D, K):
+    """Emulation and score outputs on N_CPU events: "dup" is the fitted set with cluster k + 64 a copy of cluster k."""
+    key = (kind, D, K)
+    if key not in _score_cache:
+        pkg = entry.load_package()
+        oracle = entry.load_oracle("f64")
+        ev = blobs(D)
+        cl = param_set(pkg, oracle, "fitted" if kind == "dup" else kind, D, K, ev)
+        if kind == "dup":
+            for f in ("means", "R", "Rinv", "constant", "pi", "N"):
+                getattr(cl, f)[64:128] = getattr(cl, f)[0:64]
+        shift, scale = standardise(ev)[:2]
+        em = Emulation(cl, K, ev[:N_CPU], shift, scale)
+        res = {}
+        for trunc in (False, True):
+            l32 = fp32_logits(em.op, fp32_y(em.op, em.zh, em.zl, trunc=trunc))
+            lab, mr, lp = fp32_score(l32, K)
+            g = fp32_gamma(l32, K)[0]
+            res["faithful_" + ("trunc" if trunc else "rn")] = em.score_check(lab, mr, lp)
+            # max_resp is the E-step's stored responsibility of the label, bit for bit
+            res["identity_" + ("trunc" if trunc else "rn")] = bool(np.array_equal(mr, g[np.arange(len(lab)), lab]))
+            if not trunc:
+                for v in SCORE_FAULTS:
+                    res[v] = em.score_check(*fp32_score(l32, K, fault=v))
+        _score_cache[key] = res
+    return _score_cache[key]
+
+
+@pytest.mark.parametrize("kind,D,K", SCORE_SHAPES)
+def test_score_faithful_within_quarter_bar(kind, D, K):
+    r = score_shape(kind, D, K)
+    print(f"\nscore {kind} D={D} K={K}: " + "  ".join(f"{v} {r[v][0]:.3g}/{r[v][1]:.3g}/{r[v][2]}" for v in ("faithful_rn", "faithful_trunc") + SCORE_FAULTS))
+    for v in ("faithful_rn", "faithful_trunc"):
+        assert r[v][0] <= 0.25 and r[v][1] <= 0.25 and r[v][2] == 0, (v, r[v])
+        assert r["identity_" + v[9:]], v
+
+
+def test_each_scoring_fault_fails():
+    """Each fault exceeds the max_resp or the logp bar, or gives a sure label that differs, at some shape."""
+    res = {s: score_shape(*s) for s in SCORE_SHAPES}
+    for v in SCORE_FAULTS:
+        caught = [s for s, r in res.items() if r[v][0] > 1.0 or r[v][1] > 1.0 or r[v][2] > 0]
+        print(f"\n  {v}: caught at {len(caught)} of {len(res)} shapes")
+        assert caught, v
+
+
+@pytest.mark.parametrize("D,K,zero", [(8, 17, [0]), (16, 65, [64]), (24, 129, list(range(64))), (8, 130, list(range(64, 128))),
+                                      (16, 70, [0, 5, 63]), (8, 80, list(range(64, 80))),
+                                      (24, 128, list(range(64, 128)))])
+def test_zero_pi_components(D, K, zero):
+    """pi = 0: ck = -inf.  The emulation gives those components gamma = 0 exactly and the log-sum-exp of the others, the
+    bar is finite, and the faithful FP32 epilogue (a -inf pass maximum floored at -FLT_MAX) stays within a quarter of it."""
+    pkg = entry.load_package()
+    oracle = entry.load_oracle("f64")
+    ev = blobs(D)
+    cl = param_set(pkg, oracle, "fitted", D, K, ev)
+    cl.pi[zero] = 0.0
+    shift, scale = standardise(ev)[:2]
+    with np.errstate(divide="ignore"):
+        em = Emulation(cl, K, ev[:N_CPU], shift, scale)
+    assert np.all(em.op["ck"][zero] == -np.inf) and np.all(em.l[:, zero] == -np.inf)
+    for a in (em.gamma, em.lse, em.gbar, em.lbar):
+        assert not np.isnan(a).any()
+    assert np.all(em.gamma[:, zero] == 0.0) and np.isfinite(em.lse).all()
+    keep = np.setdiff1d(np.arange(K), zero)
+    np.testing.assert_allclose(em.lse, lse2(em.l[:, keep])[1], rtol=1e-15, atol=0)
+    for v in ("faithful_rn", "faithful_trunc"):
+        with np.errstate(divide="ignore", invalid="ignore"):
+            g = variant_gamma(em, v)
+        assert not np.isnan(g).any() and np.all(g[:, zero] == 0.0), v
+        assert em.ratio(g) <= 0.25, (v, em.ratio(g))
 
 
 def test_bar_helpers_on_a_known_case():

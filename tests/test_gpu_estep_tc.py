@@ -12,7 +12,7 @@ Identities (exact unless stated):
      and sliced memberships of the resident E-step (same engine, so the same centre and scale);
   2. the shallow ring: chunks of 128 SMs events (at most 2 tiles per CTA, no slot reused), and chunks of one tile, give
      the deep run's memberships;
-  3. gmm_score's max_resp is the top membership bit for bit at K <= 64 (within 1e-6 above), its label the arg-max
+  3. gmm_score's max_resp is the top membership bit for bit at every K, its label the arg-max
      wherever the top two differ;
   4. the log-likelihood of gmm_estep (float32) is within 1 float32 ulp of float32(sum_e float64(logp_e)), logp from
      gmm_score (the same denominators);
@@ -125,7 +125,7 @@ def test_deep_ring_identities(pkg, D, K):
     with engine(pkg, ev, K) as eng:
         ll, memb = resident(eng, K, mixture(pkg, ev, K))
         # 3. cross-kernel, 4. log-likelihood accounting
-        lab, mr, lp = check_shard(eng, K, ev, ll, bit_exact_mr=K <= 64)
+        lab, mr, lp = check_shard(eng, K, ev, ll)
         assert_ll_ulp(ll, lp, "estep vs score")
         # 1. position invariance, one chunk
         eng.score_stats_profile(reset=True)
@@ -161,7 +161,7 @@ def test_small_shapes_and_one_tile_launches(pkg, D, K):
         ev = np.ascontiguousarray(ev_all[:n])
         with engine(pkg, ev, K) as eng:
             ll, memb = resident(eng, K, cl)
-            lab, mr, lp = check_shard(eng, K, ev, ll, bit_exact_mr=K <= 64)
+            lab, mr, lp = check_shard(eng, K, ev, ll)
             assert_ll_ulp(ll, lp, name)
             np.testing.assert_array_equal(score_memberships(eng, K, ev, TILE), memb, err_msg=f"{name}: one tile per launch")
             r = min(37, n - 1)

@@ -12,7 +12,8 @@ The emulator restates the kernel's logits bit for bit:
 Everything after the logits is measured against gamma = exp(l - LSE(l)) and LSE(l) in float64 of the emulated logits.
 
 The bar covers what is not emulated.  cuobjdump -sass of the kernel shows the logit operations as written and the online
-update contracted to one FFMA, run_sum = fma(run_sum, expf(run_max - m2), expf(l - m2)).  The error of run_sum is carried
+update contracted to one FFMA, run_sum = fma(run_sum, expf(run_max - m2), expf(l - m2)), with run_max starting at
+-FLT_MAX (a component with pi = 0 has the logit -inf and adds expf(-inf) = 0).  The error of run_sum is carried
 through the K steps in the kernel's order (simt_bar), to first order in each step:
   * each expf: at most 2 ulp (2^-22 relative; the CUDA Math API, the build has no -use_fast_math), after the rounding of
     its argument (u |a|, u = 2^-24), and 2^-148 absolute for results in the subnormal range (no FTZ in this build);
@@ -36,6 +37,8 @@ The module asserts, on the shapes of tests/test_gpu_simt.py:
      using run_max instead of denom, and coordinate 0 read from the next SoA row;
   3. the emulated logits agree with a float64 evaluation of -1/2 (x - mu)^T Rinv (x - mu) + constant + ln pi within the
      a-priori bound of the FP32 triangle, so the emulator computes the same mathematics.
+  4. with components at pi = 0 (the first, the last, a whole 16-cluster chunk, the first chunk) the faithful emulation gives
+     them a responsibility of exactly 0, and the others and the log-densities stay within FAITHFUL_MAX of the bar.
 Run it as a script (python tests/test_simt_error_model.py) for the table of worst error / bar per shape.
 """
 import ctypes
@@ -55,6 +58,7 @@ LOG_ULP = 2.0 ** -23          # logf: 1 ulp
 EXP_SUB = 2.0 ** -148         # expf: 2 ulp of a subnormal result
 FLOOR = 2.0 ** -146           # absolute part of the responsibility bar
 CHUNK = 16                    # kEstepClusterChunk
+FLT_MAX = float(np.finfo(np.float32).max)
 FAITHFUL_MAX = 0.9            # the faithful FP32 emulation's share of the bar (module docstring, item 1)
 FAULTS = ("uncombined", "stale_chunk", "no_rescale", "no_ln_pi", "sweep_run_max", "next_row")
 
@@ -141,12 +145,14 @@ def lse64(l):
 def simt_bar(l):
     """gamma, LSE (float64 of the emulated logits [n][K]) and the per-(event, cluster) / per-event bars."""
     n, K = l.shape
-    Mx = np.full(n, -np.inf)
+    Mx = np.full(n, -FLT_MAX)                    # the kernel's start: a -inf logit (pi = 0) ahead of every finite one adds 0
     Sx = np.zeros(n)
     B = np.zeros(n)
 
     def rel(a):                                  # relative error of expf(fl32(a)) against exp(a)
-        fa = np.isfinite(a)
+        # expf(-inf) and expf(-FLT_MAX - l) (the start of the running maximum, a < -FLT_MAX / 2 for any logit l of the
+        # kernel's range) are exactly 0 and carry no error
+        fa = np.isfinite(a) & (a > -0.5 * FLT_MAX)
         return np.where(fa, EXP_REL + np.expm1(U * np.abs(np.where(fa, a, 0.0))) * (1 + EXP_REL), 0.0)
 
     for k in range(K):
@@ -175,7 +181,7 @@ def faithful(l):
     """The kernel's FP32 sequence after the logits, expf / logf as float32 roundings of float64: (gamma, denom)."""
     n, K = l.shape
     l32 = l.astype(np.float32)
-    run_max = np.full(n, -np.inf, np.float32)
+    run_max = np.full(n, -FLT_MAX, np.float32)
     run_sum = np.zeros(n)
     for k in range(K):
         m2 = np.maximum(run_max, l32[:, k])
@@ -320,6 +326,31 @@ def test_each_kernel_fault_exceeds_the_bar():
         old = [s for s, r in res.items() if r[v] > 1.0 and r[v + "_old_bar_passes"]]
         print(f"  {v}: above the bar at {len(caught)} of {len(res)} shapes, {len(old)} of them pass the old 1e-4 / 1e-6 bar")
         assert worst[v] > 1.0, (v, worst[v])
+
+
+ZERO_PI = {"first": (7, [0]), "last": (7, [6]), "chunk1": (40, list(range(16, 32))), "chunk0": (40, list(range(16)))}
+
+
+@pytest.mark.parametrize("case", list(ZERO_PI))
+@pytest.mark.parametrize("D", (5, 24))
+def test_zero_pi_components(case, D):
+    K, zero = ZERO_PI[case]
+    pkg = entry.load_package()
+    oracle = entry.load_oracle("f64")
+    ev = blobs(N_LARGE_K, D, K)
+    cl = param_set(pkg, oracle, "fitted", D, K, ev)
+    cl.pi[zero] = 0.0
+    with np.errstate(invalid="ignore"):          # fma32's TwoSum tail is NaN for c = -inf; the rounded -inf is kept
+        l = logits(np.ascontiguousarray(ev[:N_CPU]), epack(cl, K))
+    assert np.all(l[:, zero] == -np.inf) and np.isfinite(np.delete(l, zero, 1)).all()
+    with np.errstate(invalid="ignore"):          # (-inf) - (-FLT_MAX) etc. inside the bar; its results are checked below
+        gamma, lse, gbar, lbar = simt_bar(l)
+    g, den = faithful(l)
+    for a in (gamma, lse, gbar, lbar, g, den):
+        assert not np.isnan(a).any(), case
+    assert np.all(g[:, zero] == 0.0) and np.all(gamma[:, zero] == 0.0)
+    np.testing.assert_allclose(lse, lse64(np.delete(l, zero, 1)), rtol=1e-15, atol=0)
+    assert (np.abs(g - gamma) / gbar).max() <= FAITHFUL_MAX and (np.abs(den - lse) / lbar).max() <= FAITHFUL_MAX
 
 
 def _exact_fma32(a, b, c):
