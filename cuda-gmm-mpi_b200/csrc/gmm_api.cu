@@ -24,11 +24,13 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <string>
 #include <thread>
 #include <vector>
 
 #include "../../include/gmm.h"
+#include "cuda_owned.h"
 #include "host_math.h"
 #include "kernels_simt.cuh"
 #include "kernels_condition.cuh"
@@ -39,13 +41,6 @@
 #include "kernels_combine.cuh"
 
 namespace gmm {
-
-#define CUDA_TRY(expr)                                                                        \
-    do {                                                                                      \
-        cudaError_t e_ = (expr);                                                              \
-        if (e_ != cudaSuccess)                                                                \
-            return fail(GMM_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));    \
-    } while (0)
 
 // ---- NCCL, loaded lazily so that the library imports without it -----------
 struct NcclApi {
@@ -91,17 +86,19 @@ struct PhaseTimer {          // replaces cudaTimer_t / profile_t (gaussian.cu:33
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> pending;
     double total_ms = 0;
 };
-// Timing events are recycled: cudaEventCreate / Destroy cost microseconds each and sat inside the EM loop.
+// Timing events are recycled: cudaEventCreate / Destroy cost microseconds each and sat inside the EM loop.  The pool owns
+// every event it made, lent or not.
 struct EventPool {
+    std::vector<Event> owned;
     std::vector<cudaEvent_t> free_list;
     cudaEvent_t get() {
         if (!free_list.empty()) { cudaEvent_t e = free_list.back(); free_list.pop_back(); return e; }
-        cudaEvent_t e = nullptr;
-        cudaEventCreate(&e);
-        return e;
+        Event e;
+        if (e.create(cudaEventDefault) != GMM_OK) return nullptr;
+        owned.push_back(std::move(e));
+        return owned.back();
     }
     void put(cudaEvent_t e) { if (e) free_list.push_back(e); }
-    void destroy() { for (cudaEvent_t e : free_list) cudaEventDestroy(e); free_list.clear(); }
 };
 
 // Persistent worker team for the per-iteration host finalisation (K independent clusters, a few microseconds each).
@@ -217,7 +214,7 @@ struct PeerTable {
 };
 struct PeerExchange {
     PeerTable tab{};
-    void* base = nullptr;                       // own allocation: [2][cap] doubles, then the flags
+    DeviceArray<char> base;                     // own allocation: [2][cap] doubles, then the flags
     void* opened[kXMaxRanks] = {nullptr};       // cudaIpcOpenMemHandle results to close
     unsigned long long epoch = 0;
     bool ok = false;
@@ -278,38 +275,20 @@ allreduce_peer_kernel(PeerTable t, double* __restrict__ stats, int len, int pari
 // plus the running state of the tensor kernel's passes (K > 64).
 struct ScoreBuffers {
     long long cap = 0;                          // events per chunk
-    float* h_in[2] = {nullptr, nullptr};
-    float* d_in[2] = {nullptr, nullptr};
-    char* d_out[2] = {nullptr, nullptr};
-    char* h_out[2] = {nullptr, nullptr};
-    float* d_run_den = nullptr;
-    float* d_run_bl = nullptr;
-    int* d_run_bk = nullptr;
-    cudaStream_t copy = nullptr;                // H2D of the next chunk / D2H of the last one, beside the kernels
-    cudaEvent_t h2d[2] = {nullptr, nullptr}, kern[2] = {nullptr, nullptr}, d2h[2] = {nullptr, nullptr};
-    cudaEvent_t t0[2] = {nullptr, nullptr}, t1[2] = {nullptr, nullptr};
+    PinnedArray<float> h_in[2];
+    DeviceArray<float> d_in[2];
+    DeviceArray<char> d_out[2];
+    PinnedArray<char> h_out[2];
+    DeviceArray<float> d_run_den;
+    DeviceArray<float> d_run_bl;
+    DeviceArray<int> d_run_bk;
+    Stream copy;                                // H2D of the next chunk / D2H of the last one, beside the kernels
+    Event h2d[2], kern[2], d2h[2];
+    Event t0[2], t1[2];
     double kernel_ms = 0, wall_ms = 0;          // gmm_get_score_profile
     long long tensor_chunks = 0, simt_chunks = 0;
     static constexpr size_t kHeader = 16;
     static size_t out_bytes(long long cap) { return kHeader + (size_t)cap * 12; }
-    void release() {
-        for (int s = 0; s < 2; s++) {
-            if (h_in[s]) cudaFreeHost(h_in[s]);
-            if (h_out[s]) cudaFreeHost(h_out[s]);
-            cudaFree(d_in[s]); cudaFree(d_out[s]);
-            h_in[s] = d_in[s] = nullptr; h_out[s] = d_out[s] = nullptr;
-        }
-        cudaFree(d_run_den); cudaFree(d_run_bl); cudaFree(d_run_bk);
-        d_run_den = d_run_bl = nullptr; d_run_bk = nullptr;
-        cap = 0;
-    }
-    void destroy() {
-        release();
-        for (int s = 0; s < 2; s++)
-            for (cudaEvent_t* e : {&h2d[s], &kern[s], &d2h[s], &t0[s], &t1[s]})
-                if (*e) { cudaEventDestroy(*e); *e = nullptr; }
-        if (copy) { cudaStreamDestroy(copy); copy = nullptr; }
-    }
 };
 
 // Time and kernel counts of the calls that stream E- and M-steps over chunks (gmm_get_score_stats_profile,
@@ -326,134 +305,76 @@ struct StatsProfile {
 struct ScoreStatsBuffers {
     long long cap = 0;                          // events per chunk
     size_t pitch = 0;                           // row pitch in floats of the SoA copies and the responsibilities (multiple of 32)
-    float* d_z = nullptr;                       // [D][pitch] standardised SoA copy (tensor M-step)
-    float* d_xs = nullptr;                      // [D][pitch] raw SoA copy (SIMT kernels)
-    float* d_xo = nullptr;                      // [D][pitch] observed SoA copy of gmm_condition_stats (its n_obs rows)
-    float* d_shift_f = nullptr;                 // [GMM_MAX_DIMENSIONS] the centre in float (gmm_condition_stats' missing rows)
-    float* d_memb = nullptr;                    // [8 ceil(Kmax / 8)][pitch] responsibilities of the chunk
-    float* h_memb = nullptr;                    // pinned [Kmax][cap]
-    double* d_stats = nullptr;                  // [Kmax F + 1]
-    double* h_stats = nullptr;                  // pinned
-    int* d_flag = nullptr;
-    int* h_flag = nullptr;                      // pinned
-    cudaEvent_t ev_flag = nullptr;
-    cudaEvent_t p0[2] = {nullptr, nullptr}, p1[2] = {nullptr, nullptr}, k0[2] = {nullptr, nullptr}, k1[2] = {nullptr, nullptr};
+    DeviceArray<float> d_z;                     // [D][pitch] standardised SoA copy (tensor M-step)
+    DeviceArray<float> d_xs;                    // [D][pitch] raw SoA copy (SIMT kernels)
+    DeviceArray<float> d_xo;                    // [D][pitch] observed SoA copy of gmm_condition_stats (its n_obs rows)
+    DeviceArray<float> d_shift_f;               // [GMM_MAX_DIMENSIONS] the centre in float (gmm_condition_stats' missing rows)
+    DeviceArray<float> d_memb;                  // [8 ceil(Kmax / 8)][pitch] responsibilities of the chunk
+    PinnedArray<float> h_memb;                  // [Kmax][cap]
+    DeviceArray<double> d_stats;                // [Kmax F + 1]
+    PinnedArray<double> h_stats;
+    DeviceArray<int> d_flag;
+    PinnedArray<int> h_flag;
+    Event ev_flag;
+    Event p0[2], p1[2], k0[2], k1[2];
     StatsProfile prof;                          // gmm_get_score_stats_profile
     StatsProfile cond_prof;                     // gmm_get_condition_stats_profile
-    void release_chunk() {
-        cudaFree(d_z); cudaFree(d_xs); cudaFree(d_xo); cudaFree(d_memb);
-        if (h_memb) cudaFreeHost(h_memb);
-        d_z = d_xs = d_xo = d_memb = h_memb = nullptr;
-        cap = 0; pitch = 0;
-    }
-    void destroy() {
-        release_chunk();
-        cudaFree(d_stats); cudaFree(d_flag); cudaFree(d_shift_f);
-        d_shift_f = nullptr;
-        if (h_stats) cudaFreeHost(h_stats);
-        if (h_flag) cudaFreeHost(h_flag);
-        d_stats = h_stats = nullptr; d_flag = h_flag = nullptr;
-        if (ev_flag) { cudaEventDestroy(ev_flag); ev_flag = nullptr; }
-        for (int b = 0; b < 2; b++)
-            for (cudaEvent_t* e : {&p0[b], &p1[b], &k0[b], &k1[b]})
-                if (*e) { cudaEventDestroy(*e); *e = nullptr; }
-    }
 };
 
-// gmm_seed_kmeans' buffers: allocated on its first call (the shard's size is fixed), freed by gmm_destroy.
+// gmm_seed_kmeans' buffers, allocated on its first call (the shard's size is fixed; the transfer slots follow the rank count).
 struct KmeansBuffers {
-    bool ready = false;
-    int nb = 0, nba = 0, nxfer = 0;             // blocks of the k-means++ kernels / of the assignment; slots of d_xfer
-    double* d_d2 = nullptr;                     // [n] squared distance to the nearest chosen centre
-    int* d_labels = nullptr;                    // [n] Lloyd labels
-    double* d_bsum = nullptr;                   // [nb] per-block sums of d2
-    double* d_bpot = nullptr;                   // [nb][kSeedMaxCand] per-block candidate potentials
-    int* d_bchanged = nullptr;                  // [nba] changed labels per assignment block
-    double* d_binertia = nullptr;               // [nba] distances per assignment block
-    float* d_cand = nullptr;                    // [kSeedMaxCand][D] candidate rows
-    SeedPick* d_pick = nullptr;                 // [kSeedMaxCand]
-    int* d_pick_idx = nullptr;                  // [kSeedMaxCand]
-    float* d_centres = nullptr;                 // [Kmax][D]
-    double* d_xfer = nullptr;                   // [nranks][16] zero-padded per-rank values
-    double* h_bsum = nullptr;                   // pinned mirrors
-    double* h_bpot = nullptr;
-    int* h_bchanged = nullptr;
-    double* h_binertia = nullptr;
-    SeedPick* h_pick = nullptr;
-    double* h_xfer = nullptr;
-    void destroy() {
-        cudaFree(d_d2); cudaFree(d_labels); cudaFree(d_bsum); cudaFree(d_bpot); cudaFree(d_bchanged); cudaFree(d_binertia);
-        cudaFree(d_cand); cudaFree(d_pick); cudaFree(d_pick_idx); cudaFree(d_centres); cudaFree(d_xfer);
-        for (void* p : {(void*)h_bsum, (void*)h_bpot, (void*)h_bchanged, (void*)h_binertia, (void*)h_pick, (void*)h_xfer})
-            if (p) cudaFreeHost(p);
-        *this = KmeansBuffers();
-    }
+    int nb = 0, nba = 0;                        // blocks of the k-means++ kernels / of the assignment
+    DeviceArray<double> d_d2;                   // [n] squared distance to the nearest chosen centre
+    DeviceArray<int> d_labels;                  // [n] Lloyd labels
+    DeviceArray<double> d_bsum;                 // [nb] per-block sums of d2
+    DeviceArray<double> d_bpot;                 // [nb][kSeedMaxCand] per-block candidate potentials
+    DeviceArray<int> d_bchanged;                // [nba] changed labels per assignment block
+    DeviceArray<double> d_binertia;             // [nba] distances per assignment block
+    DeviceArray<float> d_cand;                  // [kSeedMaxCand][D] candidate rows
+    DeviceArray<SeedPick> d_pick;               // [kSeedMaxCand]
+    DeviceArray<int> d_pick_idx;                // [kSeedMaxCand]
+    DeviceArray<float> d_centres;               // [Kmax][D]
+    DeviceArray<double> d_xfer;                 // [nranks][16] zero-padded per-rank values
+    PinnedArray<double> h_bsum;                 // pinned mirrors
+    PinnedArray<double> h_bpot;
+    PinnedArray<int> h_bchanged;
+    PinnedArray<double> h_binertia;
+    PinnedArray<SeedPick> h_pick;
+    PinnedArray<double> h_xfer;
 };
 
-// gmm_sample's parameter block (kernels_sample.cuh layout, sized for Kmax) and its pinned staging: allocated on the first
-// call, freed by gmm_destroy.  Its chunks stream through gmm_score's slots.
+// gmm_sample's parameter block (kernels_sample.cuh layout, sized for Kmax) and its pinned staging, allocated on the first
+// call.  Its chunks stream through gmm_score's slots.
 struct SampleBuffers {
-    double* d_block = nullptr;
-    char* h_block = nullptr;
+    DeviceArray<double> d_block;
+    PinnedArray<char> h_block;
     double kernel_ms = 0, wall_ms = 0;          // gmm_get_sample_profile
-    void destroy() {
-        cudaFree(d_block);
-        if (h_block) cudaFreeHost(h_block);
-        d_block = nullptr; h_block = nullptr;
-    }
 };
 
 // gmm_condition's parameter block (sized for Kmax and the largest record any observed set of this D needs) and its
 // pinned mirror, allocated on the first call; per slot of gmm_score's two, the imputations of a chunk (device and pinned:
 // cond_mean [chunk][NM] then cond_var [chunk][NM]), allocated on the first imputing call and grown with chunk x NM, never
-// shrunk.  All freed by gmm_destroy.  Its chunks stream through gmm_score's slots.
+// shrunk.  Its chunks stream through gmm_score's slots.
 struct ConditionBuffers {
-    float* d_block = nullptr;
-    float* h_block = nullptr;
-    float* d_imp[2] = {nullptr, nullptr};
-    float* h_imp[2] = {nullptr, nullptr};
-    size_t imp_floats = 0;                      // floats per slot
+    DeviceArray<float> d_block;
+    PinnedArray<float> h_block;
+    DeviceArray<float> d_imp[2];
+    PinnedArray<float> h_imp[2];
     double kernel_ms = 0, wall_ms = 0;          // gmm_get_condition_profile
-    void release_imp() {
-        for (int s = 0; s < 2; s++) {
-            cudaFree(d_imp[s]);
-            if (h_imp[s]) cudaFreeHost(h_imp[s]);
-            d_imp[s] = h_imp[s] = nullptr;
-        }
-        imp_floats = 0;
-    }
-    void destroy() {
-        release_imp();
-        cudaFree(d_block);
-        if (h_block) cudaFreeHost(h_block);
-        d_block = h_block = nullptr;
-    }
 };
 
 // gmm_combine / gmm_combine_labels: per-(range, value) partials of the passes, their reduced sums and pinned mirror (sized
-// for the largest pass seen), the live groups' member lists, and the labels' device outputs; allocated on first use, freed
-// by gmm_destroy.
+// for the largest pass seen), the live groups' member lists, and the labels' device outputs; allocated on first use.
 struct CombineBuffers {
-    double* d_part = nullptr;
-    size_t part_doubles = 0;
-    double* d_sum = nullptr;
-    double* h_sum = nullptr;
-    size_t sum_doubles = 0;
-    int* d_groups = nullptr;                    // [2 kCombMaxK + 1]: members, then offsets
-    int* h_groups = nullptr;                    // pinned
-    int* d_lab = nullptr;                       // [memb_pitch]
-    float* d_max = nullptr;                     // [memb_pitch]
-    cudaEvent_t t0 = nullptr, t1 = nullptr;
+    DeviceArray<double> d_part;
+    DeviceArray<double> d_sum;
+    PinnedArray<double> h_sum;
+    DeviceArray<int> d_groups;                  // [2 kCombMaxK + 1]: members, then offsets
+    PinnedArray<int> h_groups;
+    DeviceArray<int> d_lab;                     // [memb_pitch]
+    DeviceArray<float> d_max;                   // [memb_pitch]
+    Event t0, t1;
     double kernel_ms = 0, wall_ms = 0, labels_wall_ms = 0;   // gmm_get_combine_profile
-    void destroy() {
-        cudaFree(d_part); cudaFree(d_sum); cudaFree(d_groups); cudaFree(d_lab); cudaFree(d_max);
-        if (h_sum) cudaFreeHost(h_sum);
-        if (h_groups) cudaFreeHost(h_groups);
-        if (t0) cudaEventDestroy(t0);
-        if (t1) cudaEventDestroy(t1);
-        d_part = d_sum = h_sum = nullptr; d_groups = h_groups = d_lab = nullptr; d_max = nullptr; t0 = t1 = nullptr;
-        part_doubles = sum_doubles = 0;
-    }
 };
 
 }  // namespace gmm
@@ -461,24 +382,24 @@ struct CombineBuffers {
 using namespace gmm;
 
 struct gmm_ctx {
+    Stream stream;               // first member: destroyed last, after every buffer and event its work may use
     int device = 0, n = 0, D = 0, Kmax = 0, F = 0;
     long long n_global = 0, offset = 0;
-    cudaStream_t stream = nullptr;
     int num_sms = 132;
     // events
-    float* d_x_aos = nullptr;    // [n][D]  as supplied (TMA source of the tensor path)
-    float* d_x_soa = nullptr;    // [D][n]  transpose for the SIMT kernels
+    DeviceArray<float> d_x_aos;  // [n][D]  as supplied (TMA source of the tensor path)
+    DeviceArray<float> d_x_soa;  // [D][n]  transpose for the SIMT kernels
     // responsibilities, cluster-major [Kmax][n]
-    float* d_memb = nullptr;
+    DeviceArray<float> d_memb;
     size_t memb_pitch = 0;           // row pitch in floats (multiple of 32: TMA-aligned rows)
-    float* d_memb_saved = nullptr;   // best configuration during gmm_fit
-    cudaEvent_t ev_stats = nullptr;  // statistics have reached the host
+    DeviceArray<float> d_memb_saved; // best configuration during gmm_fit
+    Event ev_stats;                  // statistics have reached the host
     // parameters
-    float* d_epack = nullptr;    // SIMT E-step parameters [Kmax][epack_stride]
-    float* h_epack = nullptr;    // pinned staging
-    double* d_stats = nullptr;   // [Kmax*F + 1]
-    double* h_stats = nullptr;   // pinned
-    double* d_shift = nullptr;   // [32]
+    DeviceArray<float> d_epack;  // SIMT E-step parameters [Kmax][epack_stride]
+    PinnedArray<float> h_epack;  // staging
+    DeviceArray<double> d_stats; // [Kmax*F + 1]
+    PinnedArray<double> h_stats;
+    DeviceArray<double> d_shift; // [32]
     double shift[GMM_MAX_DIMENSIONS] = {0};
     bool have_shift = false;
     double scale[GMM_MAX_DIMENSIONS] = {0};   // global per-dimension standard deviation
@@ -506,8 +427,8 @@ struct gmm_ctx {
     double fit_reduce_ms = 0, fit_seed_ms = 0, fit_save_ms = 0;   // gmm_fit phases (gmm_get_fit_profile)
     long long mstep_tensor = 0, mstep_simt = 0;                   // M-step launches by kernel
     long long iterations = 0;
-    TcState* tc = nullptr;       // tensor-core path state (kernels_tc.cuh)
-    HostPool* pool = nullptr;    // worker team of the per-iteration host finalisation (created on first use)
+    std::unique_ptr<TcState, TcStateDelete> tc;   // tensor-core path state (kernels_tc.cuh)
+    std::unique_ptr<HostPool> pool;              // worker team of the per-iteration host finalisation (created on first use)
     PeerExchange xchg;           // peer-memory all-reduce of the statistics (gmm_comm_init; falls back to NCCL)
     int allreduce_mode = 1;      // option "allreduce": 1 = peer-memory kernel when available, 0 = ncclAllReduce
     bool estep_tensor_ready = false;   // the tensor E-step operand of the current parameters is uploaded
@@ -515,12 +436,12 @@ struct gmm_ctx {
     int finalize_mode = 1;       // option "finalize": 1 = on the device when the tensor E-step serves the state, 0 = host
     bool dev_fin_failed = false; // a cluster needed the host path once: this context stays on it
     bool dev_fin_agreed = true;  // every rank of the communicator can (gmm_comm_init): the replay re-issues collectives
-    float* d_pset[2] = {nullptr, nullptr};   // parameter sets written by the kernel (iteration parity)
-    float* h_pset = nullptr;     // pinned staging of one set
-    float* d_avgvar = nullptr;   // [Kmax]
-    int* d_bad = nullptr;        // [2] first failed iteration (-1), code
-    double* d_llprev = nullptr;  // [2] log-likelihood slot seen by the finalisation of iteration parity
-    char* h_small = nullptr;     // pinned: int bad[2] | double ll[2] | float avgvar[Kmax]
+    DeviceArray<float> d_pset[2];   // parameter sets written by the kernel (iteration parity)
+    PinnedArray<float> h_pset;   // staging of one set
+    DeviceArray<float> d_avgvar; // [Kmax]
+    DeviceArray<int> d_bad;      // [2] first failed iteration (-1), code
+    DeviceArray<double> d_llprev;   // [2] log-likelihood slot seen by the finalisation of iteration parity
+    PinnedArray<char> h_small;   // int bad[2] | double ll[2] | float avgvar[Kmax]
     PhaseTimer t_final;
     long long dev_finalize_launches = 0, dev_replays = 0;
     int fin_fault_iter = -1;     // option "finalize_fault_iter" (tests): that iteration of the next batch reports a failure
@@ -534,15 +455,15 @@ struct gmm_ctx {
     SampleBuffers sample;        // gmm_sample: parameter block, allocated on first use
     ConditionBuffers cond;       // gmm_condition: parameter block and imputation buffers, allocated on first use
     // gmm_set_weights: per-event weights of the shard, used by the E-step log-likelihood and the M-step statistics
-    float* d_w = nullptr;        // [memb_pitch], zero beyond n (allocated on the first call)
+    DeviceArray<float> d_w;      // [memb_pitch], zero beyond n (allocated on the first call)
     bool weighted = false;       // d_w is in effect
     double w_total = 0;          // global sum of the weights (the N of the default epsilon and of the Rissanen score)
     double w_scale = 1;          // the global largest weight (the tensor M-step divides the weights by it)
     bool w_tensor_ok = true;     // the weights' dynamic range fits the tensor M-step (kWeightRangeTc)
     bool seeding = false;        // gmm_seed_kmeans: its M-steps ignore the weights
     // gmm_vb_em: block partials of the responsibility entropy (resp_entropy_kernel), allocated on first use
-    double* d_ent = nullptr;     // [ent_blocks + 1]: the partials, then the rank's sum for the all-reduce
-    double* h_ent = nullptr;     // pinned mirror
+    DeviceArray<double> d_ent;   // [ent_blocks + 1]: the partials, then the rank's sum for the all-reduce
+    PinnedArray<double> h_ent;
     int ent_blocks = 0;
     PhaseTimer t_entropy;
     double vb_final_ms = 0, vb_wall_ms = 0;   // gmm_get_vb_profile
@@ -606,7 +527,7 @@ static int estep_path_of(const gmm_ctx* c) { return c->estep_path >= 0 ? c->este
 static int mstep_path_of(const gmm_ctx* c) { return c->mstep_path >= 0 ? c->mstep_path : c->path; }
 static bool use_tensor_estep(const gmm_ctx* c, int K) { return estep_path_of(c) != GMM_PATH_SIMT && c->n > 0 && tc_estep_supported(c->D, K); }
 // Weights of the shard for the E- and M-step kernels (NULL: unit weights; seeding ignores them).
-static const float* step_weights(const gmm_ctx* c) { return c->weighted && !c->seeding ? c->d_w : nullptr; }
+static const float* step_weights(const gmm_ctx* c) { return c->weighted && !c->seeding ? c->d_w.get() : nullptr; }
 // Largest dynamic range max w / min positive w of the weights that the tensor M-step serves.  A weight whose scaled value
 // is not 1 moves a whole group of confident events off the points the operand's fixed-point part holds exactly, and their
 // common FP16 rounding then biases the statistics: the CPU emulation (tests/test_weights_error_model.py, DESIGN §5.11)
@@ -617,7 +538,7 @@ static const float* step_weights(const gmm_ctx* c) { return c->weighted && !c->s
 constexpr double kWeightRangeTc = 1.0;
 // (the tensor M-step also needs the data range to fit its fixed-point operand budget: known once the moments are)
 static bool use_tensor_mstep(const gmm_ctx* c, int K) {
-    return mstep_path_of(c) != GMM_PATH_SIMT && c->n > 0 && tc_mstep_supported(c->D, K) && (!c->have_shift || tc_mstep_ready(c->tc));
+    return mstep_path_of(c) != GMM_PATH_SIMT && c->n > 0 && tc_mstep_supported(c->D, K) && (!c->have_shift || tc_mstep_ready(c->tc.get()));
 }
 // N of the default epsilon and of the Rissanen score: the number of events, or the sum of the weights
 static double em_count(const gmm_ctx* c) { return c->weighted ? c->w_total : (double)c->n_global; }
@@ -625,7 +546,7 @@ static double em_count(const gmm_ctx* c) { return c->weighted ? c->w_total : (do
 static int check_path(const gmm_ctx* c, int K) {
     if (mstep_path_of(c) == GMM_PATH_TENSOR && !tc_mstep_supported(c->D, K))
         return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the wgmma kernels do not cover this (D, K)");
-    if (mstep_path_of(c) == GMM_PATH_TENSOR && c->n > 0 && c->have_shift && !tc_mstep_ready(c->tc))
+    if (mstep_path_of(c) == GMM_PATH_TENSOR && c->n > 0 && c->have_shift && !tc_mstep_ready(c->tc.get()))
         return fail(GMM_ERR_ARG, "GMM_PATH_TENSOR requested but the data range (outliers beyond 64 standard deviations) exceeds the "
                                  "tensor M-step's fixed-point operand budget");
     return GMM_OK;
@@ -638,9 +559,9 @@ static size_t stats_capacity(const gmm_ctx* c) { return std::max((size_t)c->Kmax
 
 // The worker team of the host finalisation, created on first use and resized to the context's host_threads.
 static HostPool* host_pool(gmm_ctx* c) {
-    if (!c->pool) c->pool = new HostPool(c->host_threads);
+    if (!c->pool) c->pool.reset(new HostPool(c->host_threads));
     else c->pool->resize(c->host_threads);
-    return c->pool;
+    return c->pool.get();
 }
 
 // fn(i) for i in [0, n), the items of a loop over K clusters: on the worker team when K >= 8, serially below.
@@ -664,23 +585,23 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
     if (use_tensor_estep(c, K)) {
         if (int rc = ensure_moments(c)) return rc;
         // events further than 2^14 global standard deviations from the centre would overflow the FP16 event operand
-        int rc = tc_estep_range_ok(c->tc) ? tc_params_begin(c->tc, K, c->stream)
+        int rc = tc_estep_range_ok(c->tc.get()) ? tc_params_begin(c->tc.get(), K, c->stream)
                                           : fail(GMM_ERR_STATE, "tensor E-step: the data range exceeds the FP16 event operand");
         if (rc == GMM_OK) {
             if (with_finalize)                     // pi needs every N[k] = (float)S0 before the per-cluster loop
                 for (int k = 0; k < K; k++) c->host.N[k] = (float)c->h_stats[(size_t)k * c->F];
             if (with_constants) mixing_weights(K, &c->host);
-            const int kp = tc_params_padded(c->tc, K), D = c->D;
+            const int kp = tc_params_padded(c->tc.get(), K), D = c->D;
             std::atomic<int> bad_all{0};
             const std::function<void(int)> per_cluster = [&](int k) {
                 if (with_finalize && k < K) finalize_cluster(c->h_stats, c->shift, k, D, &c->host);
                 int b;
                 double W[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS];
                 if (with_constants && k < K && constants_cluster_spd(k, D, &c->host, W)) {
-                    b = tc_params_cluster_w(c->tc, &c->host, k, K, W);      // one factorisation serves Rinv, ln det and the operand
+                    b = tc_params_cluster_w(c->tc.get(), &c->host, k, K, W);      // one factorisation serves Rinv, ln det and the operand
                 } else {
                     if (with_constants && k < K) constants_cluster(k, D, &c->host);
-                    b = tc_params_cluster(c->tc, &c->host, k, K);
+                    b = tc_params_cluster(c->tc.get(), &c->host, k, K);
                 }
                 int cur = bad_all.load(std::memory_order_relaxed);
                 while (b > cur && !bad_all.compare_exchange_weak(cur, b)) {}
@@ -688,7 +609,7 @@ static int upload_params(gmm_ctx* c, int K, bool with_constants = false, bool wi
             run_clusters(c, K, kp, per_cluster);
             const int bad = bad_all.load();
             with_constants = with_finalize = false;
-            rc = tc_params_commit(c->tc, K, bad, c->stream);
+            rc = tc_params_commit(c->tc.get(), K, bad, c->stream);
         }
         if (rc == GMM_OK) c->estep_tensor_ready = true;
         else if (rc != GMM_ERR_STATE || estep_path_of(c) == GMM_PATH_TENSOR) return rc;
@@ -831,7 +752,7 @@ static int zero_stats(gmm_ctx* c, int K) {
 // log-likelihood added to stats[K*F].
 static int run_estep(gmm_ctx* c, int K) {
     timer_begin(c, c->t_estep);
-    int rc = c->estep_tensor_ready ? tc_launch_estep(c->tc, K, c->d_stats + (size_t)K * c->F, c->stream, step_weights(c))
+    int rc = c->estep_tensor_ready ? tc_launch_estep(c->tc.get(), K, c->d_stats + (size_t)K * c->F, c->stream, step_weights(c))
                                    : launch_estep_simt(c, K);
     timer_end(c, c->t_estep);
     c->memb_valid = (rc == GMM_OK);
@@ -851,7 +772,7 @@ static int run_mstep_accumulate(gmm_ctx* c, int K) {
     timer_begin(c, c->t_mstep);
     int rc;
     if (use_tensor_mstep(c, K) && (!w || c->w_tensor_ok)) {
-        rc = tc_launch_mstep(c->tc, K, c->d_stats, c->stream, w, w ? c->w_scale : 1.0);
+        rc = tc_launch_mstep(c->tc.get(), K, c->d_stats, c->stream, w, w ? c->w_scale : 1.0);
         c->mstep_tensor++;
     }
     else { rc = launch_mstep_simt(c, K); c->mstep_simt++; }
@@ -931,7 +852,7 @@ static int ensure_moments(gmm_ctx* c) {
         c->shift[d] = mean;
         c->scale[d] = var > 0 ? std::sqrt(var) : 1.0;
     }
-    if (int rc = tc_set_shift_scale(c->tc, c->shift, c->scale, xmin, xmax, c->stream)) return rc;   // rounds shift to float in place
+    if (int rc = tc_set_shift_scale(c->tc.get(), c->shift, c->scale, xmin, xmax, c->stream)) return rc;   // rounds shift to float in place
     CUDA_TRY(cudaMemcpyAsync(c->d_shift, c->shift, sizeof(double) * D, cudaMemcpyHostToDevice, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
     c->have_shift = true;
@@ -1016,7 +937,9 @@ int gmm_create(gmm_ctx** out, int device, int n_local, int D, int Kmax, const fl
     if (prop.major != 9 || prop.minor != 0)
         return fail(GMM_ERR_CUDA, std::string("device '") + prop.name + "' is not sm_90 (H100); kernels are built for sm_90a only");
 
-    gmm_ctx* c = new gmm_ctx();
+    // a failed step returns: gmm_destroy drains the stream, and the owners free whatever was made
+    std::unique_ptr<gmm_ctx, void (*)(gmm_ctx*)> own(new gmm_ctx(), gmm_destroy);
+    gmm_ctx* c = own.get();
     c->device = device; c->n = n_local; c->D = D; c->Kmax = Kmax; c->F = num_features(D);
     c->n_global = n_global; c->offset = offset; c->num_sms = prop.multiProcessorCount;
     const char* ht = getenv("GMM_HOST_THREADS");
@@ -1026,55 +949,48 @@ int gmm_create(gmm_ctx** out, int device, int n_local, int D, int Kmax, const fl
     c->hN.assign(Kmax, 0); c->hpi.assign(Kmax, 0); c->hconst.assign(Kmax, 0); c->havgvar.assign(Kmax, 0);
     c->hmeans.assign((size_t)Kmax * D, 0); c->hR.assign((size_t)Kmax * D * D, 0); c->hRinv.assign((size_t)Kmax * D * D, 0);
     bind_host(c);
-#define CREATE_TRY(expr)                                                                             \
-    do {                                                                                             \
-        cudaError_t e_ = (expr);                                                                     \
-        if (e_ != cudaSuccess) {                                                                     \
-            int rc_ = fail(GMM_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));        \
-            gmm_destroy(c);                                                                          \
-            return rc_;                                                                              \
-        }                                                                                            \
-    } while (0)
-    CREATE_TRY(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
-    CREATE_TRY(cudaEventCreateWithFlags(&c->ev_stats, cudaEventDisableTiming));
+    if (int rc = c->stream.create(cudaStreamNonBlocking)) return rc;
+    if (int rc = c->ev_stats.create(cudaEventDisableTiming)) return rc;
     const size_t nmax = n_local > 0 ? (size_t)n_local : 1;
-    CREATE_TRY(cudaMalloc(&c->d_x_aos, sizeof(float) * nmax * D));
+    if (int rc = c->d_x_aos.reserve(nmax * D)) return rc;
     c->memb_pitch = (nmax + 31) / 32 * 32;         // also the row pitch of the SoA event copy
-    CREATE_TRY(cudaMalloc(&c->d_x_soa, sizeof(float) * c->memb_pitch * D));
+    if (int rc = c->d_x_soa.reserve(c->memb_pitch * D)) return rc;
     // rows in multiples of 8: the tensor E-step stores whole 8-cluster groups (zeros for the padding clusters)
-    CREATE_TRY(cudaMalloc(&c->d_memb, sizeof(float) * c->memb_pitch * (size_t)((Kmax + 7) / 8 * 8)));
-    CREATE_TRY(cudaMalloc(&c->d_epack, sizeof(float) * (size_t)Kmax * epack_stride(D)));
-    CREATE_TRY(cudaMallocHost(&c->h_epack, sizeof(float) * (size_t)Kmax * epack_stride(D)));
-    CREATE_TRY(cudaMalloc(&c->d_stats, sizeof(double) * stats_capacity(c)));
-    CREATE_TRY(cudaMemsetAsync(c->d_stats, 0, sizeof(double) * ((size_t)Kmax * c->F + 1), c->stream));
-    CREATE_TRY(cudaMallocHost(&c->h_stats, sizeof(double) * stats_capacity(c)));
-    CREATE_TRY(cudaMalloc(&c->d_shift, sizeof(double) * GMM_MAX_DIMENSIONS));
-    CREATE_TRY(cudaMemsetAsync(c->d_shift, 0, sizeof(double) * GMM_MAX_DIMENSIONS, c->stream));
+    if (int rc = c->d_memb.reserve(c->memb_pitch * (size_t)((Kmax + 7) / 8 * 8))) return rc;
+    if (int rc = c->d_epack.reserve((size_t)Kmax * epack_stride(D))) return rc;
+    if (int rc = c->h_epack.reserve((size_t)Kmax * epack_stride(D))) return rc;
+    if (int rc = c->d_stats.reserve(stats_capacity(c))) return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_stats, 0, sizeof(double) * ((size_t)Kmax * c->F + 1), c->stream));
+    if (int rc = c->h_stats.reserve(stats_capacity(c))) return rc;
+    if (int rc = c->d_shift.reserve(GMM_MAX_DIMENSIONS)) return rc;
+    CUDA_TRY(cudaMemsetAsync(c->d_shift, 0, sizeof(double) * GMM_MAX_DIMENSIONS, c->stream));
     if (n_local > 0 && events_aos) {
-        CREATE_TRY(cudaMemcpyAsync(c->d_x_aos, events_aos, sizeof(float) * (size_t)n_local * D, cudaMemcpyHostToDevice, c->stream));
+        CUDA_TRY(cudaMemcpyAsync(c->d_x_aos, events_aos, sizeof(float) * (size_t)n_local * D, cudaMemcpyHostToDevice, c->stream));
         dim3 blk(32, 8);
         transpose_aos_to_soa_kernel<<<(n_local + 31) / 32, blk, 0, c->stream>>>(c->d_x_aos, c->d_x_soa, c->memb_pitch, n_local, D);
-        CREATE_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
     }
     {
-        int rc = tc_create(&c->tc, c->d_x_aos, c->d_x_soa, n_local, D, Kmax, c->d_memb, c->memb_pitch, c->num_sms, c->stream);
-        if (rc) { gmm_destroy(c); return rc; }
-        tc_set_host_threads(c->tc, c->host_threads);
+        TcState* tc = nullptr;
+        const int rc = tc_create(&tc, c->d_x_aos, c->d_x_soa, n_local, D, Kmax, c->d_memb, c->memb_pitch, c->num_sms, c->stream);
+        c->tc.reset(tc);
+        if (rc) return rc;
+        tc_set_host_threads(c->tc.get(), c->host_threads);
     }
     if (const char* fm = getenv("GMM_FINALIZE")) c->finalize_mode = (std::string(fm) == "host") ? 0 : 1;
     if (n_local > 0 && tc_estep_supported(D, Kmax)) {
         const size_t setf = tc_param_set_floats(Kmax, D);
-        for (int b = 0; b < 2; b++) CREATE_TRY(cudaMalloc(&c->d_pset[b], sizeof(float) * setf));
-        CREATE_TRY(cudaMallocHost(&c->h_pset, sizeof(float) * setf));
-        CREATE_TRY(cudaMalloc(&c->d_avgvar, sizeof(float) * (size_t)Kmax));
-        CREATE_TRY(cudaMemsetAsync(c->d_avgvar, 0, sizeof(float) * (size_t)Kmax, c->stream));
-        CREATE_TRY(cudaMalloc(&c->d_bad, 2 * sizeof(int)));
-        CREATE_TRY(cudaMalloc(&c->d_llprev, 2 * sizeof(double)));
-        CREATE_TRY(cudaMallocHost(&c->h_small, 32 + sizeof(float) * (size_t)Kmax));
+        for (int b = 0; b < 2; b++)
+            if (int rc = c->d_pset[b].reserve(setf)) return rc;
+        if (int rc = c->h_pset.reserve(setf)) return rc;
+        if (int rc = c->d_avgvar.reserve(Kmax)) return rc;
+        CUDA_TRY(cudaMemsetAsync(c->d_avgvar, 0, sizeof(float) * (size_t)Kmax, c->stream));
+        if (int rc = c->d_bad.reserve(2)) return rc;
+        if (int rc = c->d_llprev.reserve(2)) return rc;
+        if (int rc = c->h_small.reserve(32 + sizeof(float) * (size_t)Kmax)) return rc;
     }
-    CREATE_TRY(cudaStreamSynchronize(c->stream));
-#undef CREATE_TRY
-    *out = c;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    *out = own.release();
     return GMM_OK;
 }
 
@@ -1115,11 +1031,11 @@ int gmm_upload_events_file(gmm_ctx* c, const char* path) {
     const size_t row = sizeof(float) * (size_t)c->D;
     const size_t total = row * (size_t)c->n;
     const size_t chunk = std::max<size_t>(row, ((size_t)32 << 20) / row * row);
-    char* stage[2] = {nullptr, nullptr};
-    cudaEvent_t done[2] = {nullptr, nullptr};
+    PinnedArray<char> stage[2];
+    Event done[2];
     int rc = GMM_OK;
     for (int b = 0; b < 2 && rc == GMM_OK; b++) {
-        if (cudaMallocHost(&stage[b], chunk) != cudaSuccess || cudaEventCreateWithFlags(&done[b], cudaEventDisableTiming) != cudaSuccess)
+        if (stage[b].reserve(chunk) != GMM_OK || done[b].create(cudaEventDisableTiming) != GMM_OK)
             rc = fail(GMM_ERR_CUDA, "gmm_upload_events_file: pinned staging allocation failed");
     }
     size_t off = 0;
@@ -1134,7 +1050,7 @@ int gmm_upload_events_file(gmm_ctx* c, const char* path) {
             got += (size_t)r;
         }
         if (rc != GMM_OK) break;
-        if (cudaMemcpyAsync(reinterpret_cast<char*>(c->d_x_aos) + off, stage[b], len, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+        if (cudaMemcpyAsync(reinterpret_cast<char*>(c->d_x_aos.get()) + off, stage[b], len, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
             cudaEventRecord(done[b], c->stream) != cudaSuccess) { rc = fail(GMM_ERR_CUDA, "gmm_upload_events_file: copy failed"); break; }
         off += len;
     }
@@ -1145,10 +1061,6 @@ int gmm_upload_events_file(gmm_ctx* c, const char* path) {
         if (cudaGetLastError() != cudaSuccess) rc = fail(GMM_ERR_CUDA, "transpose launch failed");
     }
     if (cudaStreamSynchronize(c->stream) != cudaSuccess && rc == GMM_OK) rc = fail(GMM_ERR_CUDA, "gmm_upload_events_file: copy failed");
-    for (int b = 0; b < 2; b++) {
-        if (stage[b]) cudaFreeHost(stage[b]);
-        if (done[b]) cudaEventDestroy(done[b]);
-    }
     c->have_shift = false;
     c->memb_valid = false;
     c->estep_tensor_ready = false;
@@ -1163,27 +1075,6 @@ void gmm_destroy(gmm_ctx* c) {
     collect_all(c);
     peer_exchange_destroy(c);
     if (c->comm && nccl().ok) nccl().CommDestroy(c->comm);
-    tc_destroy(c->tc);
-    c->score.destroy();
-    c->sstats.destroy();
-    c->kmeans.destroy();
-    c->sample.destroy();
-    c->cond.destroy();
-    c->comb.destroy();
-    delete c->pool;
-    cudaFree(c->d_x_aos); cudaFree(c->d_x_soa); cudaFree(c->d_memb); cudaFree(c->d_memb_saved);
-    cudaFree(c->d_epack); cudaFree(c->d_stats); cudaFree(c->d_shift);
-    cudaFree(c->d_pset[0]); cudaFree(c->d_pset[1]); cudaFree(c->d_avgvar); cudaFree(c->d_bad); cudaFree(c->d_llprev);
-    cudaFree(c->d_w);
-    cudaFree(c->d_ent);
-    if (c->h_ent) cudaFreeHost(c->h_ent);
-    if (c->h_pset) cudaFreeHost(c->h_pset);
-    if (c->h_small) cudaFreeHost(c->h_small);
-    if (c->h_epack) cudaFreeHost(c->h_epack);
-    if (c->h_stats) cudaFreeHost(c->h_stats);
-    if (c->ev_stats) cudaEventDestroy(c->ev_stats);
-    c->events.destroy();
-    if (c->stream) cudaStreamDestroy(c->stream);
     delete c;
 }
 
@@ -1202,24 +1093,23 @@ static int peer_exchange_setup(gmm_ctx* c) {
     me.device = c->device;
     me.ok = (G <= kXMaxRanks && getenv("GMM_NO_PEER_ALLREDUCE") == nullptr) ? 1 : 0;
     me.dev_fin = c->d_pset[0] ? 1 : 0;
-    if (me.ok && cudaMalloc(&x.base, bytes) != cudaSuccess) { x.base = nullptr; me.ok = 0; cudaGetLastError(); }
+    if (me.ok && x.base.reserve(bytes) != GMM_OK) me.ok = 0;
     if (me.ok) {
         cudaMemset(x.base, 0, bytes);
-        me.ptr = (unsigned long long)(uintptr_t)x.base;
+        me.ptr = (unsigned long long)(uintptr_t)x.base.get();
         if (cudaIpcGetMemHandle(&me.handle, x.base) != cudaSuccess) { me.ok = 0; cudaGetLastError(); }
     }
     // gather the hellos (device staging; NCCL is the only channel the C ABI has between ranks)
-    PeerHello* d_all = nullptr;
+    DeviceArray<PeerHello> d_all;
     std::vector<PeerHello> all((size_t)G);
-    CUDA_TRY(cudaMalloc(&d_all, sizeof(PeerHello) * G));
+    if (int rc = d_all.reserve(G)) return rc;
     CUDA_TRY(cudaMemcpyAsync(d_all + c->rank, &me, sizeof(PeerHello), cudaMemcpyHostToDevice, c->stream));
     {
         ncclResult_t r = nccl().AllGather(d_all + c->rank, d_all, sizeof(PeerHello), ncclChar, c->comm, c->stream);
-        if (r != ncclSuccess) { cudaFree(d_all); return fail(GMM_ERR_NCCL, std::string("ncclAllGather: ") + nccl().GetErrorString(r)); }
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllGather: ") + nccl().GetErrorString(r));
     }
     CUDA_TRY(cudaMemcpyAsync(all.data(), d_all, sizeof(PeerHello) * G, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
-    cudaFree(d_all);
     int ok = 1;
     for (int p = 0; p < G; p++) ok &= all[p].ok;
     c->dev_fin_agreed = true;
@@ -1248,15 +1138,14 @@ static int peer_exchange_setup(gmm_ctx* c) {
     }
     // a rank that failed to map somebody must take everybody back to NCCL: agree on the minimum
     {
-        double* d_ok = nullptr;
+        DeviceArray<double> d_ok;
         double h_ok = ok ? 1.0 : 0.0;
-        CUDA_TRY(cudaMalloc(&d_ok, sizeof(double)));
+        if (int rc = d_ok.reserve(1)) return rc;
         CUDA_TRY(cudaMemcpyAsync(d_ok, &h_ok, sizeof(double), cudaMemcpyHostToDevice, c->stream));
         ncclResult_t r = nccl().AllReduce(d_ok, d_ok, 1, ncclDouble, ncclMin, c->comm, c->stream);
-        if (r != ncclSuccess) { cudaFree(d_ok); return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r)); }
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
         CUDA_TRY(cudaMemcpyAsync(&h_ok, d_ok, sizeof(double), cudaMemcpyDeviceToHost, c->stream));
         CUDA_TRY(cudaStreamSynchronize(c->stream));
-        cudaFree(d_ok);
         ok = h_ok > 0.5;
     }
     x.ok = ok != 0;
@@ -1268,7 +1157,7 @@ static void peer_exchange_destroy(gmm_ctx* c) {
     PeerExchange& x = c->xchg;
     for (int p = 0; p < kXMaxRanks; p++)
         if (x.opened[p]) { cudaIpcCloseMemHandle(x.opened[p]); x.opened[p] = nullptr; }
-    if (x.base) { cudaFree(x.base); x.base = nullptr; }
+    x.base.reset();
     x.ok = false;
 }
 
@@ -1287,7 +1176,7 @@ int gmm_comm_init(gmm_ctx* c, int nranks, int rank, const char id_in[128]) {
     c->rank = rank; c->nranks = nranks;
     if (!c->host_threads_fixed) {                   // the ranks of one box share its cores
         c->host_threads = default_host_threads(nranks);
-        tc_set_host_threads(c->tc, c->host_threads);
+        tc_set_host_threads(c->tc.get(), c->host_threads);
     }
     if (nranks == 1) return GMM_OK;
     if (!id_in) return fail(GMM_ERR_ARG, "gmm_comm_init: null id");
@@ -1317,7 +1206,7 @@ int gmm_set_option(gmm_ctx* c, const char* key, double value) {
     else if (k == "host_threads") {
         c->host_threads = value < 1 ? 1 : (int)value;
         c->host_threads_fixed = true;
-        tc_set_host_threads(c->tc, c->host_threads);
+        tc_set_host_threads(c->tc.get(), c->host_threads);
     }
     else if (k == "estep_path" || k == "mstep_path") {
         const int p = (int)value;
@@ -1404,8 +1293,8 @@ int gmm_set_weights(gmm_ctx* c, const float* weights, double* total_out) {
     }
     if (c->nranks > 1) {
         double h[5] = {sum, bad, has, wmax, -wmin};   // summed | maximised
-        double* d_h = nullptr;
-        CUDA_TRY(cudaMalloc(&d_h, sizeof(h)));
+        DeviceArray<double> d_h;
+        if (int rc = d_h.reserve(5)) return rc;
         ncclResult_t r = ncclSuccess;
         cudaError_t e = cudaMemcpyAsync(d_h, h, sizeof(h), cudaMemcpyHostToDevice, c->stream);
         if (e == cudaSuccess) {
@@ -1414,7 +1303,6 @@ int gmm_set_weights(gmm_ctx* c, const float* weights, double* total_out) {
             if (r == ncclSuccess) e = cudaMemcpyAsync(h, d_h, sizeof(h), cudaMemcpyDeviceToHost, c->stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         }
-        cudaFree(d_h);
         if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
         if (e != cudaSuccess) return fail(GMM_ERR_CUDA, std::string("gmm_set_weights: ") + cudaGetErrorString(e));
         sum = h[0]; bad = h[1]; has = h[2]; wmax = h[3]; wmin = -h[4];
@@ -1429,8 +1317,8 @@ int gmm_set_weights(gmm_ctx* c, const float* weights, double* total_out) {
     }
     if (bad != 0.0) return fail(GMM_ERR_ARG, "gmm_set_weights: a weight is negative or not finite");
     if (!(sum > 0.0)) return fail(GMM_ERR_ARG, "gmm_set_weights: the weights sum to zero");
-    if (!c->d_w) {
-        CUDA_TRY(cudaMalloc(&c->d_w, sizeof(float) * c->memb_pitch));
+    if (c->d_w.size() < c->memb_pitch) {
+        if (int rc = c->d_w.reserve(c->memb_pitch)) return rc;
         CUDA_TRY(cudaMemsetAsync(c->d_w, 0, sizeof(float) * c->memb_pitch, c->stream));   // the M-step reads whole 32-event tiles
     }
     if (c->n > 0) CUDA_TRY(cudaMemcpyAsync(c->d_w, weights, sizeof(float) * (size_t)c->n, cudaMemcpyHostToDevice, c->stream));
@@ -1524,7 +1412,7 @@ static int em_iteration(gmm_ctx* c, int K, float* prev_loglik) {
 // ---- EM iterations with the finalisation on the device --------------------------------------------------------
 static bool dev_finalize_ok(const gmm_ctx* c, int K) {
     return c->finalize_mode == 1 && !c->dev_fin_failed && c->dev_fin_agreed && c->d_pset[0] && c->n > 0 && c->estep_tensor_ready && K == c->cur_K &&
-           use_tensor_estep(c, K) && tc_finalize_supported(c->tc, K);
+           use_tensor_estep(c, K) && tc_finalize_supported(c->tc.get(), K);
 }
 
 // Parameter set `which` (K-prefixes of its arrays) -> pinned staging; valid after the next stream synchronisation.
@@ -1554,7 +1442,7 @@ static int em_iteration(gmm_ctx* c, int K, float* prev_loglik);
 // iteration started from and runs the remaining iterations through its own path; the context then stays on the host path.
 static int run_dev_iterations(gmm_ctx* c, int K, int iters, float* ll_prev) {
     if (iters <= 0) return GMM_OK;
-    int* h_bad = reinterpret_cast<int*>(c->h_small);
+    int* h_bad = reinterpret_cast<int*>(c->h_small.get());
     double* h_ll = reinterpret_cast<double*>(c->h_small + 16);
     h_bad[0] = -1; h_bad[1] = 0;
     CUDA_TRY(cudaMemcpyAsync(c->d_bad, h_bad, 2 * sizeof(int), cudaMemcpyHostToDevice, c->stream));
@@ -1562,7 +1450,7 @@ static int run_dev_iterations(gmm_ctx* c, int K, int iters, float* ll_prev) {
         if (int rc = run_mstep_accumulate(c, K)) return rc;
         if (int rc = reduce_stats_device(c, K)) return rc;
         timer_begin(c, c->t_final);
-        int rc = tc_launch_finalize(c->tc, K, c->d_stats, c->d_avgvar, c->d_pset[i & 1], c->d_llprev + (i & 1), c->d_bad, i, c->fin_fault_iter, c->stream);
+        int rc = tc_launch_finalize(c->tc.get(), K, c->d_stats, c->d_avgvar, c->d_pset[i & 1], c->d_llprev + (i & 1), c->d_bad, i, c->fin_fault_iter, c->stream);
         timer_end(c, c->t_final);
         if (rc) return rc;
         c->dev_finalize_launches++;
@@ -1689,27 +1577,24 @@ int gmm_em(gmm_ctx* c, int K, int min_iters, int max_iters, float epsilon, float
 // Buffers for chunks of c->score_chunk events: allocated on first use, grown (never shrunk) when the option grows.
 static int score_buffers(gmm_ctx* c) {
     ScoreBuffers& s = c->score;
-    if (!s.copy) {
-        CUDA_TRY(cudaStreamCreateWithFlags(&s.copy, cudaStreamNonBlocking));
-        for (int b = 0; b < 2; b++) {
-            for (cudaEvent_t* e : {&s.h2d[b], &s.kern[b], &s.d2h[b]}) CUDA_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-            CUDA_TRY(cudaEventCreate(&s.t0[b]));
-            CUDA_TRY(cudaEventCreate(&s.t1[b]));
-        }
-    }
-    const long long want = c->score_chunk;
-    if (s.cap >= want) return GMM_OK;
-    s.release();
+    if (int rc = s.copy.create(cudaStreamNonBlocking)) return rc;
     for (int b = 0; b < 2; b++) {
-        CUDA_TRY(cudaMallocHost(&s.h_in[b], sizeof(float) * (size_t)want * c->D));
-        CUDA_TRY(cudaMalloc(&s.d_in[b], sizeof(float) * (size_t)want * c->D));
-        CUDA_TRY(cudaMalloc(&s.d_out[b], ScoreBuffers::out_bytes(want)));
-        CUDA_TRY(cudaMallocHost(&s.h_out[b], ScoreBuffers::out_bytes(want)));
+        for (Event* e : {&s.h2d[b], &s.kern[b], &s.d2h[b]})
+            if (int rc = e->create(cudaEventDisableTiming)) return rc;
+        for (Event* e : {&s.t0[b], &s.t1[b]})
+            if (int rc = e->create(cudaEventDefault)) return rc;
+    }
+    const long long want = std::max(s.cap, c->score_chunk);
+    for (int b = 0; b < 2; b++) {
+        if (int rc = s.h_in[b].reserve((size_t)want * c->D)) return rc;
+        if (int rc = s.d_in[b].reserve((size_t)want * c->D)) return rc;
+        if (int rc = s.d_out[b].reserve(ScoreBuffers::out_bytes(want))) return rc;
+        if (int rc = s.h_out[b].reserve(ScoreBuffers::out_bytes(want))) return rc;
     }
     if (c->Kmax > 64) {
-        CUDA_TRY(cudaMalloc(&s.d_run_den, sizeof(float) * (size_t)want));
-        CUDA_TRY(cudaMalloc(&s.d_run_bl, sizeof(float) * (size_t)want));
-        CUDA_TRY(cudaMalloc(&s.d_run_bk, sizeof(int) * (size_t)want));
+        if (int rc = s.d_run_den.reserve(want)) return rc;
+        if (int rc = s.d_run_bl.reserve(want)) return rc;
+        if (int rc = s.d_run_bk.reserve(want)) return rc;
     }
     s.cap = want;
     return GMM_OK;
@@ -1835,7 +1720,7 @@ static int score_batch(gmm_ctx* c, int K, const float* ev, long long n, const Sc
         if (!on_tensor)
             if (int rc = ensure_epack(c, K, &epack_ready)) return rc;
         CUDA_TRY(cudaEventRecord(s.t0[b], c->stream));
-        int rc = on_tensor ? tc_launch_score(c->tc, K, io, c->stream) : launch_score_simt(c, D, K, c->d_epack, io);
+        int rc = on_tensor ? tc_launch_score(c->tc.get(), K, io, c->stream) : launch_score_simt(c, D, K, c->d_epack, io);
         if (rc) return rc;
         CUDA_TRY(cudaEventRecord(s.t1[b], c->stream));
         (on_tensor ? s.tensor_chunks : s.simt_chunks)++;
@@ -1890,31 +1775,31 @@ int gmm_get_score_profile(gmm_ctx* c, double out[4], int reset) {
 // ---- E-step + M-step statistics of new events ---------------------------------------------------------------------------
 static int score_stats_buffers(gmm_ctx* c, bool with_memberships, bool with_observed = false) {
     ScoreStatsBuffers& t = c->sstats;
-    if (!t.ev_flag) {
-        CUDA_TRY(cudaEventCreateWithFlags(&t.ev_flag, cudaEventDisableTiming));
-        for (int b = 0; b < 2; b++)
-            for (cudaEvent_t* e : {&t.p0[b], &t.p1[b], &t.k0[b], &t.k1[b]}) CUDA_TRY(cudaEventCreate(e));
-        CUDA_TRY(cudaMalloc(&t.d_stats, sizeof(double) * ((size_t)c->Kmax * c->F + 1)));
-        CUDA_TRY(cudaMallocHost(&t.h_stats, sizeof(double) * ((size_t)c->Kmax * c->F + 1)));
-        CUDA_TRY(cudaMalloc(&t.d_flag, sizeof(int)));
-        CUDA_TRY(cudaMallocHost(&t.h_flag, sizeof(int)));
-        CUDA_TRY(cudaMalloc(&t.d_shift_f, sizeof(float) * GMM_MAX_DIMENSIONS));
-    }
-    const long long want = c->score_chunk;
-    if (t.cap < want) {
-        t.release_chunk();
-        const size_t pitch = ((size_t)want + 31) / 32 * 32, rows = (size_t)(c->Kmax + 7) / 8 * 8;
-        CUDA_TRY(cudaMalloc(&t.d_z, sizeof(float) * pitch * c->D));
-        CUDA_TRY(cudaMalloc(&t.d_xs, sizeof(float) * pitch * c->D));
-        CUDA_TRY(cudaMalloc(&t.d_memb, sizeof(float) * pitch * rows));
+    if (int rc = t.ev_flag.create(cudaEventDisableTiming)) return rc;
+    for (int b = 0; b < 2; b++)
+        for (Event* e : {&t.p0[b], &t.p1[b], &t.k0[b], &t.k1[b]})
+            if (int rc = e->create(cudaEventDefault)) return rc;
+    if (int rc = t.d_stats.reserve((size_t)c->Kmax * c->F + 1)) return rc;
+    if (int rc = t.h_stats.reserve((size_t)c->Kmax * c->F + 1)) return rc;
+    if (int rc = t.d_flag.reserve(1)) return rc;
+    if (int rc = t.h_flag.reserve(1)) return rc;
+    if (int rc = t.d_shift_f.reserve(GMM_MAX_DIMENSIONS)) return rc;
+    const long long want = std::max(t.cap, c->score_chunk);
+    const size_t pitch = ((size_t)want + 31) / 32 * 32, rows = (size_t)(c->Kmax + 7) / 8 * 8;
+    if (int rc = t.d_z.reserve(pitch * c->D)) return rc;
+    if (int rc = t.d_xs.reserve(pitch * c->D)) return rc;
+    if (t.d_memb.size() < pitch * rows) {
+        if (int rc = t.d_memb.reserve(pitch * rows)) return rc;
         // rows above K that no E-step of this call writes are read by the tensor M-step's 32-cluster boxes (their columns
         // are discarded): keep them finite
         CUDA_TRY(cudaMemsetAsync(t.d_memb, 0, sizeof(float) * pitch * rows, c->stream));
-        t.cap = want;
-        t.pitch = pitch;
     }
-    if (with_memberships && !t.h_memb) CUDA_TRY(cudaMallocHost(&t.h_memb, sizeof(float) * (size_t)c->Kmax * t.cap));
-    if (with_observed && !t.d_xo) CUDA_TRY(cudaMalloc(&t.d_xo, sizeof(float) * t.pitch * c->D));
+    t.cap = want;
+    t.pitch = pitch;
+    if (with_memberships)
+        if (int rc = t.h_memb.reserve((size_t)c->Kmax * t.cap)) return rc;
+    if (with_observed)
+        if (int rc = t.d_xo.reserve(t.pitch * c->D)) return rc;
     return GMM_OK;
 }
 
@@ -1976,7 +1861,7 @@ static int stats_batch(gmm_ctx* c, int K, const float* ev, int width, long long 
         (ce ? pr.e_tensor : pr.e_simt)++;
         CUDA_TRY(cudaEventRecord(s.kern[b], c->stream));          // the device input chunk is free again
         if (with_stats) {
-            rc = cm ? tc_launch_mstep_on(c->tc, K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
+            rc = cm ? tc_launch_mstep_on(c->tc.get(), K, t.d_z, t.d_memb, t.pitch, m, t.d_stats, c->stream)
                     : launch_mstep_simt_on(c, K, t.d_xs, m, t.d_memb, t.pitch, t.d_stats);
             if (rc) return rc;
             (cm ? pr.m_tensor : pr.m_simt)++;
@@ -2007,13 +1892,13 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
     const bool e_tensor = c->estep_tensor_ready;
     const bool m_tensor = with_stats && use_tensor_mstep(c, K);
     const bool raw_always = !e_tensor || (with_stats && !m_tensor);   // the context's own selection puts a SIMT kernel on every chunk
-    const float* shift_f = (e_tensor || m_tensor) ? tc_shift_f(c->tc) : nullptr;
-    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
+    const float* shift_f = (e_tensor || m_tensor) ? tc_shift_f(c->tc.get()) : nullptr;
+    const float zb = m_tensor ? tc_mstep_zbound(c->tc.get()) : INFINITY;
     if ((e_tensor || m_tensor) && !shift_f) return fail(GMM_ERR_STATE, "gmm_score_stats: the tensor kernels have no centre");
     auto prep = [&](int b, int m) -> int {
         score_stats_prep_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(
-            s.d_in[b], m, D, shift_f, shift_f ? tc_inv_scale_f(c->tc) : nullptr, zb, m_tensor ? t.d_z : nullptr,
-            raw_always ? t.d_xs : nullptr, t.pitch, t.d_flag);
+            s.d_in[b], m, D, shift_f, shift_f ? tc_inv_scale_f(c->tc.get()) : nullptr, zb, m_tensor ? t.d_z.get() : nullptr,
+            raw_always ? t.d_xs.get() : nullptr, t.pitch, t.d_flag);
         CUDA_TRY(cudaGetLastError());
         return GMM_OK;
     };
@@ -2022,7 +1907,7 @@ static int score_stats_batch(gmm_ctx* c, int K, const float* ev, long long n, bo
             transpose_aos_to_soa_kernel<<<(m + 31) / 32, dim3(32, 8), 0, c->stream>>>(s.d_in[b], t.d_xs, t.pitch, m, D);
             CUDA_TRY(cudaGetLastError());
         }
-        return ce ? tc_launch_estep_on(c->tc, K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
+        return ce ? tc_launch_estep_on(c->tc.get(), K, s.d_in[b], m, t.d_memb, t.pitch, s.d_run_den, t.d_stats + KF, c->stream)
                   : launch_estep_simt_on(c, D, K, c->d_epack, t.d_xs, m, t.d_memb, t.pitch, t.d_stats + KF);
     };
     return stats_batch(c, K, ev, D, n, with_stats, memberships, e_tensor, m_tensor, pr, "gmm_score_stats", prep, estep);
@@ -2068,29 +1953,26 @@ int gmm_get_score_stats_profile(gmm_ctx* c, double out[7], int reset) {
 // ---- k-means++ and Lloyd seeding ------------------------------------------------------------------------------------------
 static int kmeans_buffers(gmm_ctx* c) {
     KmeansBuffers& b = c->kmeans;
-    if (b.ready) return GMM_OK;
-    const size_t n = (size_t)std::max(c->n, 1), D = (size_t)c->D;
+    const size_t n = (size_t)std::max(c->n, 1), D = (size_t)c->D, xfer = 16 * (size_t)c->nranks;
     b.nb = (int)((n + kSeedBlockEvents - 1) / kSeedBlockEvents);
     b.nba = (int)((n + kAssignThreads - 1) / kAssignThreads);
-    b.nxfer = 16 * c->nranks;
-    CUDA_TRY(cudaMalloc(&b.d_d2, sizeof(double) * n));
-    CUDA_TRY(cudaMalloc(&b.d_labels, sizeof(int) * n));
-    CUDA_TRY(cudaMalloc(&b.d_bsum, sizeof(double) * b.nb));
-    CUDA_TRY(cudaMalloc(&b.d_bpot, sizeof(double) * b.nb * kSeedMaxCand));
-    CUDA_TRY(cudaMalloc(&b.d_bchanged, sizeof(int) * b.nba));
-    CUDA_TRY(cudaMalloc(&b.d_binertia, sizeof(double) * b.nba));
-    CUDA_TRY(cudaMalloc(&b.d_cand, sizeof(float) * kSeedMaxCand * D));
-    CUDA_TRY(cudaMalloc(&b.d_pick, sizeof(SeedPick) * kSeedMaxCand));
-    CUDA_TRY(cudaMalloc(&b.d_pick_idx, sizeof(int) * kSeedMaxCand));
-    CUDA_TRY(cudaMalloc(&b.d_centres, sizeof(float) * (size_t)c->Kmax * D));
-    CUDA_TRY(cudaMalloc(&b.d_xfer, sizeof(double) * b.nxfer));
-    CUDA_TRY(cudaMallocHost(&b.h_bsum, sizeof(double) * b.nb));
-    CUDA_TRY(cudaMallocHost(&b.h_bpot, sizeof(double) * b.nb * kSeedMaxCand));
-    CUDA_TRY(cudaMallocHost(&b.h_bchanged, sizeof(int) * b.nba));
-    CUDA_TRY(cudaMallocHost(&b.h_binertia, sizeof(double) * b.nba));
-    CUDA_TRY(cudaMallocHost(&b.h_pick, sizeof(SeedPick) * kSeedMaxCand));
-    CUDA_TRY(cudaMallocHost(&b.h_xfer, sizeof(double) * b.nxfer));
-    b.ready = true;
+    if (int rc = b.d_d2.reserve(n)) return rc;
+    if (int rc = b.d_labels.reserve(n)) return rc;
+    if (int rc = b.d_bsum.reserve(b.nb)) return rc;
+    if (int rc = b.d_bpot.reserve((size_t)b.nb * kSeedMaxCand)) return rc;
+    if (int rc = b.d_bchanged.reserve(b.nba)) return rc;
+    if (int rc = b.d_binertia.reserve(b.nba)) return rc;
+    if (int rc = b.d_cand.reserve(kSeedMaxCand * D)) return rc;
+    if (int rc = b.d_pick.reserve(kSeedMaxCand)) return rc;
+    if (int rc = b.d_pick_idx.reserve(kSeedMaxCand)) return rc;
+    if (int rc = b.d_centres.reserve((size_t)c->Kmax * D)) return rc;
+    if (int rc = b.d_xfer.reserve(xfer)) return rc;
+    if (int rc = b.h_bsum.reserve(b.nb)) return rc;
+    if (int rc = b.h_bpot.reserve((size_t)b.nb * kSeedMaxCand)) return rc;
+    if (int rc = b.h_bchanged.reserve(b.nba)) return rc;
+    if (int rc = b.h_binertia.reserve(b.nba)) return rc;
+    if (int rc = b.h_pick.reserve(kSeedMaxCand)) return rc;
+    if (int rc = b.h_xfer.reserve(xfer)) return rc;
     return GMM_OK;
 }
 
@@ -2102,13 +1984,13 @@ static int kmeans_rank_values(gmm_ctx* c, const double* mine, int m, std::vector
     std::copy(mine, mine + m, all.begin() + (size_t)c->rank * m);
     if (c->nranks == 1) return GMM_OK;
     const size_t len = (size_t)c->nranks * m;
-    std::copy(all.begin(), all.end(), b.h_xfer);
+    std::copy(all.begin(), all.end(), b.h_xfer.get());
     CUDA_TRY(cudaMemcpyAsync(b.d_xfer, b.h_xfer, sizeof(double) * len, cudaMemcpyHostToDevice, c->stream));
     ncclResult_t r = nccl().AllReduce(b.d_xfer, b.d_xfer, len, ncclDouble, ncclSum, c->comm, c->stream);
     if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
     CUDA_TRY(cudaMemcpyAsync(b.h_xfer, b.d_xfer, sizeof(double) * len, cudaMemcpyDeviceToHost, c->stream));
     CUDA_TRY(cudaStreamSynchronize(c->stream));
-    std::copy(b.h_xfer, b.h_xfer + len, all.begin());
+    std::copy(b.h_xfer.get(), b.h_xfer + len, all.begin());
     return GMM_OK;
 }
 
@@ -2374,11 +2256,9 @@ static int vb_default_moments(gmm_ctx* c, double* mean, double* cov) {
 // resp_entropy_kernel over the current memberships, its partials queued to the pinned mirror (read after the next stream
 // synchronisation by vb_entropy_sum).  timer: the profile the kernel counts in (NULL: none).
 static int vb_entropy_launch(gmm_ctx* c, int K, int* grid_out, PhaseTimer* timer) {
-    if (!c->d_ent) {
-        c->ent_blocks = kEntropyBlocksPerSm * c->num_sms;
-        CUDA_TRY(cudaMalloc(&c->d_ent, sizeof(double) * (size_t)(c->ent_blocks + 1)));
-        CUDA_TRY(cudaMallocHost(&c->h_ent, sizeof(double) * (size_t)(c->ent_blocks + 1)));
-    }
+    c->ent_blocks = kEntropyBlocksPerSm * c->num_sms;
+    if (int rc = c->d_ent.reserve((size_t)c->ent_blocks + 1)) return rc;
+    if (int rc = c->h_ent.reserve((size_t)c->ent_blocks + 1)) return rc;
     const int nq = (c->n + 3) / 4;
     const int grid = std::max(1, std::min(c->ent_blocks, (nq + kEntropyThreads - 1) / kEntropyThreads));
     *grid_out = c->n > 0 ? grid : 0;
@@ -2514,28 +2394,13 @@ static int check_memberships(const gmm_ctx* c, int K, const char* who) {
 
 static int combine_buffers(gmm_ctx* c, size_t part, size_t sum) {
     CombineBuffers& b = c->comb;
-    if (!b.d_groups) {
-        CUDA_TRY(cudaMalloc(&b.d_groups, sizeof(int) * (2 * kCombMaxK + 1)));
-        CUDA_TRY(cudaMallocHost(&b.h_groups, sizeof(int) * (2 * kCombMaxK + 1)));
-        CUDA_TRY(cudaEventCreate(&b.t0));
-        CUDA_TRY(cudaEventCreate(&b.t1));
-    }
-    if (part > b.part_doubles) {
-        cudaFree(b.d_part);
-        b.d_part = nullptr;
-        b.part_doubles = 0;
-        CUDA_TRY(cudaMalloc(&b.d_part, sizeof(double) * part));
-        b.part_doubles = part;
-    }
-    if (sum > b.sum_doubles) {
-        cudaFree(b.d_sum);
-        if (b.h_sum) cudaFreeHost(b.h_sum);
-        b.d_sum = b.h_sum = nullptr;
-        b.sum_doubles = 0;
-        CUDA_TRY(cudaMalloc(&b.d_sum, sizeof(double) * sum));
-        CUDA_TRY(cudaMallocHost(&b.h_sum, sizeof(double) * sum));
-        b.sum_doubles = sum;
-    }
+    if (int rc = b.d_groups.reserve(2 * kCombMaxK + 1)) return rc;
+    if (int rc = b.h_groups.reserve(2 * kCombMaxK + 1)) return rc;
+    if (int rc = b.t0.create(cudaEventDefault)) return rc;
+    if (int rc = b.t1.create(cudaEventDefault)) return rc;
+    if (int rc = b.d_part.reserve(part)) return rc;
+    if (int rc = b.d_sum.reserve(sum)) return rc;
+    if (int rc = b.h_sum.reserve(sum)) return rc;
     return GMM_OK;
 }
 
@@ -2698,10 +2563,8 @@ int gmm_combine_labels(gmm_ctx* c, int K, const int* group, int G, int* labels_o
     const auto t0 = std::chrono::steady_clock::now();
     CombineBuffers& b = c->comb;
     if (int rc = combine_buffers(c, 1, 1)) return rc;
-    if (!b.d_lab) {
-        CUDA_TRY(cudaMalloc(&b.d_lab, sizeof(int) * c->memb_pitch));
-        CUDA_TRY(cudaMalloc(&b.d_max, sizeof(float) * c->memb_pitch));
-    }
+    if (int rc = b.d_lab.reserve(c->memb_pitch)) return rc;
+    if (int rc = b.d_max.reserve(c->memb_pitch)) return rc;
     if (c->n > 0) {
         if (int rc = combine_upload_groups(c, groups)) return rc;
         const int nq = (c->n + 3) / 4;
@@ -2733,7 +2596,7 @@ int gmm_get_combine_profile(gmm_ctx* c, double out[3], int reset) {
 // gmm.h in cluster order.  *klast = the last cluster with pi > 0.
 static int sample_params(gmm_ctx* c, int K, int* klast) {
     const int D = c->D, REC = sample_rec_floats(D);
-    double* cum = reinterpret_cast<double*>(c->sample.h_block);
+    double* cum = reinterpret_cast<double*>(c->sample.h_block.get());
     float* rec = reinterpret_cast<float*>(cum + sample_cum_len(K));
     double run = 0.0;
     *klast = -1;
@@ -2815,8 +2678,8 @@ int gmm_sample(gmm_ctx* c, int K, long long n, unsigned long long seed, long lon
     CUDA_TRY(cudaSetDevice(c->device));
     const auto t0 = std::chrono::steady_clock::now();
     SampleBuffers& sb = c->sample;
-    if (!sb.d_block) CUDA_TRY(cudaMalloc(&sb.d_block, sample_block_bytes(c->Kmax, c->D)));
-    if (!sb.h_block) CUDA_TRY(cudaMallocHost(&sb.h_block, sample_block_bytes(c->Kmax, c->D)));
+    if (int rc = sb.d_block.reserve(sample_block_bytes(c->Kmax, c->D) / sizeof(double))) return rc;   // a multiple of 16 bytes
+    if (int rc = sb.h_block.reserve(sample_block_bytes(c->Kmax, c->D))) return rc;
     int klast = 0;
     int rc = sample_params(c, K, &klast);
     if (rc == GMM_OK && n > 0) {
@@ -2850,8 +2713,8 @@ static size_t condition_block_floats(int Kmax, int D) {
 // gmm_condition's parameter block and its pinned mirror, allocated on the first call of either conditioning call.
 static int condition_block(gmm_ctx* c) {
     ConditionBuffers& cb = c->cond;
-    if (!cb.d_block) CUDA_TRY(cudaMalloc(&cb.d_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
-    if (!cb.h_block) CUDA_TRY(cudaMallocHost(&cb.h_block, sizeof(float) * condition_block_floats(c->Kmax, c->D)));
+    if (int rc = cb.d_block.reserve(condition_block_floats(c->Kmax, c->D))) return rc;
+    if (int rc = cb.h_block.reserve(condition_block_floats(c->Kmax, c->D))) return rc;
     return GMM_OK;
 }
 
@@ -2989,16 +2852,9 @@ int gmm_condition(gmm_ctx* c, int K, const int* obs_dims, int n_obs, const float
     int rc = condition_params(c, K, obs_dims, n_obs, mis, nm, impute);
     if (rc == GMM_OK && n > 0) {
         rc = score_buffers(c);
-        const size_t want = 2 * (size_t)c->score_chunk * nm;
-        if (rc == GMM_OK && impute && cb.imp_floats < want) {
-            cb.release_imp();
-            for (int b = 0; b < 2 && rc == GMM_OK; b++) {
-                cudaError_t e = cudaMalloc(&cb.d_imp[b], sizeof(float) * want);
-                if (e == cudaSuccess) e = cudaMallocHost(&cb.h_imp[b], sizeof(float) * want);
-                if (e != cudaSuccess) rc = fail(GMM_ERR_CUDA, std::string("gmm_condition: imputation buffers: ") + cudaGetErrorString(e));
-            }
-            if (rc == GMM_OK) cb.imp_floats = want;
-            else cb.release_imp();
+        for (int b = 0; b < 2 && rc == GMM_OK && impute; b++) {
+            rc = cb.d_imp[b].reserve(2 * (size_t)c->score_chunk * nm);
+            if (rc == GMM_OK) rc = cb.h_imp[b].reserve(2 * (size_t)c->score_chunk * nm);
         }
         if (rc == GMM_OK)
             rc = condition_batch(c, K, n_obs, nm, impute, events_obs, n, {labels, max_resp, logp, &ll}, cond_mean, cond_var);
@@ -3028,8 +2884,8 @@ static int condition_stats_batch(gmm_ctx* c, int K, int n_obs, unsigned obs_mask
     const int D = c->D;
     const size_t KF = (size_t)K * c->F;
     const bool m_tensor = with_stats && use_tensor_mstep(c, K);
-    const float* inv_scale_f = m_tensor ? tc_inv_scale_f(c->tc) : nullptr;
-    const float zb = m_tensor ? tc_mstep_zbound(c->tc) : INFINITY;
+    const float* inv_scale_f = m_tensor ? tc_inv_scale_f(c->tc.get()) : nullptr;
+    const float zb = m_tensor ? tc_mstep_zbound(c->tc.get()) : INFINITY;
     if (m_tensor && !inv_scale_f) return fail(GMM_ERR_STATE, "gmm_condition_stats: the tensor M-step has no centre");
     float shift_f[GMM_MAX_DIMENSIONS] = {0};               // the float centre the M-steps use (c->shift is rounded to it
     for (int d = 0; d < D; d++) shift_f[d] = (float)c->shift[d];   // whenever the wgmma M-step can run)
@@ -3048,7 +2904,7 @@ static int condition_stats_batch(gmm_ctx* c, int K, int n_obs, unsigned obs_mask
         return launch_estep_simt_on(c, n_obs, K, c->cond.d_block, t.d_xo, m, t.d_memb, t.pitch, t.d_stats + KF);
     };
     return stats_batch(c, K, ev, n_obs, n, with_stats, memberships, false, m_tensor, t.cond_prof, "gmm_condition_stats",
-                       [&](int b, int m) { return prep(b, m, t.d_xo, m_tensor ? t.d_z : nullptr, with_stats && !m_tensor ? t.d_xs : nullptr); },
+                       [&](int b, int m) { return prep(b, m, t.d_xo, m_tensor ? t.d_z.get() : nullptr, with_stats && !m_tensor ? t.d_xs.get() : nullptr); },
                        estep);
 }
 
@@ -3171,8 +3027,8 @@ int gmm_fit(gmm_ctx* c, int K0, int target_K, int min_iters, int max_iters, clus
     const float epsilon = em_epsilon(D, em_count(c));
     float min_rissanen = 0;
     int ideal = K0;
-    if (saved->memberships && !c->d_memb_saved && c->n > 0)
-        CUDA_TRY(cudaMalloc(&c->d_memb_saved, sizeof(float) * c->memb_pitch * c->Kmax));
+    if (saved->memberships && c->n > 0)
+        if (int rc = c->d_memb_saved.reserve(c->memb_pitch * c->Kmax)) return rc;
     for (int K = K0; K >= stop_number;) {
         float likelihood; int iters;
         if (int rc = gmm_em(c, K, min_iters, max_iters, epsilon, &likelihood, &iters)) return rc;

@@ -57,6 +57,7 @@
 #include <type_traits>
 #include <vector>
 
+#include "cuda_owned.h"
 #include "host_math.h"
 #include "kernels_tc.cuh"
 #include "mstep_rows.h"
@@ -65,13 +66,6 @@
 namespace gmm {
 
 using namespace ptx;
-
-#define TC_CUDA_TRY(expr)                                                                     \
-    do {                                                                                      \
-        cudaError_t e_ = (expr);                                                              \
-        if (e_ != cudaSuccess)                                                                \
-            return fail(GMM_ERR_CUDA, std::string(#expr) + ": " + cudaGetErrorString(e_));    \
-    } while (0)
 
 // ---------------------------------------------------------------------------
 // M-step kernel configuration
@@ -1391,23 +1385,22 @@ score_tc_kernel(const float* __restrict__ x_aos, const uint8_t* __restrict__ b_i
 struct TcState {
     const float* d_x = nullptr;
     const float* d_x_soa = nullptr;
-    float* d_z_soa = nullptr;        // [D][memb_pitch] centred/scaled SoA copy (M-step TMA source)
+    DeviceArray<float> d_z_soa;      // [D][memb_pitch] centred/scaled SoA copy (M-step TMA source)
     float* d_memb = nullptr;
     size_t memb_pitch = 0;
     int n = 0, D = 0, Kmax = 0, num_sms = 132;
     CUtensorMap tm_x{}, tm_g{};
     bool maps_ok = false;
-    float* d_shift_f = nullptr;      // [32]
-    float* d_inv_scale_f = nullptr;  // [32]
-    double* d_scale = nullptr;       // [32] = 1 / inv_scale_f (double)
-    float* d_scratch = nullptr;      // [32-cluster blocks][ranges][MT][128][32] per-range partial sums, written once per launch
-    size_t scratch_floats = 0;
+    DeviceArray<float> d_shift_f;    // [32]
+    DeviceArray<float> d_inv_scale_f;   // [32]
+    DeviceArray<double> d_scale;     // [32] = 1 / inv_scale_f (double)
+    DeviceArray<float> d_scratch;    // [32-cluster blocks][ranges][MT][128][32] per-range partial sums, written once per launch
     bool have_shift = false;
     bool mstep_ready = false;        // the fixed-point quanta of the feature rows are set and inside the supported range
     float zmax[GMM_MAX_DIMENSIONS] = {0};    // power-of-two bound of |z_d| over the whole data set
     MMagic magic{0.f, 0.f};          // rounding constants of the coordinate / product rows
-    int3* d_rowmap = nullptr;        // [MT * 128] operand row -> (packed statistic, dimension i, dimension j)
-    int* d_opmap = nullptr;          // [MT * 128] operand row -> its factors a | b << 8 (mstep_row_layout)
+    DeviceArray<int3> d_rowmap;      // [MT * 128] operand row -> (packed statistic, dimension i, dimension j)
+    DeviceArray<int> d_opmap;        // [MT * 128] operand row -> its factors a | b << 8 (mstep_row_layout)
     CUtensorMap tm_cx{}, tm_cg{};    // tc_launch_mstep_on: maps over the caller's chunk buffers, for cmap_n events
     const void* cmap_z = nullptr;
     const void* cmap_g = nullptr;
@@ -1419,13 +1412,13 @@ struct TcState {
     uint8_t* d_bimg = nullptr;       // [MAXNG * B_GROUP] resident B operand image
     uint8_t* h_bimg = nullptr;       // pinned
     size_t bimg_bytes = 0;
-    uint8_t* d_opnd = nullptr;       // [ck (e_ck_len floats) | B image]; d_ck / d_bimg point into it
-    uint8_t* h_opnd = nullptr;       // pinned mirror
-    cudaEvent_t ev_h2d = nullptr;    // the last operand copy has left the pinned buffer
+    DeviceArray<uint8_t> d_opnd;     // [ck (e_ck_len floats) | B image]; d_ck / d_bimg point into it
+    PinnedArray<uint8_t> h_opnd;     // mirror
+    Event ev_h2d;                    // the last operand copy has left the pinned buffer
     bool h2d_pending = false;
     float* d_ck = nullptr;           // [passes][ck 64 | mult 64]: additive constant and quadratic-form multiplier per cluster
     float* h_ck = nullptr;           // pinned mirror
-    float* d_den = nullptr;          // [memb_pitch] running / total log-denominator per event (Kmax > 64 only)
+    DeviceArray<float> d_den;        // [memb_pitch] running / total log-denominator per event (Kmax > 64 only)
     int e_ck_len = 0;                // Kmax rounded up to whole passes of 64
     int e_NG = 0;
     int host_threads = 8;
@@ -1481,12 +1474,12 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
     t->d_x = d_x_aos; t->d_x_soa = d_x_soa; t->d_memb = d_memb; t->memb_pitch = memb_pitch; t->n = n; t->D = D; t->Kmax = Kmax; t->num_sms = num_sms;
     *out = t;
     if (n <= 0 || !tc_mstep_supported(D, Kmax)) return GMM_OK;
-    TC_CUDA_TRY(cudaMalloc(&t->d_shift_f, sizeof(float) * GMM_MAX_DIMENSIONS));
-    TC_CUDA_TRY(cudaMalloc(&t->d_inv_scale_f, sizeof(float) * GMM_MAX_DIMENSIONS));
-    TC_CUDA_TRY(cudaMalloc(&t->d_scale, sizeof(double) * GMM_MAX_DIMENSIONS));
+    if (int rc = t->d_shift_f.reserve(GMM_MAX_DIMENSIONS)) return rc;
+    if (int rc = t->d_inv_scale_f.reserve(GMM_MAX_DIMENSIONS)) return rc;
+    if (int rc = t->d_scale.reserve(GMM_MAX_DIMENSIONS)) return rc;
     // tensor maps: SoA events [D][pitch] viewed as (events, dims) -> smem tile [D][32 events] (SWIZZLE_128B);
     // responsibilities [Kmax][pitch] viewed as (events, clusters)
-    TC_CUDA_TRY(cudaMalloc(&t->d_z_soa, sizeof(float) * memb_pitch * D));
+    if (int rc = t->d_z_soa.reserve(memb_pitch * D)) return rc;
     if (int rc = make_map_2d(&t->tm_x, t->d_z_soa, (uint64_t)n, (uint64_t)D, (uint64_t)memb_pitch * 4, kTE, (uint32_t)D, /*swizzle128=*/true)) return rc;
     if (int rc = make_map_2d(&t->tm_g, d_memb, (uint64_t)n, (uint64_t)Kmax, (uint64_t)memb_pitch * 4, kTE, kNCL, /*swizzle128=*/true)) return rc;
     t->maps_ok = true;
@@ -1496,14 +1489,15 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
         t->bimg_bytes = (size_t)passes * pass_bytes_for(D);
         // one staging / device buffer [ck | B image]: the operand of an iteration travels in ONE H2D copy
         const size_t ck_bytes = sizeof(float) * 2 * t->e_ck_len;     // 512 B per pass: keeps the image 16-byte aligned
-        TC_CUDA_TRY(cudaMalloc(&t->d_opnd, ck_bytes + t->bimg_bytes));
-        TC_CUDA_TRY(cudaMallocHost(&t->h_opnd, ck_bytes + t->bimg_bytes));
-        t->d_ck = reinterpret_cast<float*>(t->d_opnd);
-        t->h_ck = reinterpret_cast<float*>(t->h_opnd);
+        if (int rc = t->d_opnd.reserve(ck_bytes + t->bimg_bytes)) return rc;
+        if (int rc = t->h_opnd.reserve(ck_bytes + t->bimg_bytes)) return rc;
+        t->d_ck = reinterpret_cast<float*>(t->d_opnd.get());
+        t->h_ck = reinterpret_cast<float*>(t->h_opnd.get());
         t->d_bimg = t->d_opnd + ck_bytes;
         t->h_bimg = t->h_opnd + ck_bytes;
-        TC_CUDA_TRY(cudaEventCreateWithFlags(&t->ev_h2d, cudaEventDisableTiming));
-        if (passes > 1) TC_CUDA_TRY(cudaMalloc(&t->d_den, sizeof(float) * memb_pitch));
+        if (int rc = t->ev_h2d.create(cudaEventDisableTiming)) return rc;
+        if (passes > 1)
+            if (int rc = t->d_den.reserve(memb_pitch)) return rc;
         t->emap_ok = true;
     }
     const int mt = mstep_tiles(D);
@@ -1524,15 +1518,13 @@ int tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, 
             }
         }
         for (char c : seen) if (!c) return fail(GMM_ERR_STATE, "tensor M-step row map: a statistic is not produced");
-        TC_CUDA_TRY(cudaMalloc(&t->d_rowmap, sizeof(int3) * rm.size()));
-        TC_CUDA_TRY(cudaMemcpy(t->d_rowmap, rm.data(), sizeof(int3) * rm.size(), cudaMemcpyHostToDevice));
-        TC_CUDA_TRY(cudaMalloc(&t->d_opmap, sizeof(int) * om.size()));
-        TC_CUDA_TRY(cudaMemcpy(t->d_opmap, om.data(), sizeof(int) * om.size(), cudaMemcpyHostToDevice));
+        if (int rc = t->d_rowmap.reserve(rm.size())) return rc;
+        CUDA_TRY(cudaMemcpy(t->d_rowmap, rm.data(), sizeof(int3) * rm.size(), cudaMemcpyHostToDevice));
+        if (int rc = t->d_opmap.reserve(om.size())) return rc;
+        CUDA_TRY(cudaMemcpy(t->d_opmap, om.data(), sizeof(int) * om.size(), cudaMemcpyHostToDevice));
     }
     const int ytiles = (Kmax + 63) / 64 * (64 / kNCL);         // 32-cluster column blocks of whole 64-cluster CTAs
-    t->scratch_floats = (size_t)num_sms * ytiles * mt * 128 * kNCL;
-    TC_CUDA_TRY(cudaMalloc(&t->d_scratch, sizeof(float) * t->scratch_floats));
-    return GMM_OK;
+    return t->d_scratch.reserve((size_t)num_sms * ytiles * mt * 128 * kNCL);
 }
 
 void tc_set_host_threads(TcState* t, int n) { if (t) t->host_threads = n < 1 ? 1 : n; }
@@ -1544,14 +1536,7 @@ bool tc_estep_range_ok(const TcState* t) {
     return true;
 }
 
-void tc_destroy(TcState* t) {
-    if (!t) return;
-    cudaFree(t->d_shift_f); cudaFree(t->d_inv_scale_f); cudaFree(t->d_scale); cudaFree(t->d_scratch);
-    cudaFree(t->d_opnd); cudaFree(t->d_den); cudaFree(t->d_z_soa); cudaFree(t->d_rowmap); cudaFree(t->d_opmap);
-    if (t->h_opnd) cudaFreeHost(t->h_opnd);
-    if (t->ev_h2d) cudaEventDestroy(t->ev_h2d);
-    delete t;
-}
+void tc_destroy(TcState* t) { delete t; }
 
 int tc_set_shift_scale(TcState* t, double* shift, const double* scale, const double* xmin, const double* xmax, cudaStream_t stream) {
     if (!t || !t->maps_ok) return GMM_OK;
@@ -1583,15 +1568,15 @@ int tc_set_shift_scale(TcState* t, double* shift, const double* scale, const dou
         t->magic.lin = (float)(1.5 * 8388608.0 * q);
         t->magic.prod = (float)(1.5 * 8388608.0 * q * (double)zb);
     }
-    TC_CUDA_TRY(cudaMemcpyAsync(t->d_shift_f, sf, sizeof(sf), cudaMemcpyHostToDevice, stream));
-    TC_CUDA_TRY(cudaMemcpyAsync(t->d_inv_scale_f, isf, sizeof(isf), cudaMemcpyHostToDevice, stream));
-    TC_CUDA_TRY(cudaMemcpyAsync(t->d_scale, sc, sizeof(sc), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(t->d_shift_f, sf, sizeof(sf), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(t->d_inv_scale_f, isf, sizeof(isf), cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaMemcpyAsync(t->d_scale, sc, sizeof(sc), cudaMemcpyHostToDevice, stream));
     {
         dim3 grid((unsigned)std::min<long long>(4LL * t->num_sms, ((long long)t->n + 255) / 256), (unsigned)t->D);
         standardise_soa_kernel<<<grid, 256, 0, stream>>>(t->d_x_soa, t->d_z_soa, t->memb_pitch, t->n, t->D, t->d_shift_f, t->d_inv_scale_f);
-        TC_CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
     }
-    TC_CUDA_TRY(cudaStreamSynchronize(stream));         // the staging arrays live on this stack frame
+    CUDA_TRY(cudaStreamSynchronize(stream));         // the staging arrays live on this stack frame
     t->have_shift = true;
     return GMM_OK;
 }
@@ -1745,7 +1730,7 @@ int tc_params_begin(TcState* t, int K, cudaStream_t stream) {
     if (!t->have_shift) return fail(GMM_ERR_STATE, "tensor E-step needs the global moments (shift/scale) first");
     (void)stream;
     if (t->h2d_pending) {                                // the previous copy out of the pinned buffer must have finished
-        TC_CUDA_TRY(cudaEventSynchronize(t->ev_h2d));
+        CUDA_TRY(cudaEventSynchronize(t->ev_h2d));
         t->h2d_pending = false;
     }
     for (int k = K; k < t->e_ck_len; k++) {               // padding clusters: never win the log-sum-exp
@@ -1765,8 +1750,8 @@ int tc_params_commit(TcState* t, int K, int bad, cudaStream_t stream) {
     t->e_NG = (K + 15) / 16;
     // only the supergroups in use travel (the image is contiguous per supergroup; 4 supergroups = 64 clusters)
     const size_t used = (size_t)t->e_NG * (pass_bytes_for(t->D) / 4);
-    TC_CUDA_TRY(cudaMemcpyAsync(t->d_opnd, t->h_opnd, sizeof(float) * 2 * t->e_ck_len + used, cudaMemcpyHostToDevice, stream));
-    TC_CUDA_TRY(cudaEventRecord(t->ev_h2d, stream));
+    CUDA_TRY(cudaMemcpyAsync(t->d_opnd, t->h_opnd, sizeof(float) * 2 * t->e_ck_len + used, cudaMemcpyHostToDevice, stream));
+    CUDA_TRY(cudaEventRecord(t->ev_h2d, stream));
     t->h2d_pending = true;
     return GMM_OK;
 }
@@ -2056,7 +2041,7 @@ int tc_launch_finalize(TcState* t, int K, const double* d_stats, const float* d_
         default: return fail(GMM_ERR_ARG, "device-side finalisation: unsupported D");
     }
 #undef GMM_FIN
-    TC_CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     t->e_NG = (K + 15) / 16;
     return GMM_OK;
 }
@@ -2074,8 +2059,8 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
                                            estep_tc_kernel<D, 4, true>};
     static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_estep) {
-        for (auto* k : kern0) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
-        for (auto* k : kern1) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
+        for (auto* k : kern0) CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
+        for (auto* k : kern1) CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM_BYTES));
         t->attr_estep = true;
     }
     const KernFn* kern = w ? kern1 : kern0;
@@ -2095,11 +2080,11 @@ static int launch_estep_d(TcState* t, int K, const float* x, int n, float* memb,
             memb + (size_t)(64 * p) * pitch, pitch, n, Kp, d_ll, mode, den_in, den_out, w);
         return cudaGetLastError();
     };
-    if (NP == 1) TC_CUDA_TRY(launch(0, 0, nullptr, nullptr));
+    if (NP == 1) CUDA_TRY(launch(0, 0, nullptr, nullptr));
     else {
-        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 1, p ? den : nullptr, den));
-        TC_CUDA_TRY(launch(NP - 1, 2, den, den));
-        for (int p = 0; p + 1 < NP; p++) TC_CUDA_TRY(launch(p, 3, den, nullptr));
+        for (int p = 0; p + 1 < NP; p++) CUDA_TRY(launch(p, 1, p ? den : nullptr, den));
+        CUDA_TRY(launch(NP - 1, 2, den, den));
+        for (int p = 0; p + 1 < NP; p++) CUDA_TRY(launch(p, 3, den, nullptr));
     }
     return GMM_OK;
 }
@@ -2134,7 +2119,7 @@ static int launch_score_d(TcState* t, int K, const TcScoreIo& io, cudaStream_t s
         score_tc_kernel<D, 1>, score_tc_kernel<D, 2>, score_tc_kernel<D, 3>, score_tc_kernel<D, 4>};
     static_assert(C::MAXSG == 4, "one kernel instance per supergroup count");
     if (!t->attr_score) {
-        for (auto* k : kern) TC_CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
+        for (auto* k : kern) CUDA_TRY(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM_BYTES));
         t->attr_score = true;
     }
     const int ntiles = (io.n + 127) / 128;
@@ -2148,7 +2133,7 @@ static int launch_score_d(TcState* t, int K, const TcScoreIo& io, cudaStream_t s
         kern[(Kp + C::GB - 1) / C::GB - 1]<<<grid, C::THREADS, C::SMEM_BYTES, stream>>>(
             io.x, t->d_bimg + (size_t)p * C::MAXSG * C::B_SG, t->d_ck + 128 * p, t->d_shift_f, t->d_inv_scale_f, io.n, Kp, 64 * p, p, p + 1 == NP, io.run_den, io.run_bl, io.run_bk, io.labels, io.max_resp, io.logp, io.ll,
             io.flag);
-        TC_CUDA_TRY(cudaGetLastError());
+        CUDA_TRY(cudaGetLastError());
     }
     return GMM_OK;
 }
@@ -2173,10 +2158,10 @@ static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUte
     using C64 = MCfg<D, 64>;
     static_assert(C32::SMEM_BYTES <= 232448 && C64::SMEM_BYTES <= 232448, "shared memory budget");
     if (!t->attr_mstep) {
-        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
-        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
-        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
-        TC_CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
+        CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
+        CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
+        CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 32, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C32::SMEM_BYTES));
+        CUDA_TRY(cudaFuncSetAttribute(mstep_tc_kernel<D, 64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, C64::SMEM_BYTES));
         t->attr_mstep = true;
     }
     const float w_max = (float)wscale, w_inv = (float)(1.0 / wscale);
@@ -2187,7 +2172,7 @@ static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUte
     const bool pair = K > 32;
     const int ncl = pair ? 64 : 32;
     const int gy = (K + ncl - 1) / ncl;
-    if ((size_t)gx * gy * (ncl / kNCL) * C32::MT * 128 * kNCL > t->scratch_floats) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
+    if ((size_t)gx * gy * (ncl / kNCL) * C32::MT * 128 * kNCL > t->d_scratch.size()) return fail(GMM_ERR_STATE, "tensor M-step scratch too small");
     const dim3 grid(pair ? 2 * gx : gx, gy);
     if (pair) {
         if (w) mstep_tc_kernel<D, 64, true><<<grid, C64::THREADS, C64::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, w, w_max, w_inv);
@@ -2196,10 +2181,10 @@ static int launch_mstep_d(TcState* t, int K, const CUtensorMap& tm_x, const CUte
         if (w) mstep_tc_kernel<D, 32, true><<<grid, C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, w, w_max, w_inv);
         else mstep_tc_kernel<D, 32><<<grid, C32::THREADS, C32::SMEM_BYTES, stream>>>(tm_x, tm_g, n, K, t->d_scratch, per, t->magic, t->d_opmap, nullptr, 1.0f, 1.0f);
     }
-    TC_CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     mstep_tc_finalize_kernel<<<C32::MT * 128, 256, 0, stream>>>(t->d_scratch, gx, C32::MT, K, C32::F, t->d_rowmap, t->d_scale, d_stats,
                                                                 w ? wscale : 1.0);
-    TC_CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaGetLastError());
     return GMM_OK;
 }
 
@@ -2236,8 +2221,8 @@ int tc_launch_mstep_on(TcState* t, int K, const float* d_z, const float* d_memb,
     return launch_mstep_any(t, K, t->tm_cx, t->tm_cg, n, d_stats, nullptr, 1.0, stream);
 }
 
-const float* tc_shift_f(const TcState* t) { return t && t->have_shift ? t->d_shift_f : nullptr; }
-const float* tc_inv_scale_f(const TcState* t) { return t && t->have_shift ? t->d_inv_scale_f : nullptr; }
+const float* tc_shift_f(const TcState* t) { return t && t->have_shift ? t->d_shift_f.get() : nullptr; }
+const float* tc_inv_scale_f(const TcState* t) { return t && t->have_shift ? t->d_inv_scale_f.get() : nullptr; }
 float tc_mstep_zbound(const TcState* t) {
     float zb = 0.f;
     if (t)

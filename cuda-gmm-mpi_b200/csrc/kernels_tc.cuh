@@ -15,7 +15,9 @@ bool tc_estep_supported(int D, int K);
 // memb_pitch: row pitch (in floats) of the cluster-major responsibilities buffer AND of the SoA event copy.
 int  tc_create(TcState** out, const float* d_x_aos, const float* d_x_soa, int n, int D, int Kmax, float* d_memb, size_t memb_pitch,
                int num_sms, cudaStream_t stream);
+// On failure *out still holds the partly built state, for its owner to destroy.
 void tc_destroy(TcState*);
+struct TcStateDelete { void operator()(TcState* t) const { tc_destroy(t); } };
 void tc_set_host_threads(TcState*, int n);
 // Centre/scale used inside the tensor kernels: z = (x - shift) * inv_scale, both rounded to
 // float; `shift` is updated in place to the float-rounded values actually used.  xmin / xmax: per-dimension extremes
