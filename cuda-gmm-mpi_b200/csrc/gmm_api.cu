@@ -39,6 +39,7 @@
 #include "kernels_tc.cuh"
 #include "kernels_vb.cuh"
 #include "kernels_combine.cuh"
+#include "kernels_multisample.cuh"
 
 namespace gmm {
 
@@ -377,6 +378,21 @@ struct CombineBuffers {
     double kernel_ms = 0, wall_ms = 0, labels_wall_ms = 0;   // gmm_get_combine_profile
 };
 
+// gmm_em_multisample: the reweight pass's inputs and outputs, reserved on first use and grown with S, K and the shard
+struct MultisampleBuffers {
+    DeviceArray<float> d_rho;                   // [S][K] rho_{s,k} of the next reweight
+    PinnedArray<float> h_rho;
+    DeviceArray<MsUnit> d_units;                // the shard's work units
+    PinnedArray<MsUnit> h_units;
+    DeviceArray<int> d_idx;                     // cta_begin [G + 1], then sample_part [S + 1]
+    PinnedArray<int> h_idx;
+    DeviceArray<double> d_part;                 // [records][K + 2] per (CTA, sample segment)
+    DeviceArray<double> d_mass;                 // [S][K + 1]: M_{s,k}, then n_s (all-reduced)
+    PinnedArray<double> h_mass;
+    PhaseTimer timer;                           // the reweight and finishing kernels
+    double host_ms = 0, wall_ms = 0;            // gmm_get_multisample_profile
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -468,6 +484,7 @@ struct gmm_ctx {
     PhaseTimer t_entropy;
     double vb_final_ms = 0, vb_wall_ms = 0;   // gmm_get_vb_profile
     CombineBuffers comb;         // gmm_combine / gmm_combine_labels: allocated on first use
+    MultisampleBuffers msamp;    // gmm_em_multisample: allocated on first use
 };
 
 namespace gmm {
@@ -2588,6 +2605,244 @@ int gmm_get_combine_profile(gmm_ctx* c, double out[3], int reset) {
     if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_combine_profile: bad argument");
     out[0] = c->comb.kernel_ms; out[1] = c->comb.wall_ms; out[2] = c->comb.labels_wall_ms;
     if (reset) c->comb.kernel_ms = c->comb.wall_ms = c->comb.labels_wall_ms = 0;
+    return GMM_OK;
+}
+
+// ---- EM over several samples with shared components (gmm_em_multisample) ----------------------------------------------
+struct MsPlan {
+    int E = 0, G = 0, records = 0;
+};
+
+using MsKernel = void (*)(float*, size_t, int, const float*, const float*, const MsUnit*, const int*, int, double*);
+
+// The instance of the reweight pass for the context's weights, with its dynamic shared memory allowed.
+static int ms_kernel(gmm_ctx* c, int K, int E, bool masses_only, MsKernel* fn, size_t* smem) {
+    const bool w = step_weights(c) != nullptr;
+    *fn = w ? (masses_only ? ms_reweight_kernel<true, true> : ms_reweight_kernel<true, false>)
+            : (masses_only ? ms_reweight_kernel<false, true> : ms_reweight_kernel<false, false>);
+    *smem = ms_smem_bytes(K, E, masses_only);
+    CUDA_TRY(cudaFuncSetAttribute(*fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+    return GMM_OK;
+}
+
+// One instance of the reweight pass over the plan's units.
+static int ms_launch(gmm_ctx* c, int K, const MsPlan& pl, bool masses_only) {
+    MsKernel fn;
+    size_t smem;
+    if (int rc = ms_kernel(c, K, pl.E, masses_only, &fn, &smem)) return rc;
+    MultisampleBuffers& b = c->msamp;
+    fn<<<pl.G, kMsThreads, smem, c->stream>>>(c->d_memb, c->memb_pitch, K, step_weights(c), b.d_rho, b.d_units, b.d_idx, pl.E, b.d_part);
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+
+// The shard's work units (windows of E events aligned to E, split at sample boundaries), G persistent CTAs over contiguous
+// runs of them and a partial record per (CTA, sample segment), uploaded with the buffers the pass needs.
+static int ms_plan(gmm_ctx* c, int K, int S, const long long* offsets, MsPlan* pl) {
+    MultisampleBuffers& b = c->msamp;
+    const int E = ms_window_events(K);
+    std::vector<MsUnit> units;
+    const long long lo = c->offset, hi = c->offset + c->n;
+    for (int s = 0; s < S; s++) {
+        const long long a = std::max(offsets[s], lo), z = std::min(offsets[s + 1], hi);
+        for (long long x = a; x < z;) {
+            const int l0 = (int)(x - lo);
+            const int l1 = (int)std::min<long long>(z - lo, (long long)((l0 & ~(E - 1)) + E));
+            units.push_back({s, l0, l1, 0});
+            x = lo + l1;
+        }
+    }
+    // one resident wave of whichever of the call's two instances (full, masses-only) fits fewer CTAs per SM
+    int per_sm = 0;
+    for (bool masses_only : {false, true}) {
+        MsKernel fn;
+        size_t smem;
+        int blocks = 0;
+        if (int rc = ms_kernel(c, K, E, masses_only, &fn, &smem)) return rc;
+        CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, fn, kMsThreads, smem));
+        per_sm = masses_only ? std::min(per_sm, blocks) : blocks;
+    }
+    const long long U = (long long)units.size();
+    const int G = (int)std::min<long long>(U, (long long)std::max(per_sm, 1) * c->num_sms);
+    std::vector<int> idx((size_t)G + 1 + S + 1, 0);
+    int* cta = idx.data();
+    int* spart = idx.data() + G + 1;
+    std::vector<int> rec_sample;                          // the sample of each record
+    for (int g = 0; g < G; g++) {
+        cta[g] = (int)(U * g / G);
+        cta[g + 1] = (int)(U * (g + 1) / G);
+        for (int u = cta[g]; u < cta[g + 1]; u++) {
+            if (u == cta[g] || units[(size_t)u].s != units[(size_t)u - 1].s) rec_sample.push_back(units[(size_t)u].s);
+            units[(size_t)u].part = (int)rec_sample.size() - 1;
+        }
+    }
+    const int records = (int)rec_sample.size();
+    // the records of sample s are [spart[s], spart[s + 1]): records are in CTA order and the samples never decrease
+    for (int s = 0, r = 0; s <= S; s++) {
+        while (r < records && rec_sample[(size_t)r] < s) r++;
+        spart[s] = r;
+    }
+    if (int rc = b.d_rho.reserve((size_t)S * K)) return rc;
+    if (int rc = b.h_rho.reserve((size_t)S * K)) return rc;
+    if (int rc = b.d_units.reserve(std::max<size_t>(units.size(), 1))) return rc;
+    if (int rc = b.h_units.reserve(std::max<size_t>(units.size(), 1))) return rc;
+    if (int rc = b.d_idx.reserve(idx.size())) return rc;
+    if (int rc = b.h_idx.reserve(idx.size())) return rc;
+    if (int rc = b.d_part.reserve(std::max<size_t>((size_t)records * (K + 2), 1))) return rc;
+    if (int rc = b.d_mass.reserve((size_t)S * (K + 1))) return rc;
+    if (int rc = b.h_mass.reserve((size_t)S * (K + 1))) return rc;
+    std::copy(units.begin(), units.end(), b.h_units.get());
+    std::copy(idx.begin(), idx.end(), b.h_idx.get());
+    if (!units.empty())
+        CUDA_TRY(cudaMemcpyAsync(b.d_units, b.h_units, sizeof(MsUnit) * units.size(), cudaMemcpyHostToDevice, c->stream));
+    CUDA_TRY(cudaMemcpyAsync(b.d_idx, b.h_idx, sizeof(int) * idx.size(), cudaMemcpyHostToDevice, c->stream));
+    pl->E = E;
+    pl->G = G;
+    pl->records = records;
+    return GMM_OK;
+}
+
+// The reweight pass over the memberships of the E-step that just ran, the per-sample masses summed and all-reduced, and
+// queued to the pinned mirror (valid after the next stream synchronisation).  masses_only: rho = 1, nothing written.
+static int ms_pass(gmm_ctx* c, int K, int S, const MsPlan& pl, bool masses_only) {
+    MultisampleBuffers& b = c->msamp;
+    timer_begin(c, b.timer);
+    if (pl.G > 0)
+        if (int rc = ms_launch(c, K, pl, masses_only)) return rc;
+    const long long vals = (long long)S * (K + 1);
+    const int grid = (int)std::max<long long>(1, std::min<long long>(4LL * c->num_sms, (vals + kMsFinishThreads - 1) / kMsFinishThreads));
+    ms_finish_kernel<<<grid, kMsFinishThreads, 0, c->stream>>>(b.d_part, b.d_idx + pl.G + 1, S, K, b.d_mass,
+                                                                masses_only ? nullptr : c->d_stats + (size_t)K * c->F);
+    CUDA_TRY(cudaGetLastError());
+    timer_end(c, b.timer);
+    if (c->nranks > 1) {
+        ncclResult_t r = nccl().AllReduce(b.d_mass, b.d_mass, (size_t)vals, ncclDouble, ncclSum, c->comm, c->stream);
+        if (r != ncclSuccess) return fail(GMM_ERR_NCCL, std::string("ncclAllReduce: ") + nccl().GetErrorString(r));
+    }
+    CUDA_TRY(cudaMemcpyAsync(b.h_mass, b.d_mass, sizeof(double) * (size_t)vals, cudaMemcpyDeviceToHost, c->stream));
+    return GMM_OK;
+}
+
+// rho_{s,k} = (float)(pi_{s,k} / (double)pi_k) of the current pooled set (0 where pi_k = 0: pi_{s,k} is 0 there), uploaded.
+static int ms_upload_rho(gmm_ctx* c, int K, int S, const std::vector<double>& pi) {
+    MultisampleBuffers& b = c->msamp;
+    for (int s = 0; s < S; s++)
+        for (int k = 0; k < K; k++) {
+            const double p = (double)c->host.pi[k];
+            b.h_rho[(size_t)s * K + k] = p > 0.0 ? (float)(pi[(size_t)s * K + k] / p) : 0.0f;
+        }
+    CUDA_TRY(cudaMemcpyAsync(b.d_rho, b.h_rho, sizeof(float) * (size_t)S * K, cudaMemcpyHostToDevice, c->stream));
+    return GMM_OK;
+}
+
+static int em_multisample_run(gmm_ctx* c, int K, int S, const long long* offsets, const double* pi_init, int min_iters, int max_iters,
+                              float epsilon, double* pi_out, double* n_out, float* loglik_out, float* logliks_out, int* iters_out) {
+    MultisampleBuffers& b = c->msamp;
+    std::vector<double> pi((size_t)S * K);                   // the pi_{s,k} of the last reweight
+    for (int s = 0; s < S; s++) {
+        double sum = 0.0;
+        if (pi_init)
+            for (int k = 0; k < K; k++) sum += pi_init[(size_t)s * K + k];
+        for (int k = 0; k < K; k++) pi[(size_t)s * K + k] = pi_init ? pi_init[(size_t)s * K + k] / sum : (double)c->host.pi[k];
+    }
+    if (int rc = ensure_moments(c)) return rc;
+    if (epsilon < 0) epsilon = em_epsilon(c->D, em_count(c));
+    MsPlan pl;
+    if (int rc = ms_plan(c, K, S, offsets, &pl)) return rc;
+    if (pi_init)
+        if (int rc = ms_upload_rho(c, K, S, pi)) return rc;
+    const size_t ll_idx = (size_t)K * c->F;
+    if (int rc = zero_stats(c, K)) return rc;
+    if (int rc = run_estep(c, K)) return rc;                 // the start: the E-step under the pooled set, then the reweight
+    if (int rc = ms_pass(c, K, S, pl, /*masses_only=*/!pi_init)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    for (int s = 0; s < S; s++)
+        if (!(b.h_mass[(size_t)s * (K + 1) + K] > 0.0)) {
+            if (pi_init) c->memb_valid = false;
+            return fail(GMM_ERR_ARG, "gmm_em_multisample: sample " + std::to_string(s) + " has total weight 0");
+        }
+    float likelihood = 0, old_likelihood = 0, change = epsilon * 2;
+    int iters = 0;
+    for (;;) {                                               // gmm_em's loop (gaussian.cu:532), a reweight after every E-step
+        const bool must_continue = iters < min_iters;
+        const bool may_continue = iters < max_iters;
+        if (!must_continue && !may_continue) {
+            if (int rc = reduce_loglik_to_host(c, K, &likelihood)) return rc;
+            if (logliks_out) logliks_out[iters] = likelihood;
+            break;
+        }
+        if (int rc = run_mstep_accumulate(c, K)) return rc;
+        if (int rc = reduce_stats_to_host(c, K)) return rc;   // also waits for the masses of the last reweight
+        likelihood = (float)c->h_stats[ll_idx];
+        if (logliks_out) logliks_out[iters] = likelihood;
+        if (iters > 0) change = likelihood - old_likelihood;
+        if (!(must_continue || (std::fabs(change) > epsilon && may_continue))) break;
+        old_likelihood = likelihood;
+        const auto h0 = std::chrono::steady_clock::now();
+        if (int rc = finalize_and_upload(c, K)) return rc;
+        for (int s = 0; s < S; s++) {
+            const double* m = b.h_mass + (size_t)s * (K + 1);
+            for (int k = 0; k < K; k++) pi[(size_t)s * K + k] = std::max(m[k] / m[K], 1e-10);
+        }
+        if (int rc = ms_upload_rho(c, K, S, pi)) return rc;
+        b.host_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - h0).count();
+        if (int rc = zero_stats(c, K)) return rc;
+        if (int rc = run_estep(c, K)) return rc;
+        if (int rc = ms_pass(c, K, S, pl, false)) return rc;
+        iters++;
+        c->iterations++;
+    }
+    collect_all(c);
+    timer_collect(c, b.timer);
+    if (pi_out) std::copy(pi.begin(), pi.end(), pi_out);
+    if (n_out)
+        for (int s = 0; s < S; s++) n_out[s] = b.h_mass[(size_t)s * (K + 1) + K];
+    if (loglik_out) *loglik_out = likelihood;
+    if (iters_out) *iters_out = iters;
+    return GMM_OK;
+}
+
+int gmm_em_multisample(gmm_ctx* c, int K, int S, const long long* offsets, const double* pi_init, int min_iters, int max_iters,
+                       float epsilon, double* pi_out, double* n_out, float* loglik_out, float* logliks_out, int* iters_out) {
+    if (int rc = check_K(c, K, "gmm_em_multisample")) return rc;
+    if (S < 1 || S > kMsMaxSamples) return fail(GMM_ERR_ARG, "gmm_em_multisample: S must be in [1, 4096]");
+    if (!offsets || offsets[0] != 0 || offsets[S] != c->n_global)
+        return fail(GMM_ERR_ARG, "gmm_em_multisample: offsets must run from 0 to the global event count");
+    for (int s = 0; s < S; s++)
+        if (offsets[s + 1] <= offsets[s]) return fail(GMM_ERR_ARG, "gmm_em_multisample: offsets must be strictly increasing");
+    if (min_iters < 0 || max_iters < min_iters) return fail(GMM_ERR_ARG, "gmm_em_multisample: need 0 <= min_iters <= max_iters");
+    if (K != c->cur_K)
+        return fail(GMM_ERR_STATE, "gmm_em_multisample: parameters for this K have not been set (gmm_seed / gmm_set_clusters)");
+    if (c->params_partial) return fail(GMM_ERR_STATE, "gmm_em_multisample: called between gmm_mstep and gmm_constants");
+    if (pi_init)
+        for (int s = 0; s < S; s++) {
+            double sum = 0.0;
+            for (int k = 0; k < K; k++) {
+                const double v = pi_init[(size_t)s * K + k];
+                if (!(v >= 0.0) || !std::isfinite(v))
+                    return fail(GMM_ERR_ARG, "gmm_em_multisample: pi_init row " + std::to_string(s) + " has a negative or non-finite entry");
+                if (v > 0.0 && !(c->host.pi[k] > 0.0f))
+                    return fail(GMM_ERR_ARG, "gmm_em_multisample: pi_init[" + std::to_string(s) + "][" + std::to_string(k) +
+                                                 "] > 0 where the current pi is 0");
+                sum += v;
+            }
+            if (!(sum > 0.0)) return fail(GMM_ERR_ARG, "gmm_em_multisample: pi_init row " + std::to_string(s) + " sums to 0");
+        }
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    const int rc = em_multisample_run(c, K, S, offsets, pi_init, min_iters, max_iters, epsilon, pi_out, n_out, loglik_out, logliks_out,
+                                      iters_out);
+    c->msamp.wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_get_multisample_profile(gmm_ctx* c, double out[3], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_multisample_profile: bad argument");
+    MultisampleBuffers& b = c->msamp;
+    cudaStreamSynchronize(c->stream);
+    timer_collect(c, b.timer);
+    out[0] = b.timer.total_ms; out[1] = b.host_ms; out[2] = b.wall_ms;
+    if (reset) { b.timer.total_ms = 0; b.host_ms = b.wall_ms = 0; }
     return GMM_OK;
 }
 

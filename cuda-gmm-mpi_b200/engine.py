@@ -139,6 +139,9 @@ def load_library():
     L.gmm_host_combine_groups.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p]
     L.gmm_host_combine_elbow.argtypes = [C.c_void_p, C.c_void_p, C.c_int, _IP]
     L.gmm_get_combine_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_em_multisample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p,
+                                     C.c_void_p, _FP, C.c_void_p, _IP]
+    L.gmm_get_multisample_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
     L.gmm_stats_len.argtypes = [C.c_int, C.c_int]
@@ -571,6 +574,33 @@ class Engine:
         out = (C.c_double * 3)()
         _check(self.lib.gmm_get_combine_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], wall_ms=out[1], labels_wall_ms=out[2])
+
+    def em_multisample(self, K, offsets, pi_init=None, min_iters=0, max_iters=100, epsilon=-1.0, logliks=False):
+        """EM over S samples with shared components and per-sample mixing weights (gmm_em_multisample), from the current
+        K-cluster parameters.  offsets: the S + 1 global event offsets of the samples; pi_init: [S][K] starting weights or
+        None (the pooled pi).  Returns (pi [S][K] float64, n [S] float64, loglik, iters, logliks [iters + 1] or None)."""
+        off = np.ascontiguousarray(offsets, np.int64).reshape(-1)
+        S = off.size - 1
+        if S < 1:
+            raise ValueError("offsets must hold at least two values")
+        p0 = None
+        if pi_init is not None:
+            p0 = np.ascontiguousarray(pi_init, np.float64)
+            if p0.shape != (S, K):
+                raise ValueError(f"pi_init must be [{S}][{K}], got {p0.shape}")
+        pi = np.empty((S, K), np.float64)
+        n = np.empty(S, np.float64)
+        lls = np.full(max(int(max_iters), 0) + 1, np.nan, np.float32) if logliks else None
+        ll, it = C.c_float(), C.c_int()
+        _check(self.lib.gmm_em_multisample(self.h, K, S, off.ctypes.data, p0.ctypes.data if p0 is not None else None, int(min_iters),
+                                           int(max_iters), float(epsilon), pi.ctypes.data, n.ctypes.data, C.byref(ll),
+                                           lls.ctypes.data if lls is not None else None, C.byref(it)))
+        return pi, n, ll.value, it.value, (lls[:it.value + 1] if lls is not None else None)
+
+    def multisample_profile(self, reset=False):
+        out = (C.c_double * 3)()
+        _check(self.lib.gmm_get_multisample_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], host_ms=out[1], wall_ms=out[2])
 
     def comm_rank(self):
         r, n = C.c_int(), C.c_int()

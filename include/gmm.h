@@ -584,6 +584,68 @@ int  gmm_host_combine_elbow(const double* entropy, const double* x /* [K] or NUL
  * gmm_combine, out[2] wall ms inside gmm_combine_labels.                                                             */
 int  gmm_get_combine_profile(gmm_ctx*, double out[3], int reset);
 
+/* ---- EM over several samples with shared components (the maximum-likelihood counterpart of Cron et al., PLoS Comput
+ * Biol 9 (2013) e1003130, without the HDP prior) ----------------------------------------------------------------------
+ * A study is many samples (patients, time points, stimulations) measured on the same panel.  Separate fits give components
+ * that are not aligned; one pooled fit classifies every event under the pool's mixing weights, biasing each sample's
+ * counts toward the pool where populations overlap.  This model keeps the means and covariances shared and gives each
+ * sample s its own mixing weights pi_{s,k}: aligned populations and per-sample abundances from one fit.  ("Sample" is a
+ * set of events measured together, not a draw of gmm_sample.)
+ * Semantics (restated in float64 / float32 numpy by tests/_multisample_ref.py):
+ *   - sample s is the global event range [offsets[s], offsets[s+1]); w_n is the weight of gmm_set_weights (1 without).
+ *   - the library's E-step under the pooled set (pi_k) gives r_nk ~ pi_k N(x_n | k).  With rho_{s,k} = pi_{s,k} / pi_k the
+ *     per-sample posterior is r'_nk = r_nk rho_{s,k} / S_n, S_n = sum_j r_nj rho_{s,j}, and ln p'(x_n) = ln p(x_n) + ln S_n.
+ *     The pooled pi keeps rho <= N / n_s, so no responsibility the reweight needs has underflowed.
+ *   - reweight, per event of sample s, in float with one rounding per operation: t_k = r_k * rho_{s,k}, S = t_0 + t_1 + ...
+ *     in increasing k, r'_k = t_k / S; the log-likelihood correction is w_n log((double)S), summed in double.  Only rows
+ *     k < K of the shard's events are written.  An event whose every t_k is 0 (possible only with zeros in pi_init) gets
+ *     NaN memberships and a -inf log-likelihood.
+ *   - masses M_{s,k} = sum_{n in s} w_n r'_nk and n_s = sum_{n in s} w_n, in double in a fixed order without atomics,
+ *     zeros for samples outside a rank's shard, summed over the ranks by one ncclAllReduce.
+ *   - start: an E-step under the current parameter set for K, then the reweight with pi^0_{s,k} = pi_init[s][k] / sum_j
+ *     pi_init[s][j] (rows need not be normalised).  pi_init = NULL: pi^0_{s,k} = pi_k and rho = 1; the pass then only forms
+ *     the masses, writes no membership and adds nothing to the log-likelihood, so the start equals gmm_estep bit for bit.
+ *   - loop: gmm_em's (the same stop rule, epsilon < 0 selecting the same default, min_iters / max_iters as there), with the
+ *     reweight after every E-step.  Each iteration: the M-step statistics over r', one reduction of them (its
+ *     log-likelihood slot already holds sum w ln p + sum w ln S), the stop test, the host finalisation of gmm_em (N, means,
+ *     R, avgvar rules, constants, the pooled pi with its 0.5 / 1e-10 rules), pi_{s,k} = max(M_{s,k} / n_s, 1e-10) in double
+ *     (floored, not renormalised), rho_{s,k} = (float)(pi_{s,k} / (double)pi_k), then the E-step and the reweight.  Every
+ *     iteration takes the host finalisation (the device-side one of option "finalize" is not used).
+ *   - afterwards: the context holds the pooled parameter set (a valid gmm_em set: gmm_score, gmm_sample and
+ *     gmm_get_clusters see it), cur_K = K, and the memberships are the per-sample posteriors of the last E-step:
+ *     gmm_combine and gmm_combine_labels work on them, a later gmm_estep replaces them with pooled ones.  gmm_get_profile
+ *     counts the iterations.
+ *   - scoring new events of sample s: put pi_out[s] (as float) into the clusters' pi, gmm_set_clusters, then gmm_score.
+ * Collective over the ranks of a communicator, like gmm_em: the same K, S, offsets, pi_init and iteration arguments on
+ * every rank.  A sample may straddle shards.
+ *   offsets      [S+1] global event offsets: offsets[0] = 0, offsets[S] = n_global, strictly increasing; 1 <= S <= 4096
+ *   pi_init      [S][K] starting weights, or NULL
+ *   pi_out       [S][K] the pi_{s,k} the last E-step used, or NULL
+ *   n_out        [S] n_s, or NULL
+ *   loglik_out   the last E-step's multi-sample log-likelihood sum_n w_n ln p'(x_n)
+ *   logliks_out  [max_iters + 1] or NULL: that of E-step i, E-step 0 being the start
+ *   iters_out    iterations run
+ * Kernels (csrc/kernels_multisample.cuh, sm_90a): one reweight pass that reads and writes each membership once (windows of
+ * E events staged in shared memory, persistent CTAs over units that never cross a sample boundary, one partial per CTA and
+ * sample segment) and a finishing kernel that adds the partials per sample in order and the correction into the
+ * statistics' log-likelihood slot.  The E- and M-step kernels, the K > 64 passes and the all-reduce are the library's own.
+ * Errors: K outside [1, Kmax], S outside [1, 4096], bad offsets, a pi_init row with a negative or non-finite entry or a zero
+ * sum, a pi_init entry > 0 where the current pi_k is 0, min_iters < 0 or max_iters < min_iters -> GMM_ERR_ARG; a sample
+ * whose total weight is 0 -> GMM_ERR_ARG (found after the start E-step; the memberships are then valid only when pi_init is
+ * NULL); K != the K of the current parameters or a call between gmm_mstep and gmm_constants -> GMM_ERR_STATE; a failed
+ * collective -> GMM_ERR_NCCL.
+ * Device memory: rho [S][K] floats, the work units (about n_local / E + S), the CTA and sample indices, the partial records
+ * ((CTAs + S) x (K + 2) doubles at most) and the masses [S][K + 1] doubles, with pinned mirrors; reserved on first use,
+ * grown with S, K and the shard, freed by gmm_destroy.                                                                */
+int  gmm_em_multisample(gmm_ctx*, int K, int S, const long long* offsets /* [S+1] global */,
+                        const double* pi_init /* [S][K] or NULL */, int min_iters, int max_iters, float epsilon,
+                        double* pi_out /* [S][K] or NULL */, double* n_out /* [S] or NULL */,
+                        float* loglik_out, float* logliks_out /* [max_iters + 1] or NULL */, int* iters_out);
+
+/* Since the last reset: out[0] reweight and finishing kernels ms (0 with option "profile" = 0), out[1] host ms of the
+ * finalisations and the pi / rho updates, out[2] wall ms inside gmm_em_multisample.                                  */
+int  gmm_get_multisample_profile(gmm_ctx*, double out[3], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
