@@ -40,6 +40,7 @@
 #include "kernels_vb.cuh"
 #include "kernels_combine.cuh"
 #include "kernels_multisample.cuh"
+#include "kernels_modes.cuh"
 
 namespace gmm {
 
@@ -393,6 +394,29 @@ struct MultisampleBuffers {
     double host_ms = 0, wall_ms = 0;            // gmm_get_multisample_profile
 };
 
+// gmm_modes / gmm_mode_labels: the component records with inv_sigma and the float centre behind them, the mode list, the
+// state of a chunk's points (kernels_modes.cuh), the active lists of the rounds and, per slot of gmm_score's two, a chunk's
+// outputs [labels int | iters int | logp float | endpoints float [D]] and their pinned mirror; reserved on first use.
+struct ModesBuffers {
+    long long cap = 0;                          // points of the state buffers and the slots
+    DeviceArray<float> d_rec;
+    PinnedArray<float> h_rec;
+    const float* d_inv_sigma = nullptr;         // inside d_rec
+    const float* d_centre = nullptr;
+    DeviceArray<float> d_modes;                 // [max(n_modes, Kmax)][DP] (gmm_modes: its starts)
+    DeviceArray<float> d_x;                     // [cap][DP]
+    DeviceArray<int> d_it, d_st;                // [cap]
+    DeviceArray<int> d_act[2];                  // [cap] active lists of consecutive rounds
+    DeviceArray<int> d_bcount;                  // block counts / offsets of the compaction, then the active count
+    PinnedArray<int> h_count;
+    Event t0, t1;                               // around gmm_modes' kernels
+    DeviceArray<char> d_out[2];
+    PinnedArray<char> h_out[2];
+    double kernel_ms = 0, modes_wall_ms = 0, labels_wall_ms = 0;   // gmm_get_modes_profile
+    long long event_iters = 0;
+    static size_t out_bytes(long long cap, int D) { return (size_t)cap * (12 + 4 * (size_t)D); }
+};
+
 }  // namespace gmm
 
 using namespace gmm;
@@ -485,6 +509,7 @@ struct gmm_ctx {
     double vb_final_ms = 0, vb_wall_ms = 0;   // gmm_get_vb_profile
     CombineBuffers comb;         // gmm_combine / gmm_combine_labels: allocated on first use
     MultisampleBuffers msamp;    // gmm_em_multisample: allocated on first use
+    ModesBuffers modes;          // gmm_modes / gmm_mode_labels: allocated on first use
 };
 
 namespace gmm {
@@ -3214,6 +3239,409 @@ int gmm_get_condition_stats_profile(gmm_ctx* c, double out[4], int reset) {
     StatsProfile& t = c->sstats.cond_prof;
     out[0] = t.kernel_ms; out[1] = t.wall_ms; out[2] = (double)t.m_tensor; out[3] = (double)t.m_simt;
     if (reset) t = StatsProfile();
+    return GMM_OK;
+}
+
+// ---- modes of the mixture ---------------------------------------------------------------------------------------------
+// The host side of gmm_modes / gmm_mode_labels (kernels_modes.cuh): the parameters in double, their float records, the
+// rounds of mode_iter_kernel with the compaction between them, and the labels.
+struct ModeParams {
+    int D = 0, DP = 0, Kc = 0, Kp = 0;          // dimensions, padded dimensions, components with pi > 0, padded record count
+    std::vector<int> comp;                      // [Kc] the component of each record
+    std::vector<double> mu, S, lc;              // [Kc][D] mu - c, [Kc][D][D] (P + P^T) / 2, [Kc] constant + ln pi
+    double centre[GMM_MAX_DIMENSIONS] = {0}, inv_sigma[GMM_MAX_DIMENSIONS] = {0};
+};
+
+static bool chol_spd(const double* S, int D) {
+    double L[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS];
+    for (int j = 0; j < D; j++)
+        for (int i = j; i < D; i++) {
+            double t = S[i * D + j];
+            for (int k = 0; k < j; k++) t -= L[i * D + k] * L[j * D + k];
+            if (i == j) {
+                if (!(t > 0.0) || !std::isfinite(t)) return false;
+                L[j * D + j] = std::sqrt(t);
+            } else {
+                L[i * D + j] = t / L[j * D + j];
+            }
+        }
+    return true;
+}
+
+// ln p at y (relative to the centre, double) and, with H, the Hessian of ln p there [D][D].
+static double mode_logp(const ModeParams& mp, const double* y, double* H) {
+    const int D = mp.D;
+    std::vector<double> l(mp.Kc), v((size_t)mp.Kc * D);
+    double mx = -INFINITY;
+    for (int k = 0; k < mp.Kc; k++) {
+        double q = 0;
+        for (int i = 0; i < D; i++) {
+            double t = 0;
+            for (int j = 0; j < D; j++) t += mp.S[((size_t)k * D + i) * D + j] * (y[j] - mp.mu[(size_t)k * D + j]);
+            v[(size_t)k * D + i] = t;
+            q += (y[i] - mp.mu[(size_t)k * D + i]) * t;
+        }
+        l[k] = mp.lc[k] - 0.5 * q;
+        mx = std::max(mx, l[k]);
+    }
+    double s = 0;
+    for (int k = 0; k < mp.Kc; k++) s += std::exp(l[k] - mx);
+    const double lp = mx + std::log(s);
+    if (H) {
+        double g[GMM_MAX_DIMENSIONS] = {0};
+        for (int i = 0; i < D * D; i++) H[i] = 0;
+        for (int k = 0; k < mp.Kc; k++) {
+            const double r = std::exp(l[k] - lp);
+            const double* vk = &v[(size_t)k * D];
+            for (int i = 0; i < D; i++) {
+                g[i] -= r * vk[i];
+                for (int j = 0; j < D; j++) H[i * D + j] += r * (vk[i] * vk[j] - mp.S[((size_t)k * D + i) * D + j]);
+            }
+        }
+        for (int i = 0; i < D; i++)
+            for (int j = 0; j < D; j++) H[i * D + j] -= g[i] * g[j];
+    }
+    return lp;
+}
+
+static double mode_rho(const ModeParams& mp, const double* a, const double* b) {
+    double r = 0;
+    for (int d = 0; d < mp.D; d++) r = std::max(r, std::fabs(a[d] - b[d]) * mp.inv_sigma[d]);
+    return r;
+}
+
+// The checks shared by both calls, in gmm.h's order.
+static int mode_check(gmm_ctx* c, int K, int max_iter, double* tol, double* merge_tol, const char* who) {
+    if (int rc = check_K(c, K, who)) return rc;
+    if (max_iter < 1) return fail(GMM_ERR_ARG, std::string(who) + ": max_iter must be at least 1");
+    if (!std::isfinite(*tol) || !std::isfinite(*merge_tol)) return fail(GMM_ERR_ARG, std::string(who) + ": tol and merge_tol must be finite");
+    if (*tol < 0) *tol = 1e-5;
+    if (*merge_tol < 0) *merge_tol = 1e-2;
+    if (*merge_tol < 10 * *tol) return fail(GMM_ERR_ARG, std::string(who) + ": merge_tol must be at least 10 tol");
+    return GMM_OK;
+}
+
+// The parameters of the current set in double, their records uploaded (with inv_sigma and the float centre behind them).
+static int mode_params(gmm_ctx* c, int K, const char* who, ModeParams& mp) {
+    const clusters_t& h = c->host;
+    const int D = c->D, DP = (D + 3) & ~3;
+    mp.D = D; mp.DP = DP;
+    mp.comp.clear();
+    for (int k = 0; k < K; k++)
+        if (h.pi[k] > 0.0f) mp.comp.push_back(k);
+    mp.Kc = (int)mp.comp.size();
+    if (mp.Kc == 0) return fail(GMM_ERR_STATE, std::string(who) + ": no component has pi > 0");
+    mp.Kp = (mp.Kc + kModeChunk - 1) / kModeChunk * kModeChunk;
+    double cd[GMM_MAX_DIMENSIONS] = {0}, var[GMM_MAX_DIMENSIONS] = {0};
+    for (int k : mp.comp)
+        for (int d = 0; d < D; d++) {
+            cd[d] += (double)h.pi[k] * h.means[(size_t)k * D + d];
+            var[d] += (double)h.pi[k] * h.R[((size_t)k * D + d) * D + d];
+        }
+    for (int d = 0; d < D; d++) {
+        mp.centre[d] = (double)(float)cd[d];
+        const double sg = std::sqrt(var[d]);
+        if (!(sg > 0.0) || !std::isfinite(sg)) return fail(GMM_ERR_STATE, std::string(who) + ": a dimension has no positive spread");
+        mp.inv_sigma[d] = 1.0 / sg;
+    }
+    mp.mu.assign((size_t)mp.Kc * D, 0.0); mp.S.assign((size_t)mp.Kc * D * D, 0.0); mp.lc.assign(mp.Kc, 0.0);
+    for (int i = 0; i < mp.Kc; i++) {
+        const int k = mp.comp[i];
+        for (int d = 0; d < D; d++) mp.mu[(size_t)i * D + d] = (double)h.means[(size_t)k * D + d] - mp.centre[d];
+        const float* P = h.Rinv + (size_t)k * D * D;
+        for (int a = 0; a < D; a++)
+            for (int b = 0; b < D; b++) mp.S[((size_t)i * D + a) * D + b] = 0.5 * ((double)P[a * D + b] + (double)P[b * D + a]);
+        if (!chol_spd(&mp.S[(size_t)i * D * D], D))
+            return fail(GMM_ERR_STATE, std::string(who) + ": the inverse covariance of component " + std::to_string(k) + " is not positive definite");
+        mp.lc[i] = (double)h.constant[k] + std::log((double)h.pi[k]);
+    }
+    ModesBuffers& b = c->modes;
+    const int REC = mode_rec_floats(DP);
+    const size_t nrec = (size_t)c->Kmax / kModeChunk * kModeChunk + kModeChunk;
+    if (int rc = b.d_rec.reserve(nrec * REC + 2 * GMM_MAX_DIMENSIONS)) return rc;
+    if (int rc = b.h_rec.reserve(nrec * REC + 2 * GMM_MAX_DIMENSIONS)) return rc;
+    CUDA_TRY(cudaStreamSynchronize(c->stream));             // the pinned records of an earlier call have been copied
+    float* r = b.h_rec;
+    std::memset(r, 0, sizeof(float) * ((size_t)mp.Kp * REC + 2 * GMM_MAX_DIMENSIONS));
+    for (int i = 0; i < mp.Kp; i++) {
+        float* p = r + (size_t)i * REC;
+        if (i >= mp.Kc) { p[DP + DP * DP] = -INFINITY; continue; }
+        for (int d = 0; d < D; d++) p[d] = (float)mp.mu[(size_t)i * D + d];
+        for (int a = 0; a < D; a++)
+            for (int bb = 0; bb < D; bb++) p[DP + a * DP + bb] = (float)mp.S[((size_t)i * D + a) * D + bb];
+        p[DP + DP * DP] = (float)mp.lc[i];
+    }
+    float* aux = r + (size_t)mp.Kp * REC;                    // inv_sigma [32] (0 beyond D), then the float centre [32]
+    for (int d = 0; d < D; d++) { aux[d] = (float)mp.inv_sigma[d]; aux[GMM_MAX_DIMENSIONS + d] = (float)mp.centre[d]; }
+    CUDA_TRY(cudaMemcpyAsync(b.d_rec, b.h_rec, sizeof(float) * ((size_t)mp.Kp * REC + 2 * GMM_MAX_DIMENSIONS), cudaMemcpyHostToDevice,
+                             c->stream));
+    b.d_inv_sigma = b.d_rec + (size_t)mp.Kp * REC;
+    b.d_centre = b.d_inv_sigma + GMM_MAX_DIMENSIONS;
+    return GMM_OK;
+}
+
+// State buffers for m points and, per slot, the outputs of a chunk of m events.
+static int mode_buffers(gmm_ctx* c, long long m) {
+    ModesBuffers& b = c->modes;
+    const long long want = std::max(b.cap, m);
+    const int DP = (c->D + 3) & ~3;
+    if (int rc = b.d_x.reserve((size_t)want * DP)) return rc;
+    if (int rc = b.d_it.reserve(want)) return rc;
+    if (int rc = b.d_st.reserve(want)) return rc;
+    for (int s = 0; s < 2; s++) {
+        if (int rc = b.d_act[s].reserve(want)) return rc;
+        if (int rc = b.d_out[s].reserve(ModesBuffers::out_bytes(want, c->D))) return rc;
+        if (int rc = b.h_out[s].reserve(ModesBuffers::out_bytes(want, c->D))) return rc;
+    }
+    if (int rc = b.d_bcount.reserve(want / kModeScanThreads + 2)) return rc;
+    if (int rc = b.h_count.reserve(1)) return rc;
+    if (int rc = b.d_modes.reserve((size_t)std::max(c->Kmax, 1) * DP)) return rc;
+    b.cap = want;
+    return GMM_OK;
+}
+
+// Active points of idx[0 .. m) (idx NULL: 0 .. m) -> out[0 .. *na), in order.
+static int mode_compact(gmm_ctx* c, const int* idx, int m, int* out, int* na) {
+    ModesBuffers& b = c->modes;
+    const int nb = (m + kModeScanThreads - 1) / kModeScanThreads;
+    int* count = b.d_bcount + nb;
+    if (nb > 0) {
+        mode_count_kernel<<<nb, kModeScanThreads, 0, c->stream>>>(idx, m, b.d_st, b.d_bcount);
+        mode_scan_kernel<<<1, kModeScanThreads, 0, c->stream>>>(b.d_bcount, nb, count);
+        mode_scatter_kernel<<<nb, kModeScanThreads, 0, c->stream>>>(idx, m, b.d_st, b.d_bcount, out);
+    } else {
+        CUDA_TRY(cudaMemsetAsync(count, 0, sizeof(int), c->stream));
+    }
+    CUDA_TRY(cudaGetLastError());
+    CUDA_TRY(cudaMemcpyAsync(b.h_count, count, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    CUDA_TRY(cudaStreamSynchronize(c->stream));
+    *na = *b.h_count;
+    return GMM_OK;
+}
+
+extern "C++" {
+template <int DP>
+static int mode_iter_launch(gmm_ctx* c, const ModeParams& mp, const int* act, int na, int max_iter, float tol) {
+    ModesBuffers& b = c->modes;
+    mode_iter_kernel<DP><<<(na + kModeTile - 1) / kModeTile, kModeThreads, mode_iter_smem(DP), c->stream>>>(
+        mp.D, mp.Kp, b.d_rec, b.d_inv_sigma, act, na, b.d_x, b.d_it, b.d_st, max_iter, tol, kModeRound);
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+}  // extern "C++"
+#define GMM_MODE_DISPATCH(DP, CALL)                                                                                        \
+    switch (DP) {                                                                                                          \
+        case 4: CALL(4); case 8: CALL(8); case 12: CALL(12); case 16: CALL(16);                                            \
+        case 20: CALL(20); case 24: CALL(24); case 28: CALL(28); case 32: CALL(32);                                        \
+        default: return fail(GMM_ERR_ARG, "unsupported dimension count");                                                  \
+    }
+
+// The shared-memory allowance of the iteration instance for this D, once per call (before its first round).
+extern "C++" {
+template <int DP>
+static int mode_iter_prepare() {
+    CUDA_TRY(cudaFuncSetAttribute(mode_iter_kernel<DP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)mode_iter_smem(DP)));
+    return GMM_OK;
+}
+}  // extern "C++"
+static int mode_prepare(int DP) {
+#define GMM_CALL(d) return mode_iter_prepare<d>()
+    GMM_MODE_DISPATCH(DP, GMM_CALL)
+#undef GMM_CALL
+}
+
+// Rounds over the m initialised points of the state buffers until none is active.
+static int mode_rounds(gmm_ctx* c, const ModeParams& mp, int m, int max_iter, float tol) {
+    ModesBuffers& b = c->modes;
+    int* cur = b.d_act[0];
+    int* nxt = b.d_act[1];
+    int na = 0;
+    if (int rc = mode_compact(c, nullptr, m, cur, &na)) return rc;
+    while (na > 0) {
+#define GMM_CALL(d) return mode_iter_launch<d>(c, mp, cur, na, max_iter, tol)
+        auto iter = [&]() -> int { GMM_MODE_DISPATCH(mp.DP, GMM_CALL) };
+#undef GMM_CALL
+        if (int rc = iter()) return rc;
+        if (int rc = mode_compact(c, cur, na, nxt, &na)) return rc;
+        std::swap(cur, nxt);
+    }
+    return GMM_OK;
+}
+
+extern "C++" {
+template <int DP>
+static int mode_label_launch(gmm_ctx* c, const ModeParams& mp, int m, int n_modes, float merge_tol, int* labels, float* endpoints,
+                             float* logp) {
+    ModesBuffers& b = c->modes;
+    if (m <= 0) return GMM_OK;
+    mode_label_kernel<DP><<<(m + kModeLabelThreads - 1) / kModeLabelThreads, kModeLabelThreads, 0, c->stream>>>(
+        m, mp.D, mp.Kp, b.d_rec, b.d_inv_sigma, b.d_modes, n_modes, merge_tol, b.d_x, b.d_st, b.d_centre, labels, endpoints, logp);
+    CUDA_TRY(cudaGetLastError());
+    return GMM_OK;
+}
+}  // extern "C++"
+
+int gmm_modes(gmm_ctx* c, int K, int max_iter, double tol, double merge_tol, int* n_modes_out, double* modes_out, double* mode_logp_out,
+              int* comp_mode_out, int* is_max_out, int* iters_out) {
+    if (int rc = mode_check(c, K, max_iter, &tol, &merge_tol, "gmm_modes")) return rc;
+    if (!n_modes_out || !modes_out || !comp_mode_out) return fail(GMM_ERR_ARG, "gmm_modes: n_modes_out, modes_out and comp_mode_out are required");
+    if (int rc = check_fitted(c, K, "gmm_modes")) return rc;
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    ModesBuffers& b = c->modes;
+    ModeParams mp;
+    int rc = mode_params(c, K, "gmm_modes", mp);
+    if (rc == GMM_OK) rc = b.t0.create(cudaEventDefault);
+    if (rc == GMM_OK) rc = b.t1.create(cudaEventDefault);
+    if (rc == GMM_OK) rc = mode_prepare(mp.DP);
+    if (rc == GMM_OK) rc = mode_buffers(c, mp.Kc);
+    const int D = mp.D, DP = mp.DP, n = mp.Kc;
+    std::vector<float> start((size_t)n * DP, 0.0f), x((size_t)n * DP);
+    std::vector<int> it(n), st(n);
+    if (rc == GMM_OK) {
+        for (int i = 0; i < n; i++)
+            for (int d = 0; d < D; d++) start[(size_t)i * DP + d] = (float)mp.mu[(size_t)i * D + d];
+        rc = [&]() -> int {
+            CUDA_TRY(cudaMemcpyAsync(b.d_modes, start.data(), sizeof(float) * start.size(), cudaMemcpyHostToDevice, c->stream));
+            CUDA_TRY(cudaEventRecord(b.t0, c->stream));
+            mode_init_kernel<<<(n + 255) / 256, 256, 0, c->stream>>>(b.d_modes, DP, 1, n, DP, DP, nullptr, b.d_x, b.d_it, b.d_st);
+            CUDA_TRY(cudaGetLastError());
+            if (int r = mode_rounds(c, mp, n, max_iter, (float)tol)) return r;
+            CUDA_TRY(cudaEventRecord(b.t1, c->stream));
+            CUDA_TRY(cudaMemcpyAsync(x.data(), b.d_x, sizeof(float) * x.size(), cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(cudaMemcpyAsync(it.data(), b.d_it, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(cudaMemcpyAsync(st.data(), b.d_st, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
+            CUDA_TRY(cudaStreamSynchronize(c->stream));
+            float ms = 0;
+            if (cudaEventElapsedTime(&ms, b.t0, b.t1) == cudaSuccess) b.kernel_ms += ms;
+            return GMM_OK;
+        }();
+    }
+    rc = drain_streams(c, rc, "gmm_modes");
+    if (rc == GMM_OK) {
+        // dedup in component order: an endpoint joins the first mode within merge_tol, else starts one
+        std::vector<double> pos;
+        for (int k = 0; k < K; k++) { comp_mode_out[k] = -1; if (iters_out) iters_out[k] = 0; }
+        int nm = 0;
+        for (int i = 0; i < n; i++) {
+            const int k = mp.comp[i];
+            if (iters_out) iters_out[k] = it[i];
+            b.event_iters += it[i];
+            if (st[i] != kModeConverged) continue;
+            double y[GMM_MAX_DIMENSIONS];
+            for (int d = 0; d < D; d++) y[d] = (double)x[(size_t)i * DP + d];
+            int j = 0;
+            while (j < nm && !(mode_rho(mp, y, &pos[(size_t)j * D]) <= merge_tol)) j++;
+            if (j == nm) { pos.insert(pos.end(), y, y + D); nm++; }
+            comp_mode_out[k] = j;
+        }
+        for (int j = 0; j < nm; j++) {
+            const double* y = &pos[(size_t)j * D];
+            double H[GMM_MAX_DIMENSIONS * GMM_MAX_DIMENSIONS];
+            const double lp = mode_logp(mp, y, H);
+            for (int d = 0; d < D * D; d++) H[d] = -H[d];
+            if (mode_logp_out) mode_logp_out[j] = lp;
+            if (is_max_out) is_max_out[j] = chol_spd(H, D) ? 1 : 0;
+            for (int d = 0; d < D; d++) modes_out[(size_t)j * D + d] = mp.centre[d] + y[d];
+        }
+        *n_modes_out = nm;
+    }
+    b.modes_wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+
+int gmm_mode_labels(gmm_ctx* c, int K, const float* events_aos, long long n, const double* modes, int n_modes, int max_iter, double tol,
+                    double merge_tol, int* labels, float* endpoints, float* logp_end, int* iters, long long* unmatched_out,
+                    long long* unconverged_out) {
+    if (int rc = mode_check(c, K, max_iter, &tol, &merge_tol, "gmm_mode_labels")) return rc;
+    if (n < 0) return fail(GMM_ERR_ARG, "gmm_mode_labels: n < 0");
+    if (!events_aos && n != c->n) return fail(GMM_ERR_ARG, "gmm_mode_labels: the shard (events_aos NULL) needs n = n_local");
+    if (!modes || n_modes < 1) return fail(GMM_ERR_ARG, "gmm_mode_labels: the mode list must hold at least one mode");
+    if (n > 0 && !labels) return fail(GMM_ERR_ARG, "gmm_mode_labels: labels is required");
+    if (int rc = check_fitted(c, K, "gmm_mode_labels")) return rc;
+    CUDA_TRY(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    ModesBuffers& b = c->modes;
+    ScoreBuffers& s = c->score;
+    ModeParams mp;
+    long long unmatched = 0, unconverged = 0;
+    int rc = mode_params(c, K, "gmm_mode_labels", mp);
+    const int D = mp.D, DP = mp.DP;
+    if (rc == GMM_OK && n > 0) {
+        rc = score_buffers(c);
+        if (rc == GMM_OK) rc = mode_prepare(DP);
+        if (rc == GMM_OK) rc = mode_buffers(c, std::min(n, c->score_chunk));
+        if (rc == GMM_OK) rc = b.d_modes.reserve((size_t)std::max(n_modes, c->Kmax) * DP);
+        std::vector<float> mf((size_t)n_modes * DP, 0.0f);
+        for (int j = 0; j < n_modes; j++)
+            for (int d = 0; d < D; d++) mf[(size_t)j * DP + d] = (float)(modes[(size_t)j * D + d] - mp.centre[d]);
+        if (rc == GMM_OK) rc = [&]() -> int {
+            CUDA_TRY(cudaMemcpyAsync(b.d_modes, mf.data(), sizeof(float) * mf.size(), cudaMemcpyHostToDevice, c->stream));
+            CUDA_TRY(cudaStreamSynchronize(c->stream));
+            return GMM_OK;
+        }();
+        const long long cap = b.cap;
+        auto out_lab = [&](char* base) { return reinterpret_cast<int*>(base); };
+        auto out_it = [&](char* base) { return reinterpret_cast<int*>(base + 4 * (size_t)cap); };
+        auto out_lp = [&](char* base) { return reinterpret_cast<float*>(base + 8 * (size_t)cap); };
+        auto out_ep = [&](char* base) { return reinterpret_cast<float*>(base + 12 * (size_t)cap); };
+        auto launch = [&](int sl, long long e0, int m) -> int {
+            const float* src = events_aos ? (const float*)s.d_in[sl] : c->d_x_aos + (size_t)e0 * D;
+            CUDA_TRY(cudaEventRecord(s.t0[sl], c->stream));
+            mode_init_kernel<<<(m + 255) / 256, 256, 0, c->stream>>>(src, D, 1, m, D, DP, b.d_centre, b.d_x, b.d_it, b.d_st);
+            CUDA_TRY(cudaGetLastError());
+            if (int r = mode_rounds(c, mp, m, max_iter, (float)tol)) return r;
+            char* o = b.d_out[sl];
+#define GMM_CALL(d) return mode_label_launch<d>(c, mp, m, n_modes, (float)merge_tol, out_lab(o), endpoints ? out_ep(o) : nullptr, \
+                                                logp_end ? out_lp(o) : nullptr)
+            auto lab = [&]() -> int { GMM_MODE_DISPATCH(DP, GMM_CALL) };
+#undef GMM_CALL
+            if (int r = lab()) return r;
+            CUDA_TRY(cudaMemcpyAsync(out_it(o), b.d_it, sizeof(int) * (size_t)m, cudaMemcpyDeviceToDevice, c->stream));
+            CUDA_TRY(cudaEventRecord(s.t1[sl], c->stream));
+            return GMM_OK;
+        };
+        auto fetch = [&](int sl, int m, cudaStream_t stm) -> int {
+            char *dv = b.d_out[sl], *hv = b.h_out[sl];
+            CUDA_TRY(cudaMemcpyAsync(out_lab(hv), out_lab(dv), sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, stm));
+            CUDA_TRY(cudaMemcpyAsync(out_it(hv), out_it(dv), sizeof(int) * (size_t)m, cudaMemcpyDeviceToHost, stm));
+            if (logp_end) CUDA_TRY(cudaMemcpyAsync(out_lp(hv), out_lp(dv), sizeof(float) * (size_t)m, cudaMemcpyDeviceToHost, stm));
+            if (endpoints)
+                CUDA_TRY(cudaMemcpyAsync(out_ep(hv), out_ep(dv), sizeof(float) * (size_t)m * D, cudaMemcpyDeviceToHost, stm));
+            return GMM_OK;
+        };
+        auto hand_over = [&](int sl, long long e0, int m) -> int {
+            char* hv = b.h_out[sl];
+            const int* lab = out_lab(hv);
+            const int* itv = out_it(hv);
+            std::memcpy(labels + e0, lab, sizeof(int) * (size_t)m);
+            for (int i = 0; i < m; i++) {
+                unmatched += lab[i] == -2;
+                unconverged += lab[i] == -1;
+                b.event_iters += itv[i];
+            }
+            if (iters) std::memcpy(iters + e0, itv, sizeof(int) * (size_t)m);
+            if (logp_end) std::memcpy(logp_end + e0, out_lp(hv), sizeof(float) * (size_t)m);
+            if (endpoints) std::memcpy(endpoints + (size_t)e0 * D, out_ep(hv), sizeof(float) * (size_t)m * D);
+            return GMM_OK;
+        };
+        if (rc == GMM_OK) rc = stream_chunks(c, n, events_aos, D, &b.kernel_ms, launch, fetch, hand_over);
+    }
+    rc = drain_streams(c, rc, "gmm_mode_labels");
+    if (rc == GMM_OK) {
+        if (unmatched_out) *unmatched_out = unmatched;
+        if (unconverged_out) *unconverged_out = unconverged;
+    }
+    b.labels_wall_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    return rc;
+}
+#undef GMM_MODE_DISPATCH
+
+int gmm_get_modes_profile(gmm_ctx* c, double out[4], int reset) {
+    if (!c || !out) return fail(GMM_ERR_ARG, "gmm_get_modes_profile: bad argument");
+    ModesBuffers& b = c->modes;
+    out[0] = b.kernel_ms; out[1] = b.modes_wall_ms; out[2] = b.labels_wall_ms; out[3] = (double)b.event_iters;
+    if (reset) { b.kernel_ms = b.modes_wall_ms = b.labels_wall_ms = 0; b.event_iters = 0; }
     return GMM_OK;
 }
 

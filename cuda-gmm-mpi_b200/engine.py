@@ -142,6 +142,12 @@ def load_library():
     L.gmm_em_multisample.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_float, C.c_void_p,
                                      C.c_void_p, _FP, C.c_void_p, _IP]
     L.gmm_get_multisample_profile.argtypes = [C.c_void_p, _DP, C.c_int]
+    L.gmm_modes.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_double, C.c_double, _IP, C.c_void_p, C.c_void_p, C.c_void_p,
+                            C.c_void_p, C.c_void_p]
+    L.gmm_mode_labels.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_longlong, C.c_void_p, C.c_int, C.c_int, C.c_double,
+                                  C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_longlong),
+                                  C.POINTER(C.c_longlong)]
+    L.gmm_get_modes_profile.argtypes = [C.c_void_p, _DP, C.c_int]
     L.gmm_host_pool_selftest.argtypes = [C.c_int, C.c_int, C.c_int]
     L.gmm_host_invert.argtypes = [_FP, C.c_int, _FP, C.c_int]
     L.gmm_stats_len.argtypes = [C.c_int, C.c_int]
@@ -601,6 +607,47 @@ class Engine:
         out = (C.c_double * 3)()
         _check(self.lib.gmm_get_multisample_profile(self.h, out, int(reset)))
         return dict(kernel_ms=out[0], host_ms=out[1], wall_ms=out[2])
+
+    def modes(self, K, max_iter=500, tol=-1.0, merge_tol=-1.0):
+        """The modes of the current K-component mixture reached from its means (gmm_modes).  Returns dict(modes [M][D]
+        float64, logp [M], is_max bool [M], comp_mode int32 [K] (-1: pi = 0 or unconverged), iters int32 [K])."""
+        modes = np.zeros((K, self.D), np.float64)
+        lp = np.zeros(K, np.float64)
+        cm, ismax, it = np.zeros(K, np.int32), np.zeros(K, np.int32), np.zeros(K, np.int32)
+        nm = C.c_int()
+        _check(self.lib.gmm_modes(self.h, K, int(max_iter), float(tol), float(merge_tol), C.byref(nm), modes.ctypes.data, lp.ctypes.data,
+                                  cm.ctypes.data, ismax.ctypes.data, it.ctypes.data))
+        m = nm.value
+        return dict(modes=modes[:m], logp=lp[:m], is_max=ismax[:m].astype(bool), comp_mode=cm, iters=it)
+
+    def mode_labels(self, K, modes, events=None, max_iter=500, tol=-1.0, merge_tol=-1.0, endpoints=False, logp=False, iters=False):
+        """Each event's ascent (gmm_mode_labels) against the mode list modes [M][D]; events [n][D], or None for the
+        context's own shard.  Returns dict(labels int32 [n] (-1 unconverged, -2 near no listed mode), endpoints [n][D]
+        float32, logp [n] float32, iters int32 [n] (None when not asked for), unmatched, unconverged)."""
+        md = np.ascontiguousarray(modes, np.float64).reshape(-1, self.D)
+        if events is None:
+            ev, n = None, self.n
+        else:
+            ev = np.ascontiguousarray(events, np.float32)
+            if ev.ndim != 2 or ev.shape[1] != self.D:
+                raise ValueError(f"events must be [n][{self.D}], got {ev.shape}")
+            n = ev.shape[0]
+        lab = np.empty(max(n, 1), np.int32)
+        ep = np.empty((max(n, 1), self.D), np.float32) if endpoints else None
+        lp = np.empty(max(n, 1), np.float32) if logp else None
+        it = np.empty(max(n, 1), np.int32) if iters else None
+        um, uc = C.c_longlong(), C.c_longlong()
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        _check(self.lib.gmm_mode_labels(self.h, K, ptr(ev), n, md.ctypes.data if md.size else None, md.shape[0], int(max_iter),
+                                        float(tol), float(merge_tol), lab.ctypes.data, ptr(ep), ptr(lp), ptr(it), C.byref(um),
+                                        C.byref(uc)))
+        cut = lambda a: a[:n] if a is not None else None  # noqa: E731
+        return dict(labels=lab[:n], endpoints=cut(ep), logp=cut(lp), iters=cut(it), unmatched=um.value, unconverged=uc.value)
+
+    def modes_profile(self, reset=False):
+        out = (C.c_double * 4)()
+        _check(self.lib.gmm_get_modes_profile(self.h, out, int(reset)))
+        return dict(kernel_ms=out[0], modes_wall_ms=out[1], labels_wall_ms=out[2], event_iterations=int(out[3]))
 
     def comm_rank(self):
         r, n = C.c_int(), C.c_int()

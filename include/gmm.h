@@ -646,6 +646,73 @@ int  gmm_em_multisample(gmm_ctx*, int K, int S, const long long* offsets /* [S+1
  * finalisations and the pi / rho updates, out[2] wall ms inside gmm_em_multisample.                                  */
 int  gmm_get_multisample_profile(gmm_ctx*, double out[3], int reset);
 
+/* Modal clustering of a fitted mixture (Carreira-Perpinan, TPAMI 2000; Li, Ray and Lindsay, JMLR 2007): the modes of the
+ * density p(x) = sum_k pi_k N(x | mu_k, R_k) and the mode each event's hill-climb reaches (its basin of attraction).  A
+ * population is a hill of p: several components may cover one hill, and a basin may split a component that straddles two.
+ * Parameters: the set the next gmm_estep(ctx, K) would use (float means, Rinv = P, constant, pi of the host copy).
+ * Components with pi = 0 take no part.  The host derives, in double, then rounds to float: the centre c = sum_k pi_k mu_k
+ * (rounded to float first; every device coordinate is relative to it), mu~_k = mu_k - c, S_k = (P_k + P_k^T) / 2, the
+ * logit constant constant_k + ln pi_k and sigma_d = sqrt(sum_k pi_k R_k[d][d]).
+ * Iteration (step form of the fixed point; csrc/kernels_modes.cuh, FP32 on sm_90a): for a point x,
+ *   dx_k = x - mu~_k,  l_k = const_k - dx_k^T S_k dx_k / 2,  r_k = exp(l_k - ln sum_j exp l_j)  (online log-sum-exp),
+ *   g = sum_k r_k S_k (-dx_k)  (the gradient of ln p, formed from each dx_k, in increasing k),
+ *   A = sum_k r_k S_k,  delta = A^-1 g by a Cholesky factorisation,  x <- x + delta.
+ * This is MEM's x <- A^-1 sum_k r_k S_k mu~_k and keeps its monotone ascent.  A fixed point is g = 0 for any nonsingular
+ * A, so A's rounding changes only the speed of convergence, never a mode.  A point stops after the first iteration in
+ * which every |delta_d| < max(tol sigma_d, 2^-22 |x_d|), x relative to c before the step (converged): beyond about
+ * tol 2^22 spreads from the centre a float coordinate cannot resolve tol sigma_d, and the second term stops a point that
+ * has reached the float resolution there instead of letting it hop between neighbouring floats until max_iter; one that has not stopped after max_iter iterations, or whose A is not
+ * positive definite in float, is unconverged.  A point with a coordinate that is not finite runs no iteration.
+ * Distance: rho(a, b) = max_d |a_d - b_d| / sigma_d.  Each point's arithmetic is fixed: the same bits whatever its CTA,
+ * chunk, round or source, and across calls.
+ * gmm_modes runs the iteration from every mean mu~_k with pi_k > 0 and deduplicates the endpoints in component order on the
+ * host, in double: an endpoint joins the first mode with rho <= merge_tol, else starts a new mode at that endpoint.
+ *   n_modes_out    the number of modes found
+ *   modes_out      [K][D] the modes in absolute coordinates (c added back in double); the first *n_modes_out rows are set
+ *   mode_logp_out  [K] ln p at each mode, in double, or NULL
+ *   comp_mode_out  [K] the mode component k reaches; -1 for pi_k = 0 or an unconverged start
+ *   is_max_out     [K] 1 when the double-precision Hessian of ln p at the mode is negative definite, or NULL.  A mean can sit
+ *                  exactly on a saddle in a symmetric mixture, so this is reported rather than assumed
+ *   iters_out      [K] iterations run from each mean (0 for pi_k = 0), or NULL
+ * Not collective: every rank computes the same bits.
+ * gmm_mode_labels runs the iteration from every event: events_aos [n][D] rows streamed in chunks of option "score_chunk",
+ * or events_aos = NULL for the context's own shard (n must equal n_local), read in place from its device copy.
+ *   labels       [n] the listed mode of smallest rho <= merge_tol from a converged endpoint, ties to the lower index; -2 for a
+ *                converged event near no listed mode; -1 for an unconverged event or one that is not finite
+ *   endpoints    [n][D] where each event's ascent stopped (absolute float coordinates: the relative endpoint plus the float
+ *                centre, rounded once); NaN for an event that is not finite; or NULL
+ *   logp_end     [n] ln p at the endpoint (float; a pass of its own over the records, not the iteration's last value);
+ *                NaN for an event that is not finite; or NULL
+ *   iters        [n] iterations run, or NULL
+ *   unmatched_out / unconverged_out   the counts of labels -2 / -1, or NULL
+ * A mixture can have modes that no mean climbs to (three equal isotropic components at the vertices of an equilateral
+ * triangle have a fourth mode at the centroid for a range of spreads, Carreira-Perpinan and Williams 2003).  Events in such
+ * a basin get -2; their endpoints show where they went (gmm_modes' list plus those endpoints, deduplicated, is a fuller
+ * list).  Labelling by component instead: map the -1 entries of comp_mode to any group, then
+ * gmm_combine_labels(ctx, K, comp_mode, n_modes, ...) labels each event by the mode of its most likely component.  That
+ * differs from the basins where a component straddles two hills, and for events in a basin no mean reaches.
+ * tol < 0 selects 1e-5, merge_tol < 0 selects 1e-2.  Weights (gmm_set_weights) are ignored.  Nothing of the EM state
+ * changes: memberships, statistics, log-likelihood and every other profile stay as they are.
+ * Errors: K outside [1, Kmax], n < 0, max_iter < 1, tol or merge_tol not finite, merge_tol < 10 tol, a mode list that is
+ * NULL or has n_modes < 1, NULL shard with n != n_local, a required output NULL -> GMM_ERR_ARG; K != the K of the current
+ * parameters, a call between gmm_mstep and gmm_constants, no component with pi > 0, or an S_k that is not positive
+ * definite (the first such component is named in the message) -> GMM_ERR_STATE.
+ * Device memory: the component records (DP + DP^2 + 4 floats each, DP = D rounded up to a multiple of 4), the mode list,
+ * per point of a chunk DP + 4 floats of state, and per slot of two (12 + 4 D) bytes of outputs with a pinned mirror;
+ * reserved on first use, grown with the chunk, freed by gmm_destroy.                                                  */
+int  gmm_modes(gmm_ctx*, int K, int max_iter, double tol /* <0: 1e-5 */, double merge_tol /* <0: 1e-2 */,
+               int* n_modes_out, double* modes_out /* [K][D] */, double* mode_logp_out /* [K] */,
+               int* comp_mode_out /* [K] */, int* is_max_out /* [K] */, int* iters_out /* [K] */);
+int  gmm_mode_labels(gmm_ctx*, int K, const float* events_aos, long long n,
+                     const double* modes /* [n_modes][D] */, int n_modes,
+                     int max_iter, double tol, double merge_tol,
+                     int* labels, float* endpoints /* [n][D] or NULL */, float* logp_end /* [n] or NULL */,
+                     int* iters /* [n] or NULL */, long long* unmatched_out, long long* unconverged_out);
+
+/* Since the last reset: out[0] kernel ms (gmm_modes and gmm_mode_labels), out[1] wall ms in gmm_modes, out[2] wall ms in
+ * gmm_mode_labels, out[3] event-iterations run.                                                                          */
+int  gmm_get_modes_profile(gmm_ctx*, double out[4], int reset);
+
 /* Per-phase device/host time accumulated since the last reset, in ms
  * (replaces profile_t, gaussian.cu:76-106,967).
  * out[0]=estep out[1]=mstep out[2]=constants(host) out[3]=allreduce
